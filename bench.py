@@ -1,17 +1,21 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the B200-native OSS operator stack.
+"""bench.py -- headline benchmark of the H100-native OSS operator stack.
 
 Metric (BASELINE.json): SRx4 images/sec on synthetic B x 3 x 64 x 64 LQ tiles, bf16.
-Default workload (N=1): BASELINE configs[1] -- "VmambaIR-light SRx4 inference, B=8 3x64x64 LQ, bf16, 1xB200"
+Default workload (N=1): BASELINE configs[1] -- "VmambaIR-light SRx4 inference, B=8 3x64x64 LQ, bf16, 1xH100"
 (VmambaIR-light = the class-default MambaSISR6 [6,2,2,1]+6, SURVEY.md 8d); `--workload train` runs configs[2]
 (full SR net training step, 4 img/GPU, gradient all-reduce over NCCL).  Images shard on the batch axis: every
 rank processes its own batch (weak scaling), inference has no collective.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload infer|train]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload infer|train] [--dump-outputs DIR]
   torchrun --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 ... bench.py --gpus N ...
 
 One JSON line on rank 0.  `--impl reference` times the CPU oracle port of the reference path (oracle/),
-rank 0 only, one image per step.
+rank 0 only, one image per step.  `--dump-outputs DIR` (rank 0) writes what the timed paths computed in their last timed
+step as DIR/<name>.npy (float32, at most 64 MB in all): the SR batch of the inference engine (sr.npy; with `--impl reference`
+the oracle's SR image of image 0) and, for the training step, its loss (train_loss.npy) and a seeded sample of the updated
+parameters (train_params_sample.npy).  Inputs and weights are seeded,
+so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -41,7 +45,35 @@ def peaks():
         p = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3, not a measurement)"
+
+
+def gpu_info(index):
+    """name and power limit of the card the numbers were taken on"""
+    info = {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", str(index)],
+                           capture_output=True, text=True, timeout=30)
+        info["power_limit_w"] = float(r.stdout.strip().splitlines()[0])
+    except Exception:
+        pass
+    return info
+
+
+_dumped_bytes = 0  # written to the --dump-outputs directory by this process
+
+
+def dump_outputs(dirname, arrays):
+    """DIR/<name>.npy (float32) for each array; at most 64 MB over all calls of one run"""
+    global _dumped_bytes
+    import numpy as np
+    os.makedirs(dirname, exist_ok=True)
+    total = _dumped_bytes + sum(a.numel() * 4 for a in arrays.values())
+    if total > 64 << 20:
+        raise SystemExit(f"bench.py: --dump-outputs would write {total} bytes in all (> 64 MB)")
+    _dumped_bytes = total
+    for name, a in arrays.items():
+        np.save(os.path.join(dirname, f"{name}.npy"), a.detach().float().cpu().numpy())
 
 
 class ClockSampler:
@@ -154,7 +186,9 @@ def run_reference(args):
     if rank != 0:
         return
     cores = os.cpu_count()
-    ips, mean, _ = cpu_oracle_images_per_s(args.steps, args.warmup, kind=args.net)
+    ips, mean, y = cpu_oracle_images_per_s(args.steps, args.warmup, kind=args.net)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"sr": y})  # the last timed forward: image 0 of the bench batch
     out = {
         "impl": "reference", "metric": METRIC, "value": round(ips, 4), "unit": "images/s",
         "n_gpus": args.gpus, "steps": args.steps, "warmup": args.warmup, "ms_per_step": round(mean * 1e3, 2),
@@ -217,10 +251,12 @@ def run_infer(args):
         for s, e in evs:
             flush.zero_()
             s.record(eng.stream)
-            eng.step_device()
+            y_last = eng.step_device()
             e.record(eng.stream)
     torch.cuda.synchronize(dev)
     barrier(world)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"sr": y_last})
     step_ms = [s.elapsed_time(e) for s, e in evs]
     total_ms = dist_max(sum(step_ms), world, dev)
     # ---- end-to-end through the public API: pinned host -> device -> net -> host, every step ----
@@ -274,12 +310,12 @@ def run_infer(args):
         "roofline": {"kernel": f"scan_fwd_tma_kernel (largest scan of the step, {top_b / 1e6:.1f} MB of operands; config 2: u (8,384,4096) bf16)", "bound": "hbm",
                      "achieved": round(ach, 1), "peak": peak, "peak_source": peak_src, "unit": "GB/s",
                      "frac": round(ach / peak, 4),
-                     # dram__bytes_* of this launch are not measurable outside ncu: null here, the committed capture is cited
-                     "traffic": None, "traffic_cited": "profiles/ncu_scan_fwd_r2.txt (ncu --set full of this kernel inside this command)",
+                     # dram__bytes_* of this launch are not measurable with CUDA events: null here
+                     "traffic": None,
                      "algorithmic_bytes_per_launch": int(top_b),
                      "all_scans_per_step": {"launches": len(big) // 3, "GB": round(tot_b / 3 / 1e9, 4),
-                                            "ms": round(tot_ms / 3, 4), "share_of_step": round(tot_ms / 3 / ms_per_step, 3)},
-                     "note": "not HBM-bound at bf16 I/O: the MUFU (ex2), LDS and SHFL instructions of a warp queue on one path (tools/microbench.cu, profiles/scan_fwd_r2.md)"},
+                                            "ms": round(tot_ms / 3, 4), "share_of_step": round(tot_ms / 3 / ms_per_step, 3)}},
+        "gpu": gpu_info(local),
         "clocks": clocks,
     }
     if rank == 0:
@@ -305,8 +341,10 @@ def train_record(args):
     driver's 1 -> 8 GPU sweep carries a training-scaling curve next to the collective-free inference one."""
     from vmambair_b200.train_bench import run_train
     a = argparse.Namespace(**vars(args))
-    a.steps, a.warmup = min(args.steps, 10), 3
-    t = run_train(a, build_net, ClockSampler, env_rank, dist_max, barrier, peaks, sample_clocks=False)
+    a.warmup = 3
+    t, outputs = run_train(a, build_net, ClockSampler, env_rank, dist_max, barrier, peaks, sample_clocks=False)
+    if args.dump_outputs and env_rank()[0] == 0:
+        dump_outputs(args.dump_outputs, outputs)
     keep = ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "scaling", "dtype", "config", "e2e", "gpu_launches",
             "collective", "loss_last", "roofline")
     return {k: t[k] for k in keep}
@@ -323,11 +361,15 @@ def main():
                     help="inference net: light = class-default MambaSISR6 [6,2,2,1]+6 (BASELINE configs[1]); full = the YAML's "
                          "[15,1,1,1]+15 (SURVEY.md 8d asks for both)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step of each timed path as DIR/<name>.npy (float32)")
     ap.add_argument("--no-train", action="store_true", help="skip the training-step sub-record of the default run")
     ap.add_argument("--config", type=int, default=2, choices=[2, 4, 5],
                     help="1-based index into BASELINE.json configs: 2 = VmambaIR-light SRx4 inference (default, the metric's config), "
                          "4 = deraining 4 x 3x256x256, 5 = RealSR 2 x 3x128x128 per GPU")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
     if args.impl == "reference":
         return run_reference(args)
     if not torch.cuda.is_available():
@@ -339,7 +381,9 @@ def main():
     try:
         if args.workload == "train":
             from vmambair_b200.train_bench import run_train
-            out = run_train(args, build_net, ClockSampler, env_rank, dist_max, barrier, peaks)
+            out, outputs = run_train(args, build_net, ClockSampler, env_rank, dist_max, barrier, peaks)
+            if args.dump_outputs and rank == 0:
+                dump_outputs(args.dump_outputs, outputs)
         else:
             out = run_infer(args)
             if not args.no_train and args.config == 2:

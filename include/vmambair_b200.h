@@ -1,4 +1,4 @@
-/* vmambair_b200 -- C ABI of the B200-native Omni-Selective-Scan operator stack.
+/* vmambair_b200 -- C ABI of the H100-native Omni-Selective-Scan operator stack.
  *
  * Plain C: raw device pointers, explicit sizes/strides (in ELEMENTS), a dtype
  * enum and a cudaStream_t (passed as void*).  The caller owns every buffer;
@@ -26,7 +26,7 @@ extern "C" {
 typedef enum { VMB_F32 = 0, VMB_BF16 = 1, VMB_F16 = 2 } vmb_dtype;
 
 const char* vmb_last_error(void);
-/* library / build identification: "vmambair_b200 <ver> sm_100a" */
+/* library / build identification: "vmambair_b200 <ver> sm_90a" */
 const char* vmb_version(void);
 
 /* Checkpoint interval (in sequence positions) of the opaque `ckpt` buffer shared by

@@ -1,15 +1,18 @@
 #!/usr/bin/env python
-"""Rebuild the reference's own CUDA extension (selective_scan_cuda_core) for sm_100a into oracle/_ref/.
-TEST / BASELINE INFRASTRUCTURE ONLY -- the "kernel to beat" on the GPU box.
+"""Rebuild the reference's own CUDA extension (selective_scan_cuda_core) for sm_90a into oracle/_ref/.
+TEST / BASELINE INFRASTRUCTURE ONLY -- the "kernel to beat", and the source of tests/golden/scan_ref_kernel.npz.
 
-Sources are compiled where they lie under /root/reference (nothing is copied):
+Sources are compiled where they lie in a checkout of the reference project next to this repository (../reference, or
+$VMB_REFERENCE_DIR; nothing is copied):
   Mamba/kernels/selective_scan/csrc/selective_scan/cus/{selective_scan.cpp, selective_scan_core_fwd.cu, selective_scan_core_bwd.cu}
-with the reference's own nvcc flags (setup.py:115-131) except the -gencode list (setup.py:62-65 -> compute_100a/sm_100a).
+with the reference's own nvcc flags (setup.py:115-131) except the -gencode list (setup.py:62-65 -> compute_90a/sm_90a).
 """
 import os
 import sys
 
-REF = "/root/reference/Mamba/kernels/selective_scan/csrc/selective_scan"
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+REF_DIR = os.environ.get("VMB_REFERENCE_DIR") or os.path.join(os.path.dirname(ROOT), "reference")
+REF = os.path.join(REF_DIR, "Mamba", "kernels", "selective_scan", "csrc", "selective_scan")
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "_ref")
 
 
@@ -23,7 +26,7 @@ def main():
         return
     os.makedirs(OUT, exist_ok=True)
     from torch.utils.cpp_extension import load
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0a")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0a")
     os.environ.setdefault("MAX_JOBS", "4")
     load(name="selective_scan_cuda_core",
          sources=[f"{REF}/cus/selective_scan.cpp", f"{REF}/cus/selective_scan_core_fwd.cu", f"{REF}/cus/selective_scan_core_bwd.cu"],
@@ -33,9 +36,9 @@ def main():
                             "-U__CUDA_NO_BFLOAT16_OPERATORS__", "-U__CUDA_NO_BFLOAT16_CONVERSIONS__",
                             "-U__CUDA_NO_BFLOAT162_OPERATORS__", "-U__CUDA_NO_BFLOAT162_CONVERSIONS__",
                             "--expt-relaxed-constexpr", "--expt-extended-lambda", "--use_fast_math",
-                            "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo"],
+                            "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo"],
          build_directory=OUT, verbose=False, is_python_module=False)
-    for f in os.listdir(OUT):  # keep only the .so (it travels to the GPU box)
+    for f in os.listdir(OUT):  # keep only the .so
         if not f.endswith(".so"):
             os.remove(os.path.join(OUT, f))
     print("built", so)

@@ -40,7 +40,8 @@ def set_threads(n: int):
 
 def host_threads() -> int:
     """CPU threads for the oracle: PHYSICAL cores inside this process's scheduler affinity mask (cpusets / taskset), capped by the
-    cgroup CPU quota -- on a GPU box with 128 SMT threads and a 16-CPU quota, 128 OpenMP threads run the oracle ~100x slower."""
+    cgroup CPU quota -- on a GPU host with many SMT threads and a small CPU quota, one OpenMP thread per logical CPU runs the oracle
+    ~100x slower."""
     import os
     try:
         aff = os.sched_getaffinity(0)

@@ -11,7 +11,7 @@ Only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s CPU-baseline /
 (``vmambair_b200``) never does.
 
 Parity pinning: ``tests/golden/make_golden.py`` runs the *real* reference
-function (AST-extracted from /root/reference, not copied) on seeded inputs and
+function (AST-extracted from the reference project, not copied) on seeded inputs and
 commits its outputs under ``tests/golden/``; ``tests/test_oracle.py`` checks
 this restatement against those vectors.
 

@@ -11,9 +11,9 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box via gpurun)")
-    # the CPU oracle (torch convs + OpenMP C scan) on the physical cores inside the cgroup quota: all SMT threads of a GPU box
-    # with a small CPU quota make it ~100x slower (the round-2 parity tests took 18 min that way)
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
+    # the CPU oracle (torch convs + OpenMP C scan) on the physical cores inside the cgroup quota: all SMT threads of a GPU host
+    # with a small CPU quota make it ~100x slower
     import torch
     from oracle import cscan
     torch.set_num_threads(cscan.host_threads())
@@ -32,3 +32,15 @@ def pytest_collection_modifyitems(config, items):
 @pytest.fixture(scope="session")
 def golden_dir():
     return GOLDEN
+
+
+@pytest.fixture(scope="session")
+def net_sisr_tiny():
+    """input "x", output "y" and state_dict "sd/<key>" of the tiny reference SR net (tests/golden/make_golden.py gen_net),
+    stored in two files so that neither exceeds 1 MB"""
+    import numpy as np
+    z = {}
+    for name in ("net_sisr_tiny.npz", "net_sisr_tiny_up4_3.npz"):
+        with np.load(os.path.join(GOLDEN, name)) as f:
+            z.update({k: f[k] for k in f.files})
+    return z

@@ -1,11 +1,12 @@
 #!/usr/bin/env python
-"""Generate golden fixtures from the REAL reference (run in the build container only).
+"""Generate golden fixtures from the REAL reference (a checkout of the reference project next to this repository,
+../reference, or $VMB_REFERENCE_DIR).
 
-Nothing here is copied from /root/reference: the reference functions are
+Nothing here is copied from the reference: its functions are
 AST-extracted / imported at run time, executed on seeded inputs, and only
 their numeric inputs/outputs are written to tests/golden/*.npz|json.
 
-  python tests/golden/make_golden.py            # needs /root/reference
+  python tests/golden/make_golden.py            # needs the reference checkout
 
 Sources exercised:
   * selective_scan_ref         Mamba/kernels/selective_scan/test_selective_scan.py:168-234
@@ -28,8 +29,8 @@ import torch
 import torch.nn.functional as F
 from einops import rearrange, repeat
 
-REF = "/root/reference"
 OUT = os.path.dirname(os.path.abspath(__file__))
+REF = os.environ.get("VMB_REFERENCE_DIR") or os.path.join(os.path.dirname(os.path.dirname(os.path.dirname(OUT))), "reference")
 
 
 def load_ref_scan():
@@ -174,7 +175,7 @@ def gen_block(tag, mod, dim, H, W, with_grad):
     rec["y"] = y.detach().numpy()
     for k, v in np_state(blk.state_dict()).items():
         rec[f"sd/{k}"] = v
-    np.savez(f"{OUT}/block_{tag}.npz", **rec)
+    np.savez_compressed(f"{OUT}/block_{tag}.npz", **rec)
     print(f"block_{tag}.npz", sum(v.nbytes for v in rec.values()) // 1024, "KiB")
 
 
@@ -187,7 +188,10 @@ def gen_net(sisr):
     rec = {"x": x.numpy(), "y": y.numpy()}
     for k, v in np_state(net.state_dict()).items():
         rec[f"sd/{k}"] = v.astype(np.float32)
-    np.savez(f"{OUT}/net_sisr_tiny.npz", **rec)
+    # two compressed files, neither above 1 MB (tests/conftest.py::net_sisr_tiny merges them)
+    big = "sd/up4_3.body.0.weight"
+    np.savez_compressed(f"{OUT}/net_sisr_tiny.npz", **{k: v for k, v in rec.items() if k != big})
+    np.savez_compressed(f"{OUT}/net_sisr_tiny_up4_3.npz", **{big: rec[big]})
     print("net_sisr_tiny.npz", sum(v.nbytes for v in rec.values()) // 1024, "KiB")
 
 

@@ -76,10 +76,10 @@ def test_block_backward_matches_reference_golden(golden_dir, oracle_scan):
         assert (p.grad - ref).abs().max() <= 2e-3 * scale + 1e-5, n
 
 
-def test_tiny_net_matches_reference_golden(golden_dir, oracle_scan):
-    z = np.load(os.path.join(golden_dir, "net_sisr_tiny.npz"))
+def test_tiny_net_matches_reference_golden(net_sisr_tiny, oracle_scan):
+    z = net_sisr_tiny
     net = archs.MambaSISR6(dim=8, num_blocks=[1, 1, 1, 1], num_refinement_blocks=1).eval()
-    net.load_state_dict({k[3:]: torch.from_numpy(z[k]) for k in z.files if k.startswith("sd/")}, strict=True)
+    net.load_state_dict({k[3:]: torch.from_numpy(z[k]) for k in z if k.startswith("sd/")}, strict=True)
     with torch.no_grad():
         y = net(torch.from_numpy(z["x"]))
     torch.testing.assert_close(y, torch.from_numpy(z["y"]), rtol=1e-4, atol=1e-5)

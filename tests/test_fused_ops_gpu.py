@@ -257,7 +257,8 @@ def test_grouped_direction_aware_scan_equals_gathered_scan(dtype, C, H, W):
 @pytest.mark.parametrize("K,M,P,B", [(96, 192, 4096, 2), (48, 96, 256, 3), (96, 510, 1024, 2), (256, 96, 512, 1), (288, 768, 64, 4), (384, 96, 64, 2),
                                      (255, 96, 1024, 2), (127, 48, 512, 2), (48, 254, 1024, 1), (96, 510, 4096, 8)])
 def test_pixlin_tcgen05_path(dtype, K, M, P, B, monkeypatch):
-    """the tcgen05/TMEM kernel (forced on for every legal shape) against fp32 torch: plain, LN+SiLU range, gate+residual."""
+    """the persistent tensor-core kernel of pixlin_tc.cu (wgmma; the test keeps its original id), forced on for every legal
+    shape, against fp32 torch: plain, LN+SiLU range, gate+residual."""
     from vmambair_b200 import ops
     monkeypatch.setenv("VMB_PIXLIN_TC", "2")
     torch.manual_seed(K + M + P)

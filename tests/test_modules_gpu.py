@@ -56,10 +56,10 @@ def test_block_backward_golden(golden_dir, tag, variant, dim):
         assert err <= 3e-3 * r.abs().max().clamp_min(1e-6) + 1e-5, (n, float(err), float(r.abs().max()))
 
 
-def test_tiny_net_golden(golden_dir):
-    z = np.load(os.path.join(golden_dir, "net_sisr_tiny.npz"))
+def test_tiny_net_golden(net_sisr_tiny):
+    z = net_sisr_tiny
     net = archs.MambaSISR6(dim=8, num_blocks=[1, 1, 1, 1], num_refinement_blocks=1).eval()
-    net.load_state_dict({k[3:]: torch.from_numpy(z[k]) for k in z.files if k.startswith("sd/")}, strict=True)
+    net.load_state_dict({k[3:]: torch.from_numpy(z[k]) for k in z if k.startswith("sd/")}, strict=True)
     net = net.cuda()
     with torch.no_grad():
         y = net(torch.from_numpy(z["x"]).cuda())

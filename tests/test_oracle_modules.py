@@ -1,5 +1,5 @@
 """Pins the module-level CPU oracle (oracle/oss_ref.py) against outputs of the REAL reference modules
-(fixtures written by tests/golden/make_golden.py from /root/reference)."""
+(fixtures written by tests/golden/make_golden.py from the reference project)."""
 import os
 
 import numpy as np
@@ -10,7 +10,7 @@ from oracle import oss_ref
 
 
 def _sd(z):
-    return {k[3:]: torch.from_numpy(z[k]) for k in z.files if k.startswith("sd/")}
+    return {k[3:]: torch.from_numpy(z[k]) for k in z if k.startswith("sd/")}
 
 
 @pytest.mark.parametrize("tag,gate", [("sisr_c48", "mul"), ("m32_c32", "add"), ("m33_c32", "mul"), ("realsr_c32", "mul")])
@@ -25,8 +25,8 @@ def test_block_oracle_matches_reference(golden_dir, tag, gate):
     torch.testing.assert_close(y, torch.from_numpy(z["y"]), rtol=1e-4, atol=2e-5)
 
 
-def test_net_oracle_matches_reference(golden_dir):
-    z = np.load(os.path.join(golden_dir, "net_sisr_tiny.npz"))
+def test_net_oracle_matches_reference(net_sisr_tiny):
+    z = net_sisr_tiny
     y = oss_ref.net_forward(_sd(z), torch.from_numpy(z["x"]), "sisr")
     torch.testing.assert_close(y, torch.from_numpy(z["y"]), rtol=1e-4, atol=2e-5)
 

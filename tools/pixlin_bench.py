@@ -1,5 +1,5 @@
 """Per-shape sustained timing of the 1x1-conv GEMM (vmb_pixlin) on the shapes of the light SISR net at B=8, 64x64:
-mma.sync kernel (VMB_PIXLIN_TC=0) against the tcgen05/TMEM kernel (VMB_PIXLIN_TC=2).  Four rotating buffer sets
+mma.sync kernel (VMB_PIXLIN_TC=0) against the wgmma kernel (VMB_PIXLIN_TC=2).  Four rotating buffer sets
 (> L2 together for the big shapes), 10 launches per CUDA graph, 20 replays."""
 import sys, os, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

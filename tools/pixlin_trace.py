@@ -1,4 +1,4 @@
-"""Timeline of one persistent tcgen05 pixlin launch (VMB_TC_TRACE=1): per-CTA %globaltimer stamps."""
+"""Timeline of one persistent wgmma pixlin launch (VMB_TC_TRACE=1): per-CTA %globaltimer stamps."""
 import sys, os, ctypes
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 os.environ["VMB_PIXLIN_TC"] = "2"
@@ -20,13 +20,13 @@ for name, (K, M, kind) in {"w_big96": (96, 256, "plain"), "pin96": (96, 510, "ln
     call(); torch.cuda.synchronize()
     buf = (ctypes.c_longlong * (160 * 64))()
     assert _lib.lib().vmb_debug_tc_trace(buf, 160 * 64) == 0
-    t = [[buf[c * 64 + i] for i in range(64)] for c in range(148)]
+    ctas = min(160, torch.cuda.get_device_properties(0).multi_processor_count)  # one CTA per SM, <= 160 traced
+    t = [[buf[c * 64 + i] for i in range(64)] for c in range(ctas)]
     t0 = min(r[0] for r in t)
     print(name, "kernel span us:", (max(r[3] for r in t) - t0) / 1e3)
     for c in (0, 73):
         r = t[c]
         print("  cta", c, "start+%.2f setup %.2f weights %.2f end %.2f" % ((r[0] - t0) / 1e3, (r[1] - r[0]) / 1e3, (r[2] - r[1]) / 1e3, (r[3] - t0) / 1e3))
-        if r[58]: print("     prologue tile 2: loads+stats %.2f  normalise %.2f  fence %.2f" % ((r[59] - r[58]) / 1e3, (r[60] - r[59]) / 1e3, (r[61] - r[60]) / 1e3))
         print("     tile: landed  pro_done  mma_saw  mma_issued  epi_saw  epi_done   (us after weights resident)")
         for i in range(8):
             e = r[4 + 6 * i: 10 + 6 * i]

@@ -30,7 +30,7 @@ def main():
     ap.add_argument("--L", type=int, nargs="+", default=[4096])
     ap.add_argument("--dtypes", nargs="+", default=["bf16", "fp32"])
     ap.add_argument("--bwd", action="store_true")
-    ap.add_argument("--ref", action="store_true", help="also time the reference CUDA kernel rebuilt for sm_100a (oracle/_ref)")
+    ap.add_argument("--ref", action="store_true", help="also time the reference CUDA kernel rebuilt for sm_90a (oracle/_ref)")
     a = ap.parse_args()
     dev = "cuda"
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)

@@ -1,7 +1,7 @@
 """Drop-in OSS modules and networks (same class names, ctor kwargs, forward() signatures and
-state_dict keys/shapes as the reference archs), running on the sm_100a kernels of this repo.
+state_dict keys/shapes as the reference archs), running on the sm_90a kernels of this repo.
 
-Reference classes mirrored (file:line in /root/reference):
+Reference classes mirrored (file:line in the reference project):
   LayerNorm / WithBias_LayerNorm / BiasFree_LayerNorm   SRGAN/VmambaIR/archs/MambaSISR6_arch.py:149-195
   FeedForward (EFFN)                                     MambaSISR6_arch.py:201-218
   SS2D_1 (OSS module)                                    MambaSISR6_arch.py:222-498 (SISR)

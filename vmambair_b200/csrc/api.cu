@@ -15,6 +15,15 @@ bool pdl_enabled() {
     }();
     return on;
 }
+int num_sms() {
+    static const int n = [] {
+        int dev = 0, v = 0;
+        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0)
+            v = 132;  // H100 SXM
+        return v;
+    }();
+    return n;
+}
 static thread_local char g_err[512] = "";
 void set_error(const char* fmt, ...) {
     va_list ap;
@@ -29,7 +38,7 @@ static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t
 using namespace vmb;
 
 extern "C" const char* vmb_last_error(void) { return g_err; }
-extern "C" const char* vmb_version(void) { return "vmambair_b200 0.1 sm_100a"; }
+extern "C" const char* vmb_version(void) { return "vmambair_b200 0.1 sm_90a"; }
 extern "C" int vmb_scan_ckpt_interval(void) { return kScanCkpt; }
 
 extern "C" int vmb_selective_scan_fwd(const vmb_scan_fwd_args* a, void* stream) {

@@ -1,4 +1,4 @@
-// Shared device helpers for the vmambair_b200 kernels (sm_100a only).
+// Shared device helpers for the vmambair_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -38,6 +38,7 @@ void set_error(const char* fmt, ...);
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 bool pdl_enabled();  // VMB_PDL (default 1), read once
+int num_sms();       // SMs of the current device, read once (launch heuristics size their grids by it)
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
     cudaLaunchConfig_t cfg = {};
@@ -92,9 +93,10 @@ __device__ __forceinline__ float softplus_f(float x) {
 }
 __device__ __forceinline__ float sigmoid_f(float x) { return rcp_approx(1.f + ex2(-x * kLog2e)); }
 
-__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return __ffma2_rn(a, b, c); }
-__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return __fmul2_rn(a, b); }
-__device__ __forceinline__ float2 add2(float2 a, float2 b) { return __fadd2_rn(a, b); }
+// two-lane helpers: sm_90 has no packed f32x2 FMA, so each lane is one round-to-nearest FFMA / FMUL / FADD
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 
 __device__ __forceinline__ float2 shfl_up2(float2 v, int delta) {
     return make_float2(__shfl_up_sync(0xffffffffu, v.x, delta), __shfl_up_sync(0xffffffffu, v.y, delta));

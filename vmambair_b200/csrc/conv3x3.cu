@@ -525,14 +525,14 @@ int launch_tma(const Conv3Params& p, int dtype, cudaStream_t stream) {
     auto kern = conv3x3_tma_kernel<T, MT, STAGES, NHWC>;
     VMB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));  // per device: set at every launch
     // pixel tiles of the whole batch on grid.x, one CTA per tile.  The kernel can also walk several tiles per CTA (grid.x < ntile:
-    // one stream of (tile, chunk) iterations through the stage ring) -- measured on the 16 384-tile conv_last: 90.3 us persistent
-    // (740 CTAs) vs 81.3 us with a CTA per tile, so it stays off (VMB_CONV_PERSIST=1 turns it on for problems beyond 3 resident waves)
+    // one stream of (tile, chunk) iterations through the stage ring) -- it stays off by default (VMB_CONV_PERSIST=1 turns it on for
+    // problems beyond 3 resident waves)
     const int ntile = cdiv(p.W, kTW) * cdiv(p.H, kTH) * p.B, mt = cdiv(p.Cout, MT);
     int gx = ntile;
     static const bool persist = [] { const char* e = getenv("VMB_CONV_PERSIST"); return e && atoi(e) == 1; }();
     if (persist) {
         const int per_sm = (227 * 1024) / SMEM > 0 ? (227 * 1024) / SMEM : 1;
-        int cap = 148 * (per_sm > 8 ? 8 : per_sm) / mt;
+        int cap = num_sms() * (per_sm > 8 ? 8 : per_sm) / mt;
         if (cap < 1) cap = 1;
         if (ntile > 3 * cap) gx = cap;
     }
@@ -552,7 +552,7 @@ int launch_16(const Conv3Params& p, int dtype, cudaStream_t stream) {
     if (!aligned) return p.Cout <= 16 ? launch_generic<T, 16>(p, stream) : launch_generic<T, 64>(p, stream);
     // output-channel tile: the widest one that still fills one wave of CTAs (every K chunk costs a CTA a fixed barrier / re-layout
     // overhead that a wider tile amortises, but an idle SM amortises nothing)
-    const int want = 148;
+    const int want = num_sms();
     if (p.Cout > 32 && tiles * cdiv(p.Cout, 64) >= want) return launch_tma<T, 64, 3, false>(p, dtype, stream);
     if (p.Cout > 16 && tiles * cdiv(p.Cout, 32) >= want) return launch_tma<T, 32, 3, false>(p, dtype, stream);
     return launch_tma<T, 16, 4, false>(p, dtype, stream);

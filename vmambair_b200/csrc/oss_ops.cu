@@ -182,9 +182,8 @@ __global__ void __launch_bounds__(256) dwconv3x3_rows4_kernel(const DwParams p, 
 }
 
 // The same row block with the loads split from the arithmetic: all six 16 B row vectors (twelve in the gated mode: both channel sets)
-// are requested before the first use, so one thread has 6-12 loads in flight instead of one row at a time -- ncu of the interleaved
-// version: 10 % of DRAM throughput, 4.0 long-scoreboard stall cycles per issue at 16 warps per SM (profiles/ncu_dwconv_r2.txt).
-// Identical fmaf order: bit-identical results.
+// are requested before the first use, so one thread has 6-12 loads in flight instead of one row at a time (the interleaved version
+// stalls on each row load in turn).  Identical fmaf order: bit-identical results.
 template <typename in_t>
 __device__ __forceinline__ void dw_rows4_load(const in_t* __restrict__ xc, int h0, int w0, int H, int W,
                                               uint4 (&raw)[6][8 / Vec<in_t>::N]) {
@@ -471,7 +470,7 @@ __global__ void __launch_bounds__(256) cross_scan_vec_kernel(const CrossScanPara
 }
 
 // Up to four cross-scans of one geometry in ONE launch (the training path gathers x, delta and B|C of a block into the four scan
-// orders, and scatters du, ddelta, dB, dC back: 3 + 4 launches of 5-13 us each for a few MB -- launch / latency bound): blockIdx.y
+// orders, and scatters du, ddelta, dB, dC back: 3 + 4 launches for a few MB -- launch / latency bound): blockIdx.y
 // walks the rows of all segments.
 template <typename in_t>
 __global__ void __launch_bounds__(256) cross_scan_vec_multi_kernel(const CrossScanMulti m) {
@@ -659,7 +658,7 @@ int pixel_shuffle_launch(const PixelShuffleParams& p, int dtype, cudaStream_t st
     VMB_CHECK((4 * p.C) % v == 0, "pixel_shuffle: 4*C must be a multiple of %d", v);
     const int64_t total = (int64_t)p.B * p.H * p.W * (4 * p.C / v);
     int64_t blocks = (total + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > num_sms() * 16) blocks = num_sms() * 16;
     dim3 grid((unsigned)blocks);
     switch (dtype) {
         case VMB_F32: VMB_CUDA(launch_pdl(pixel_shuffle2_nhwc_kernel<float>, grid, dim3(256), 0, stream, p)); break;
@@ -963,16 +962,16 @@ __global__ void __launch_bounds__(512) merge_fused_kernel(const MergeParams p, f
 
 // the workspace regions of the fused kernel sit behind the fp32 merged values and the statistics
 static bool merge_fused_applicable(const MergeParams& p, int dtype) {
-    int mode = 2;  // VMB_MERGE_FUSED: 0 never, 1 whenever legal (tests), default: where it was measured faster
+    int mode = 2;  // VMB_MERGE_FUSED: 0 never, 1 whenever legal (tests), default: from 128 x 128 pixels per image up
     if (const char* e = getenv("VMB_MERGE_FUSED")) mode = atoi(e);
     if (mode == 0) return false;
     auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
     const bool legal = (dtype == VMB_BF16 || dtype == VMB_F16) && p.H % 16 == 0 && p.W % 16 == 0 && p.C <= 16 * MF_MAXPW &&
                        merge_fused_smem(p.C) <= 200 * 1024 && al16(p.ys) && al16(p.z) && al16(p.y2) && p.z_bs % 8 == 0 && p.z_cs % 8 == 0;
     if (!legal || mode == 1) return legal;
-    // tools/merge_bench.py (bf16, sustained): 2 x 96 x 128x128: 24.6 vs 47.7 us (the normalisation kernel of the two-kernel path walks
-    // all pixels of a channel in one CTA); 8 x 96 x 64x64: 24.6 vs 24.9, 8 x 96 x 32x32: 22 vs 8.4 -- a CTA of the single kernel
-    // needs ~20 us for its 24 channel groups at any size, so it pays from 128 x 128 pixels per image up
+    // the normalisation kernel of the two-kernel path walks all pixels of a channel in one CTA, which dominates at large images; a
+    // CTA of the single kernel walks all channel groups of its tile at any size, which dominates at small ones (tools/merge_bench.py
+    // times both)
     return (long)p.H * p.W >= 16384;
 }
 

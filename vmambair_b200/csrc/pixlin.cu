@@ -539,7 +539,7 @@ static int launch2(K kern, PixlinParams p, int PT, cudaStream_t stream) {
     // split the output channels over blockIdx.y (a) until the grid covers the SMs ~1.5x and (b), when K is resident,
     // until all weight tiles of a CTA fit in <= 64 KB of smem: then they are fetched in one batch (no per-tile wait)
     int msplit = 1;
-    while (msplit < mtiles && (long)ptiles * p.B * msplit < 148L * 3 / 2) ++msplit;
+    while (msplit < mtiles && (long)ptiles * p.B * msplit < 3L * num_sms() / 2) ++msplit;
     p.w_all = false;
     int wtiles = 2;
     if (kpad <= PL2_KC && p.w_vec) {
@@ -565,7 +565,7 @@ static int launch2(K kern, PixlinParams p, int PT, cudaStream_t stream) {
 template <typename in_t>
 static int launch_mma(const PixlinParams& p, int out_dtype, cudaStream_t stream) {
     // 128-pixel tiles when there are enough pixels to fill the GPU with them, else 64
-    bool big = (long)((p.P + 127) / 128) * p.B >= 148 && pixlin_smem(p.K, 2, 128, 2) <= 100 * 1024;
+    bool big = (long)((p.P + 127) / 128) * p.B >= num_sms() && pixlin_smem(p.K, 2, 128, 2) <= 100 * 1024;
     if (const char* e = getenv("VMB_PL_PT")) big = big && atoi(e) == 128;  // tuning override
     const int PT = big ? 128 : 64;
     if (out_dtype == VMB_F32)
@@ -579,7 +579,7 @@ static int launch_mma(const PixlinParams& p, int out_dtype, cudaStream_t stream)
 // ---- K-streamed variant: reduction-heavy plain GEMMs (K > 384, no prologue) ---------------------------------------------------
 // The data gradients W^T dY of the EFFN (2h = 510 -> C = 96) and of the folded x_proj / dt_proj (4(C + 2N) = 512 -> 96) in the
 // training path: the input (K x P) is the big operand, the output small.  The resident-K kernel above re-stages its activation tile
-// per output-channel tile and K chunk without overlap (29.6 us at B = 4, 64x64); here a CTA owns 128 output channels x 64 pixels
+// per output-channel tile and K chunk without overlap; here a CTA owns 128 output channels x 64 pixels
 // and walks K in 32-row stages through a 4-deep cp.async ring (W stage [128][32], X stage [32][64]), mma.sync m16n8k16,
 // bias / SiLU range / residual straight from the accumulators.
 constexpr int KS_MT = 128, KS_PT = 64, KS_KC = 32, KS_THREADS = 128;
@@ -722,10 +722,10 @@ static bool kstream_applicable(const PixlinParams& p, int dtype, int out_dtype) 
 template <typename K>
 static int launch(K kern, const PixlinParams& p, size_t smem, cudaStream_t stream) {
     if (smem > 48 * 1024) VMB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    // split the output channels over blockIdx.y until the grid covers the 148 SMs a few times
+    // split the output channels over blockIdx.y until the grid covers the SMs a few times
     const int ptiles = (p.P + PL_PT - 1) / PL_PT, mtiles = (p.M + PL_MT - 1) / PL_MT;
     int msplit = 1;
-    while (msplit < mtiles && (long)ptiles * p.B * msplit < 148L * 3) ++msplit;
+    while (msplit < mtiles && (long)ptiles * p.B * msplit < 3L * num_sms()) ++msplit;
     dim3 grid(ptiles, msplit, p.B);
     VMB_CUDA(launch_pdl(kern, grid, dim3(PL_THREADS), smem, stream, p));
     VMB_CUDA(cudaGetLastError());
@@ -736,7 +736,7 @@ int pixlin_launch(const PixlinParams& p, int dtype, int out_dtype, cudaStream_t 
     VMB_CHECK(p.ln_mode == 0 || p.K <= (dtype == VMB_F32 ? PL_KC / 2 : PL2_KC), "pixlin: LayerNorm prologue needs K <= %d",
               dtype == VMB_F32 ? PL_KC / 2 : PL2_KC);
     VMB_CHECK(p.gate_mode == 0 || p.K <= (dtype == VMB_F32 ? PL_KC / 2 : PL2_KC), "pixlin: gate prologue needs resident K");
-    if (pixlin_tc_applicable(p, dtype, out_dtype)) return pixlin_tc_launch(p, dtype, stream);  // tcgen05 / TMEM path
+    if (pixlin_tc_applicable(p, dtype, out_dtype)) return pixlin_tc_launch(p, dtype, stream);  // wgmma path
     if (kstream_applicable(p, dtype, out_dtype))
         return dtype == VMB_BF16 ? launch_kstream<__nv_bfloat16>(p, stream) : launch_kstream<__half>(p, stream);
     const size_t smem = pixlin_smem(p.K, dtype == VMB_F32 ? 4 : 2);

@@ -1,18 +1,19 @@
-// pixlin on the 5th-generation tensor cores: a persistent, warp-specialised tcgen05 / TMEM pipeline.
+// pixlin on the Hopper tensor cores: a persistent, warp-specialised wgmma pipeline.
 //   out[b, m, p] = epi( sum_k W[m,k] * pro(x)[b,k,p] )      (same contract as pixlin.cu)
-// One CTA per SM keeps the whole weight matrix resident in shared memory (K-major canonical UMMA layout) and walks
+// Each CTA (one or two per SM) keeps the whole weight matrix resident in shared memory (K-major canonical GMMA layout) and walks
 // 32-pixel tiles of the (b, p) plane:
-//   warp 4   producer : cp.async of the next activation tiles into a 6-stage ring (MN-major canonical layout: pixels are
-//                       the contiguous dimension of NCHW), 4 tiles in flight, mbarrier "full" per stage
-//   warps 6-9 prologue: LayerNorm / channel gate on the resident tile, in place, one 8-pixel column group per warp
-//                       (only when the call has one)
-//   warp 5   MMA      : one lane issues ceil(M/128) x K/16 tcgen05.mma (128 x 32 x 16) per tile into one of up to four
-//                       TMEM accumulator stages and commits to the "stage empty" / "accumulator full" mbarriers
-//   warps 0-3 epilogue: tcgen05.ld of their 32 TMEM lanes (lane = output channel = one contiguous pixel row),
-//                       bias / SiLU / residual, 32 B vector stores (STG.256)
-// so loads, tensor-core math and stores of different tiles overlap, and the weights are read once per SM instead of
-// once per tile.  Legal for 16-bit I/O with 16 B aligned rows, M <= 512, K <= 256 and weights + ring <= 227 KB; used where
-// measured faster than the mma.sync kernel of pixlin.cu (pixlin_tc_applicable below); FFMA kernel for fp32.
+//   warp 4    producer : cp.async of the next activation tiles into a 6-stage ring (MN-major canonical layout: pixels are
+//                        the contiguous dimension of NCHW), 4 tiles in flight, mbarrier "full" per stage
+//   warps 5-8 prologue : LayerNorm / channel gate on the resident tile, in place, one 8-pixel column group per warp
+//                        (only when the call has one)
+//   warps 0-3 consumer : one warpgroup issues the K/16 wgmma.m64n32k16 of 64 output channels back to back into register
+//                        accumulators, waits for them, then runs the epilogue: quad transpose to 8 contiguous pixels per
+//                        thread and row, bias / SiLU / residual, 16 B vector stores
+// so loads, prologue and tensor-core work of different tiles overlap (and, with two CTAs per SM, the MMAs of one CTA with
+// the epilogue of the other), and the weights are read once per CTA instead of once per tile.  One accumulator set per
+// warpgroup on purpose: with two sets in flight across commit groups ptxas cannot prove the epilogue's reads safe and
+// serialises every wgmma (C7514).  Legal for 16-bit I/O with 16 B aligned rows, M <= 512, K <= 256 and weights + ring <= 227 KB; selected by
+// VMB_PIXLIN_TC only (pixlin_tc_applicable below), the mma.sync kernel of pixlin.cu is the default; FFMA kernel for fp32.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -20,46 +21,56 @@
 
 namespace vmb {
 
-constexpr int TC_PT = 32;        // pixels per tile (UMMA N)
-constexpr int TC_MT = 128;       // output channels per MMA (UMMA M)
+constexpr int TC_PT = 32;        // pixels per tile (GMMA N)
+constexpr int TC_MT = 128;       // rows of one resident weight tile
+constexpr int TC_MB = 64;        // output channels per wgmma (GMMA M)
 constexpr int TC_NS = 6;         // activation ring stages
 constexpr int TC_LA = 4;         // tiles the producer keeps in flight (cp.async groups)
-constexpr int TC_EPI = 128;      // epilogue threads: warp w owns TMEM lanes [32w, 32w+32)
-constexpr int TC_THREADS = 320;  // 4 epilogue warps + producer + MMA + 4 prologue warps
+constexpr int TC_THREADS = 288;  // consumer warpgroup + producer + 4 prologue warps
 constexpr int TC_KGMAX = 32;     // K <= 256: a prologue lane keeps its column of the tile in registers
 constexpr int TC_MAXMT = 4;      // M <= 512
-constexpr int TC_NACC = 4;       // TMEM accumulator stages (nmt*32 columns each)
 constexpr size_t TC_SMEM_MAX = 227 * 1024;
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
 
-// UMMA shared-memory descriptor, SWIZZLE_NONE, version 1 (Blackwell): start address, leading / stride byte offsets in
-// 16 B units.  K-major operand: ((8,m),2):((1,SBO),LBO); MN-major operand: ((1,n),(8,k)):((X,SBO),(1,LBO)).
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+// GMMA shared-memory descriptor, no swizzle (layout type 0): start address, leading / stride byte offsets in 16 B units.
+// K-major operand: ((8,m),(8,2)):((1,SBO),(1,LBO)) in core-matrix rows; MN-major operand: ((8,n),(8,k)):((1,SBO),(1,LBO)).
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr >> 4) & 0x3FFF);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;  // version_ = 1
-    return d;                // base_offset 0, lbo_mode 0, layout_type 0 (SWIZZLE_NONE)
+    return d;  // base_offset 0, layout_type 0 (no swizzle)
 }
-// instruction descriptor, kind::f16: D=f32, A/B = bf16 (1) or f16 (0), A K-major, B MN-major, N>>3, M>>4
-__device__ __forceinline__ uint32_t umma_idesc(int ab_fmt, int M, int N) {
-    return (1u << 4) | ((uint32_t)ab_fmt << 7) | ((uint32_t)ab_fmt << 10) | (0u << 15) | (1u << 16) | ((uint32_t)(N >> 3) << 17) |
-           ((uint32_t)(M >> 4) << 24);
+// D[64 x 32] (+)= A[64 x 16] * B[16 x 32]: A K-major (no transpose), B MN-major (transposed), fp32 accumulators
+template <typename T> __device__ __forceinline__ void wgmma_m64n32k16(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate);
+#define VMB_WGMMA(TY)                                                                                                         \
+    asm volatile(                                                                                                             \
+        "{\n\t"                                                                                                               \
+        ".reg .pred p;\n\t"                                                                                                   \
+        "setp.ne.b32 p, %18, 0;\n\t"                                                                                          \
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32." TY "." TY " "                                                           \
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 1;\n\t"                               \
+        "}\n"                                                                                                                 \
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),        \
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])                           \
+        : "l"(adesc), "l"(bdesc), "r"(accumulate))
+template <> __device__ __forceinline__ void wgmma_m64n32k16<__nv_bfloat16>(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    VMB_WGMMA("bf16");
 }
-__device__ __forceinline__ void tc_mma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
+template <> __device__ __forceinline__ void wgmma_m64n32k16<__half>(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    VMB_WGMMA("f16");
 }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+#undef VMB_WGMMA
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses of accumulator registers across the asynchronous MMAs that write them
+__device__ __forceinline__ void acc_fence(float* d) {
+#pragma unroll
+    for (int i = 0; i < 16; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+
 __device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
 }
@@ -78,23 +89,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
             : "memory");
     } while (!done);
 }
-template <typename T> struct AbFmt;
-template <> struct AbFmt<__nv_bfloat16> { static constexpr int v = 1; };
-template <> struct AbFmt<__half> { static constexpr int v = 0; };
-__device__ __forceinline__ void tc_ld32(uint32_t taddr, float* v) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-          "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-          "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
 
 __device__ __forceinline__ float silu_tc(float v) { return v * rcp_approx(1.f + ex2(-v * kLog2e)); }
 template <typename T> __device__ __forceinline__ float2 unpack2_tc(uint32_t v);
@@ -110,8 +104,6 @@ __device__ __forceinline__ void cp16(void* smem_dst, const void* gsrc, int nbyte
 
 // element (k, n) of one activation stage, canonical MN-major no-swizzle layout: core (k/8, n/8) = 128 B, row k%8, col n%8
 __device__ __forceinline__ int b_off(int k, int n) { return (((k >> 3) * (TC_PT / 8) + (n >> 3)) << 6) + ((k & 7) << 3) + (n & 7); }
-// element (m, k) of one 128-row weight tile, canonical K-major no-swizzle layout: core (k/8, m/8) = 128 B, row m%8, col k%8
-__device__ __forceinline__ int a_off(int m, int k) { return (((k >> 3) * (TC_MT / 8) + (m >> 3)) << 6) + ((m & 7) << 3) + (k & 7); }
 
 __device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {
     uint32_t done;
@@ -126,8 +118,8 @@ __device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {
         : "memory");
     return done != 0;
 }
-// long waits (epilogue / prologue / producer): back off between polls so that the pollers do not crowd the MIO queue
-// that the working warps' LDS / STS / SHFL go through
+// long waits (producer / prologue): back off between polls so that the pollers do not crowd the MIO queue that the
+// working warps' LDS / STS / SHFL go through
 __device__ __forceinline__ void mbar_wait_sleep(uint64_t* bar, uint32_t parity, int backoff_ns) {
     const uint32_t addr = smem_u32(bar);
     uint32_t done;
@@ -156,21 +148,15 @@ __device__ __forceinline__ void cp_wait_pending(int n) {  // at most n of this t
         default: asm volatile("cp.async.wait_group 3;" ::: "memory"); break;
     }
 }
-struct alignas(32) U8 { uint32_t v[8]; };
-__device__ __forceinline__ void st256(void* p, const U8& u) {
-    asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(u.v[0]), "r"(u.v[1]), "r"(u.v[2]), "r"(u.v[3]),
-                 "r"(u.v[4]), "r"(u.v[5]), "r"(u.v[6]), "r"(u.v[7])
-                 : "memory");
-}
-__device__ __forceinline__ U8 ld256(const void* p) {
-    U8 u;
-    asm volatile("ld.global.nc.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(u.v[0]), "=r"(u.v[1]), "=r"(u.v[2]), "=r"(u.v[3]), "=r"(u.v[4]), "=r"(u.v[5]), "=r"(u.v[6]), "=r"(u.v[7])
-                 : "l"(p));
-    return u;
+__device__ __forceinline__ float2 sel4(const float2* v, int i) {  // v[i] for a run-time i without local memory
+    float2 r = v[0];
+    r = i == 1 ? v[1] : r;
+    r = i == 2 ? v[2] : r;
+    r = i == 3 ? v[3] : r;
+    return r;
 }
 
-// debug trace (VMB_TC_TRACE=1): %globaltimer stamps per CTA -- [0] start, [1] barriers/TMEM ready, [2] weights resident,
+// debug trace (VMB_TC_TRACE=1): %globaltimer stamps per CTA -- [0] start, [1] barriers ready, [2] weights resident,
 // [3] end; tile i < 10 at 4+6i: +0 copies landed, +1 prologue done, +2 MMA saw the operands, +3 MMAs issued,
 // +4 epilogue saw the accumulator, +5 epilogue done
 __device__ long long g_tc_trace[160 * 64];
@@ -181,38 +167,12 @@ __device__ __forceinline__ long long gtimer() {
 }
 
 struct TcShared {  // control block behind the operand buffers
-    uint64_t full[TC_NS], ready[TC_NS], empty[TC_NS], accf[TC_NACC], acce[TC_NACC], wfull;
-    uint32_t tmem_base, pad;
+    uint64_t full[TC_NS], ready[TC_NS], empty[TC_NS], wfull;
 };
-
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "elect.sync _|p, 0xffffffff;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t"
-        "}\n"
-        : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void tc_ld32_nowait(uint32_t taddr, uint32_t* r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-          "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-          "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // KG: compile-time bound on K/8 (a prologue lane keeps that many packed pixel pairs in registers)
 template <typename in_t, int KG>
-__global__ void __launch_bounds__(TC_THREADS, 1) pixlin_tc_kernel(const PixlinParams p, const int tmem_cols, const int wide,
-                                                                  const int trace, const int backoff) {
+__global__ void __launch_bounds__(TC_THREADS, 2) pixlin_tc_kernel(const PixlinParams p, const int trace, const int backoff) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     pdl_trigger();  // everything up to pdl_wait() below touches only weights / parameters and this CTA's own state
     if (!p.w_static) pdl_wait();  // training: the weights are the preceding kernel's output (vmb_prep_block_weights)
@@ -226,7 +186,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) pixlin_tc_kernel(const PixlinPa
     float* sBias = sLn + 2 * kpad;                                               // [nmt*128] output bias
     TcShared* sh = reinterpret_cast<TcShared*>(sBias + nmt * TC_MT);
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, lane = tid & 31;
+    const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);  // warp-uniform to the compiler: the wgmma issue path is not divergent
     const int ptiles = p.P / TC_PT;
     const int total = ptiles * p.B;
     const int my_n = ((int)blockIdx.x < total) ? (total - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
@@ -234,23 +195,15 @@ __global__ void __launch_bounds__(TC_THREADS, 1) pixlin_tc_kernel(const PixlinPa
     const in_t* __restrict__ xg = reinterpret_cast<const in_t*>(p.x);
     const in_t* __restrict__ w = reinterpret_cast<const in_t*>(p.w);
 
-    // ---- setup: barriers, TMEM, LayerNorm parameters ----
+    // ---- setup: barriers, LayerNorm parameters ----
     if (tid == 0) {
         for (int i = 0; i < TC_NS; ++i) {
             mbar_init(&sh->full[i], 32);
             mbar_init(&sh->ready[i], 128);
-            mbar_init(&sh->empty[i], 1);
+            mbar_init(&sh->empty[i], 4);  // lane 0 of each consumer warp, once the tile's MMAs have completed
         }
         mbar_init(&sh->wfull, TC_THREADS - 32);
-        for (int i = 0; i < TC_NACC; ++i) {
-            mbar_init(&sh->accf[i], 1);
-            mbar_init(&sh->acce[i], TC_EPI);
-        }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 5) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&sh->tmem_base)), "r"((uint32_t)tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
     }
     if (p.ln_mode)
         for (int k = tid; k < kpad; k += TC_THREADS) {
@@ -258,10 +211,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) pixlin_tc_kernel(const PixlinPa
             sLn[kpad + k] = (k < p.K && p.ln_mode == 1) ? p.ln_b[k] : 0.f;
         }
     for (int m = tid; m < nmt * TC_MT; m += TC_THREADS) sBias[m] = (p.bias && m < p.M) ? p.bias[m] : 0.f;
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = sh->tmem_base;
     if (tr && threadIdx.x == 0) tr[1] = gtimer();
 
     // producer state (warp 4): tiles issued / tiles whose "full" barrier has been signalled
@@ -289,15 +239,16 @@ __global__ void __launch_bounds__(TC_THREADS, 1) pixlin_tc_kernel(const PixlinPa
         // resident weights: every tile of 128 rows, rows >= M zero-filled.  A warp request covers 8 rows x 64 B (whole
         // sectors from L2, 4-way instead of 32-way bank conflict on the core-matrix layout); a warp walks 8-row groups,
         // no integer division in the loop
-        const int wq = warp < 4 ? warp : warp - 1;          // 0..8 among the nine loading warps
+        const int wq = warp < 4 ? warp : warp - 1;          // 0..7 among the eight loading warps
         const int kq = (kpad + 31) / 32;                    // groups of four 8-wide k chunks
         const int rows8 = nmt * (TC_MT / 8);
         const int kg_l = lane >> 3, m_l = lane & 7;
-        for (int r8 = wq; r8 < rows8; r8 += 9) {
+        for (int r8 = wq; r8 < rows8; r8 += 8) {
             const int mrow = r8 * 8 + m_l;
             const bool ok = mrow < p.M;
             const in_t* src = w + (int64_t)(ok ? mrow : 0) * p.w_ld;
-            in_t* dst = sA + (size_t)(r8 >> 4) * TC_MT * kpad + (((r8 & 15) << 6) + (m_l << 3));  // a_off(m, 0) of this row
+            // element (m, k) of a 128-row weight tile, canonical K-major no-swizzle layout: core (k/8, m/8) = 128 B, row m%8, col k%8
+            in_t* dst = sA + (size_t)(r8 >> 4) * TC_MT * kpad + (((r8 & 15) << 6) + (m_l << 3));
             for (int q = 0; q < kq; ++q) {
                 const int kg = q * 4 + kg_l;
                 if (kg * 8 < kpad) cp16(dst + (size_t)kg * (TC_MT / 8) * 64, src + kg * 8, ok ? 16 : 0);
@@ -307,12 +258,12 @@ __global__ void __launch_bounds__(TC_THREADS, 1) pixlin_tc_kernel(const PixlinPa
         pdl_wait();  // the weight copies fly while the preceding kernel drains; gate / residual / out are touched after this
         asm volatile("cp.async.wait_group 0;" ::: "memory");
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        mbar_arrive(&sh->wfull);  // only the MMA warp waits for the weights
+        mbar_arrive(&sh->wfull);
     }
 
     if (warp == 4) {
         // ================= producer =================
-        // a landed tile is signalled before the warp blocks on a ring stage that the MMA has not released yet
+        // a landed tile is signalled before the warp blocks on a ring stage that the MMAs have not released yet
         while (arrived < my_n) {
             bool can_issue = issued < my_n && issued - arrived < TC_LA;
             if (can_issue && issued > arrived) {
@@ -329,12 +280,12 @@ __global__ void __launch_bounds__(TC_THREADS, 1) pixlin_tc_kernel(const PixlinPa
             if (tr && lane == 0 && arrived < 10) tr[4 + 6 * arrived] = gtimer();
             ++arrived;
         }
-    } else if (warp >= 6) {
+    } else if (warp >= 5) {
         // ================= prologue: LayerNorm / gate in place =================
-        // warp 6+ng owns the 8-pixel column group ng of every tile; one warp instruction covers one 128 B core matrix
+        // warp 5+ng owns the 8-pixel column group ng of every tile; one warp instruction covers one 128 B core matrix
         // (lane = (k%8, pixel pair)), and a lane keeps its K/8 packed pixel pairs in registers between the passes
         if (has_pro) {
-            const int ng = warp - 6, r = lane >> 2;
+            const int ng = warp - 5, r = lane >> 2;
             const int kgs = kpad / 8;
             for (int it = 0; it < my_n; ++it) {
                 const int s = it % TC_NS;
@@ -343,7 +294,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) pixlin_tc_kernel(const PixlinPa
                 const int t = blockIdx.x + it * gridDim.x;
                 const int b = t / ptiles;
                 const float* __restrict__ g = p.gate_mode ? p.gate + (int64_t)b * p.g_bs : nullptr;
-                if (tr && tid == 192 && it == 2) tr[58] = gtimer();
                 uint32_t xv[KG];
 #pragma unroll
                 for (int kg = 0; kg < KG; ++kg) xv[kg] = kg < kgs ? st[kg * 128] : 0u;
@@ -382,7 +332,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) pixlin_tc_kernel(const PixlinPa
                     rs1 = rsqrtf(v1 / p.K + 1e-5f);
                 }
                 const bool wb = p.ln_mode == 1;
-                if (tr && tid == 192 && it == 2) tr[59] = gtimer();
 #pragma unroll
                 for (int kg = 0; kg < KG; ++kg) {
                     const int k = kg * 8 + r;
@@ -411,202 +360,140 @@ __global__ void __launch_bounds__(TC_THREADS, 1) pixlin_tc_kernel(const PixlinPa
                         st[kg * 128] = pack2<in_t>(f.x, f.y);
                     }
                 }
-                if (tr && tid == 192 && it == 2) tr[60] = gtimer();
                 asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                if (tr && tid == 192 && it == 2) tr[61] = gtimer();
                 mbar_arrive(&sh->ready[s]);
-                if (tr && tid == 192 && it < 10) tr[4 + 6 * it + 1] = gtimer();
+                if (tr && tid == 160 && it < 10) tr[4 + 6 * it + 1] = gtimer();
             }
-        }
-    } else if (warp == 5) {
-        // ================= MMA issue =================
-        // the whole warp walks the loops (warp-uniform operands); one elected lane issues.  Descriptors advance by adding
-        // the byte offset >> 4 to the low word (start-address field; smem addresses < 256 KB never carry out of it)
-        const uint32_t idesc = umma_idesc(AbFmt<in_t>::v, TC_MT, TC_PT);
-        const uint32_t a_tile = TC_MT * kpad * 2, x_stage = kpad * TC_PT * 2;
-        // K-major A: SBO = 128 B between 8-row groups, LBO = 16*128 B between the two 8-wide k groups
-        const uint64_t a_desc0 = umma_desc(smem_u32(sA), (TC_MT / 8) * 128, 128);
-        // MN-major B: SBO = 128 B between 8-pixel groups, LBO = 4*128 B between 8-row k groups
-        const uint64_t x_desc0 = umma_desc(smem_u32(sX), (TC_PT / 8) * 128, 128);
-        const bool leader = elect_one();
-        const int ksteps = kpad / 16;
-        mbar_wait(&sh->wfull, 0);
-        if (tr && lane == 0) tr[2] = gtimer();
-        for (int it = 0; it < my_n; ++it) {
-            const int s = it % TC_NS, a = it % TC_NACC;
-            mbar_wait(has_pro ? &sh->ready[s] : &sh->full[s], (it / TC_NS) & 1);
-            mbar_wait(&sh->acce[a], ((it / TC_NACC) & 1) ^ 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            if (tr && lane == 0 && it < 10) tr[4 + 6 * it + 2] = gtimer();
-            const uint64_t bd0 = x_desc0 + (uint64_t)((s * x_stage) >> 4);
-            uint64_t ad = a_desc0;
-            uint32_t d = tmem_base + (uint32_t)(a * nmt * TC_PT);
-            for (int mt = 0; mt < nmt; ++mt, d += TC_PT) {
-                uint64_t bd = bd0;
-                if (leader) tc_mma(d, ad, bd, idesc, 0u);
-                for (int kk = 1; kk < ksteps; ++kk) {
-                    ad += (2 * (TC_MT / 8) * 128) >> 4;  // next 16 k of the weight tile (the tiles are contiguous: after the
-                    bd += (2 * (TC_PT / 8) * 128) >> 4;  // last k step this lands on the next tile's first)
-                    if (leader) tc_mma(d, ad, bd, idesc, 1u);
-                }
-                ad += (2 * (TC_MT / 8) * 128) >> 4;
-            }
-            if (leader) {
-                tc_commit(&sh->empty[s]);  // the stage may be refilled once these MMAs have read it
-                tc_commit(&sh->accf[a]);   // ... and the accumulators are complete
-            }
-            if (tr && lane == 0 && it < 10) tr[4 + 6 * it + 3] = gtimer();
-            __syncwarp();
         }
     } else {
-        // ================= epilogue: thread = TMEM lane = output channel =================
+        // ================= consumer warpgroup: wgmma + epilogue =================
+        // one job = (tile, 64-channel block): its wgmmas, one commit group, wait, epilogue.  Descriptors advance by adding the byte offset >> 4 to the low word (start-address field; shared addresses
+        // < 256 KB never carry out of it)
+        const int nmb = (p.M + TC_MB - 1) / TC_MB;
+        const int ksteps = kpad / 16;
+        // K-major A: SBO = 128 B between 8-row groups, LBO = 16*128 B between the two 8-wide k groups of a k step
+        const uint64_t a_desc0 = gmma_desc(smem_u32(sA), (TC_MT / 8) * 128, 128);
+        // MN-major B: SBO = 128 B between 8-pixel groups, LBO = 4*128 B between the two 8-row k groups of a k step
+        const uint64_t x_desc0 = gmma_desc(smem_u32(sX), (TC_PT / 8) * 128, 128);
         const in_t* __restrict__ resg = reinterpret_cast<const in_t*>(p.residual);
         in_t* __restrict__ og = reinterpret_cast<in_t*>(p.out);
-        for (int it = 0; it < my_n; ++it) {
-            const int a = it % TC_NACC;
+        const int q = lane & 3, row0 = warp * 16 + (lane >> 2);  // accumulator rows row0, row0 + 8; pixel pairs 8j + 2q
+        float acc0[16];
+#pragma unroll
+        for (int i = 0; i < 16; ++i) acc0[i] = 0.f;
+
+        mbar_wait(&sh->wfull, 0);
+        if (tr && tid == 0) tr[2] = gtimer();
+        auto issue = [&](int it, int mb, float* acc) {
+            const int s = it % TC_NS;
+            if (mb == 0) {
+                mbar_wait(has_pro ? &sh->ready[s] : &sh->full[s], (it / TC_NS) & 1);
+                if (tr && tid == 0 && it < 10) tr[4 + 6 * it + 2] = gtimer();
+            }
+            // weight tile mb/2, rows 64*(mb%2).. : 8 row groups further in the K-major layout
+            uint64_t ad = a_desc0 + (uint64_t)(((mb >> 1) * TC_MT * kpad * 2 + (mb & 1) * 8 * 128) >> 4);
+            uint64_t bd = x_desc0 + (uint64_t)((s * kpad * TC_PT * 2) >> 4);
+            acc_fence(acc);
+            wgmma_fence();
+            wgmma_m64n32k16<in_t>(acc, ad, bd, 0u);
+            for (int kk = 1; kk < ksteps; ++kk) {
+                ad += (2 * (TC_MT / 8) * 128) >> 4;  // next 16 k of the weight tile
+                bd += (2 * (TC_PT / 8) * 128) >> 4;
+                wgmma_m64n32k16<in_t>(acc, ad, bd, 1u);
+            }
+            wgmma_commit();
+            if (tr && tid == 0 && it < 10 && mb == nmb - 1) tr[4 + 6 * it + 3] = gtimer();
+        };
+        auto finish = [&](int it, int mb, float* acc) {  // job (it, mb) has completed
+            acc_fence(acc);
+            if (mb == nmb - 1) {
+                if (lane == 0) mbar_arrive(&sh->empty[it % TC_NS]);  // the stage may be refilled
+                if (tr && tid == 0 && it < 10) tr[4 + 6 * it + 4] = gtimer();
+            }
             const int t = blockIdx.x + it * gridDim.x;
             const int b = t / ptiles, p0 = (t - b * ptiles) * TC_PT;
-            mbar_wait_sleep(&sh->accf[a], (it / TC_NACC) & 1, backoff);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            if (tr && tid == 0 && it < 10) tr[4 + 6 * it + 4] = gtimer();
-            const uint32_t t_acc = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(a * nmt * TC_PT);
-            uint32_t acc[2][32];
-            tc_ld32_nowait(t_acc, acc[0]);
-#pragma unroll 1
-            for (int mt2 = 0; mt2 < nmt; mt2 += 2) {
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int mt = mt2 + h;
-                    if (mt < nmt) {  // warp-uniform
-                        const int mg = mt * TC_MT + tid;
-                        const bool live = mg < p.M;
-                        U8 r0, r1;
-                        if (resg && live) {
-                            const in_t* rp = resg + (int64_t)b * p.r_bs + (int64_t)mg * p.r_cs + p0;
-                            if (wide) {
-                                r0 = ld256(rp);
-                                r1 = ld256(rp + 16);
-                            } else {
-                                const uint4 q0 = __ldg(reinterpret_cast<const uint4*>(rp)), q1 = __ldg(reinterpret_cast<const uint4*>(rp) + 1);
-                                const uint4 q2 = __ldg(reinterpret_cast<const uint4*>(rp) + 2), q3 = __ldg(reinterpret_cast<const uint4*>(rp) + 3);
-                                r0 = U8{{q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w}};
-                                r1 = U8{{q2.x, q2.y, q2.z, q2.w, q3.x, q3.y, q3.z, q3.w}};
-                            }
+            for (int h = 0; h < 2; ++h) {
+                const int mg = mb * TC_MB + row0 + 8 * h;
+                const float bs = sBias[mg];
+                const bool act = mg >= p.act_from && mg < p.act_to;
+                // lane q holds pixels 8j + 2q, +1 (j = 0..3); after the quad transpose it holds pixels 8q .. 8q+7
+                float2 v[4], rcv[4];
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    v[j] = make_float2(acc[4 * j + 2 * h] + bs, acc[4 * j + 2 * h + 1] + bs);
+                    if (act) v[j] = make_float2(silu_tc(v[j].x), silu_tc(v[j].y));
+                }
+                rcv[0] = sel4(v, q);
+#pragma unroll
+                for (int i = 1; i < 4; ++i) {
+                    const float2 snd = sel4(v, q ^ i);
+                    rcv[i] = make_float2(__shfl_xor_sync(0xffffffffu, snd.x, i), __shfl_xor_sync(0xffffffffu, snd.y, i));
+                }
+                float2 o[4];
+#pragma unroll
+                for (int c = 0; c < 4; ++c) o[c] = sel4(rcv, c ^ q);  // pixels 8q + 2c, +1
+                if (mg < p.M) {
+                    if (resg) {
+                        const uint4 r = __ldg(reinterpret_cast<const uint4*>(resg + (int64_t)b * p.r_bs + (int64_t)mg * p.r_cs + p0 + 8 * q));
+                        const uint32_t rw[4] = {r.x, r.y, r.z, r.w};
+#pragma unroll
+                        for (int c = 0; c < 4; ++c) {
+                            const float2 f = unpack2_tc<in_t>(rw[c]);
+                            o[c].x += f.x;
+                            o[c].y += f.y;
                         }
-                        tc_wait_ld();  // acc[h] has landed
-                        if (mt + 1 < nmt) tc_ld32_nowait(t_acc + (uint32_t)((mt + 1) * TC_PT), acc[h ^ 1]);  // overlaps this tile's epilogue
-                        if (live) {
-                            float v[32];
-                            const float bs = sBias[mg];
-#pragma unroll
-                            for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(acc[h][i]) + bs;
-                            if (mg >= p.act_from && mg < p.act_to) {
-#pragma unroll
-                                for (int i = 0; i < 32; ++i) v[i] = silu_tc(v[i]);
-                            }
-                            if (resg) {
-#pragma unroll
-                                for (int q = 0; q < 8; ++q) {
-                                    const float2 f0 = unpack2_tc<in_t>(r0.v[q]), f1 = unpack2_tc<in_t>(r1.v[q]);
-                                    v[2 * q] += f0.x;
-                                    v[2 * q + 1] += f0.y;
-                                    v[16 + 2 * q] += f1.x;
-                                    v[16 + 2 * q + 1] += f1.y;
-                                }
-                            }
-                            U8 o0, o1;
-#pragma unroll
-                            for (int q = 0; q < 8; ++q) {
-                                o0.v[q] = pack2<in_t>(v[2 * q], v[2 * q + 1]);
-                                o1.v[q] = pack2<in_t>(v[16 + 2 * q], v[16 + 2 * q + 1]);
-                            }
-                            in_t* op = og + (int64_t)b * p.o_bs + (int64_t)mg * p.o_cs + p0;
-                            if (wide) {
-                                st256(op, o0);
-                                st256(op + 16, o1);
-                            } else {
-                                uint4* o4 = reinterpret_cast<uint4*>(op);
-                                o4[0] = make_uint4(o0.v[0], o0.v[1], o0.v[2], o0.v[3]);
-                                o4[1] = make_uint4(o0.v[4], o0.v[5], o0.v[6], o0.v[7]);
-                                o4[2] = make_uint4(o1.v[0], o1.v[1], o1.v[2], o1.v[3]);
-                                o4[3] = make_uint4(o1.v[4], o1.v[5], o1.v[6], o1.v[7]);
-                            }
-                        }
-                        __syncwarp();
                     }
+                    *reinterpret_cast<uint4*>(og + (int64_t)b * p.o_bs + (int64_t)mg * p.o_cs + p0 + 8 * q) =
+                        make_uint4(pack2<in_t>(o[0].x, o[0].y), pack2<in_t>(o[1].x, o[1].y), pack2<in_t>(o[2].x, o[2].y),
+                                   pack2<in_t>(o[3].x, o[3].y));
                 }
             }
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            if (tr && tid == 0 && it < 10) tr[4 + 6 * it + 5] = gtimer();
-            mbar_arrive(&sh->acce[a]);  // this thread's TMEM reads of the stage are complete (tcgen05.wait::ld in tc_ld32)
-        }
+            if (tr && tid == 0 && it < 10 && mb == nmb - 1) tr[4 + 6 * it + 5] = gtimer();
+        };
+        for (int it = 0; it < my_n; ++it)
+            for (int mb = 0; mb < nmb; ++mb) {
+                issue(it, mb, acc0);
+                wgmma_wait<0>();
+                finish(it, mb, acc0);
+            }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
     if (tr && threadIdx.x == 0) tr[3] = gtimer();
-    if (warp == 5) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)tmem_cols) : "memory");
 }
 
 static size_t tc_smem_bytes(const PixlinParams& p) {
     const size_t kpad = (p.K + 15) / 16 * 16, nmt = (p.M + TC_MT - 1) / TC_MT;
     return nmt * TC_MT * kpad * 2 + (size_t)TC_NS * kpad * TC_PT * 2 + (2 * kpad + nmt * TC_MT) * sizeof(float) + sizeof(TcShared) + 128;
 }
-static int tc_num_sms() {
-    static int n = 0;
-    if (n == 0) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
-    }
-    return n;
-}
 
 bool pixlin_tc_applicable(const PixlinParams& p, int dtype, int out_dtype) {
-    int mode = 1;  // 0: off, 1: where it was measured faster than the mma.sync kernel, 2: whenever legal (tests)
+    // VMB_PIXLIN_TC: 0 (default) off, otherwise whenever legal (tests).  Off by default: on the H100 this kernel measured 1.2-1.9x
+    // slower than the mma.sync kernel of pixlin.cu on every legal 1x1-conv shape of the bench nets (tools/pixlin_bench.py, B = 8
+    // inference and B = 4 training, 64x64), and the bench step with it on every legal shape 10 % slower
+    int mode = 0;
     if (const char* e = getenv("VMB_PIXLIN_TC")) mode = atoi(e);
     if (mode == 0) return false;
-    const bool legal = (dtype == VMB_BF16 || dtype == VMB_F16) && out_dtype == dtype && p.vec_ok && p.w_vec && p.P % TC_PT == 0 &&
-                       p.M <= TC_MAXMT * TC_MT && p.K <= 8 * TC_KGMAX && tc_smem_bytes(p) <= TC_SMEM_MAX;
-    if (!legal || mode == 2) return legal;
-    // round-1 measurements (tools/pixlin_bench.py, profiles/pixlin_tc_r1.md): the fixed cost of a launch (barriers, TMEM,
-    // ~5-9 us for the resident weights, partly hidden behind the previous kernel by the programmatic launch) needs >= 4
-    // tiles per SM to amortise, and the LayerNorm / gate prologue warps pace the pipeline at ~2 us per tile at K = 96.
-    // Measured wins at B=8, 64x64: no prologue with K > 128 or M > 128 (x_proj fold, project_out of C=96), LayerNorm with
-    // M > 256 (project_in, C=96) or with K <= 64 and M > 128 (project_in, C=48); everything else stays on mma.sync
-    const long tiles = (long)(p.P / TC_PT) * p.B;
-    const bool has_pro = p.ln_mode != 0 || p.gate_mode != 0;
-    if (tiles < 3L * tc_num_sms()) return false;
-    // 3-4 tiles per SM (the training step's B = 4, 64x64; round 2, `PB_TRAIN=1 PB_B=4 tools/pixlin_bench.py`): the mma.sync kernel has
-    // only 1-2 CTAs per SM there and loses on every shape but the gate prologue and the reduction-heavy K > 128 -> M <= 64 ones
-    // (e.g. 96 -> 512: 13.7 vs 22.7 us, LayerNorm 96 -> 510: 18.8 vs 30.7 us, 254 -> 48: 9.9 vs 7.1 us)
-    if (tiles < 4L * tc_num_sms()) return p.gate_mode == 0 && !(p.K > 128 && p.M <= 64);
-    if (!has_pro) return p.K > 128 || p.M > 128;
-    return p.gate_mode == 0 && (p.M > 2 * TC_MT || (p.K <= 64 && p.M > TC_MT));
+    return (dtype == VMB_BF16 || dtype == VMB_F16) && out_dtype == dtype && p.vec_ok && p.w_vec && p.P % TC_PT == 0 &&
+           p.M <= TC_MAXMT * TC_MT && p.K <= 8 * TC_KGMAX && tc_smem_bytes(p) <= TC_SMEM_MAX;
 }
 
 int pixlin_tc_launch(const PixlinParams& p, int dtype, cudaStream_t stream) {
     const size_t smem = tc_smem_bytes(p);
-    const int nmt = (p.M + TC_MT - 1) / TC_MT;
-    // TC_NACC accumulator stages of nmt*32 TMEM columns each (<= 512 columns).  (Interleaving the MMAs of several tiles /
-    // weight tiles over independent accumulators was measured slower, see profiles/pixlin_tc_r1.md.)
-    const int nacc = TC_NACC;
-    int cols = 32;
-    while (cols < nacc * nmt * TC_PT) cols <<= 1;
     const long total = (long)(p.P / TC_PT) * p.B;
-    const int grid = (int)(total < tc_num_sms() ? total : tc_num_sms());
-    auto al32 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 31) == 0; };
+    // two CTAs per SM where their shared memory fits: twice the consumer warpgroups (epilogue latency) per SM
+    const long ctas = (long)num_sms() * (2 * (smem + 1024) <= 228 * 1024 ? 2 : 1);
+    const int grid = (int)(total < ctas ? total : ctas);
     const char* be = getenv("VMB_TC_BACKOFF");
     const int backoff = be ? atoi(be) : 100;
     const char* te = getenv("VMB_TC_TRACE");
     const int trace = te ? atoi(te) : 0;
-    const int wide = al32(p.out) && p.o_bs % 16 == 0 && p.o_cs % 16 == 0 &&
-                     (!p.residual || (al32(p.residual) && p.r_bs % 16 == 0 && p.r_cs % 16 == 0));
     const int kg = (p.K + 7) / 8;
 #define VMB_TC_GO(T, KGV)                                                                              \
     do {                                                                                               \
         auto k = pixlin_tc_kernel<T, KGV>;                                                             \
         VMB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));     \
-        VMB_CUDA(launch_pdl(k, dim3(grid), dim3(TC_THREADS), smem, stream, p, cols, wide, trace, backoff));                             \
+        VMB_CUDA(launch_pdl(k, dim3(grid), dim3(TC_THREADS), smem, stream, p, trace, backoff));        \
     } while (0)
     if (dtype == VMB_BF16) {
         if (kg <= 8) VMB_TC_GO(__nv_bfloat16, 8);

@@ -1,4 +1,4 @@
-// Selective-scan backward for sm_100a -- replaces selective_scan_bwd_kernel
+// Selective-scan backward for sm_90a -- replaces selective_scan_bwd_kernel
 // (reference: Mamba/kernels/selective_scan/csrc/selective_scan/cus/selective_scan_bwd_kernel.cuh:66-273).
 //
 // Same warp-autonomous mapping as the forward (scan_fwd.cu): a warp owns RB rows x (32/RB) segments

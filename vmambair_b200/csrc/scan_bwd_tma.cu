@@ -1,4 +1,4 @@
-// Selective-scan backward, TMA-staged multi-warp variant (sm_100a) -- the fast path of vmb_selective_scan_bwd.
+// Selective-scan backward, TMA-staged multi-warp variant (sm_90a) -- the fast path of vmb_selective_scan_bwd.
 // Replaces selective_scan_bwd_kernel (reference: Mamba/kernels/selective_scan/csrc/selective_scan/cus/selective_scan_bwd_kernel.cuh:66-273).
 //
 // Same per-pair math as scan_bwd.cu (F1 decay factors + local end state, forward segment scan from the forward's checkpoints,
@@ -6,8 +6,8 @@
 // the forward (scan_fwd_tma.cu):
 //   * a CTA of 4 warps owns RB*4/SS rows of one (batch, group); u / delta / dout rows and the 16 B and 16 C state rows arrive as
 //     cp.async.bulk.tensor boxes (one issuing thread, mbarrier completion) one chunk ahead, walking the sequence backwards;
-//   * ONE fp32 B/C pair tile per CTA instead of one per warp (the round-1 kernel ran single-warp CTAs: 384 warps on 148 SMs at
-//     batch 4, each converting its own tile) -> RB = 2 rows per warp is affordable: 768 warps at batch 4, 4-8 per SM;
+//   * ONE fp32 B/C pair tile per CTA instead of one per warp (single-warp CTAs would each convert their own tile) -> RB = 2
+//     rows per warp is affordable: 768 warps at batch 4, 4-8 per SM;
 //   * state split (SS): the 8 state pairs of a row over SS warps at small batch; the per-position sums over states (s1, s2) meet in
 //     shared memory, du / ddelta are written by the first warp of the row slot;
 //   * the dB/dC row reduction: warp-local smem transpose ([row][segment][T + 1] float4: the (row, segment) lanes write without bank
@@ -419,7 +419,7 @@ static int launch_bt1(const ScanBwdParams& p, const ScanBwdTmaMaps& maps, int rb
     return rb == 4 ? launch_bt2<in_t, 4>(p, maps, ss, stream) : launch_bt2<in_t, 2>(p, maps, ss, stream);
 }
 
-// (rows per warp, state split): the 255-register kernel keeps 2 CTAs x 4 warps per SM resident (296 CTAs per wave)
+// (rows per warp, state split): the 255-register kernel keeps 2 CTAs x 4 warps per SM resident (2 x SMs CTAs per wave)
 bool scan_bwd_tma_pick(const ScanBwdParams& p, int dtype, int& rb, int& ss) {
     const char* e = getenv("VMB_SCAN_BWD_TMA");
     if (e && atoi(e) == 0) return false;
@@ -427,11 +427,10 @@ bool scan_bwd_tma_pick(const ScanBwdParams& p, int dtype, int& rb, int& ss) {
     if (!p.vec_ok || p.npad != 16 || p.L < 512 || p.ckpt == nullptr) return false;
     const int rpg = p.rows_per_group;
     const long rows = (long)p.batch * p.dim;
-    // measured (tools/scan_bwd_sweep.py): RB = 2 wins at every batch (B = 8: 59 vs 83 us/img for RB = 4 although its 384 CTAs
-    // exceed one resident wave); the state split pays while the CTAs still fit one wave (B = 1: SS = 4, 114 vs 212 us/img)
+    // RB = 2 at every batch; the state split while the CTAs still fit one resident wave (tools/scan_bwd_sweep.py sweeps both)
     rb = 2;
     ss = 1;
-    while (ss < 4 && rows / (rb * 4 / ss) * 2 <= 296) ss <<= 1;
+    while (ss < 4 && rows / (rb * 4 / ss) * 2 <= 2L * num_sms()) ss <<= 1;
     if (const char* v = getenv("VMB_SCAN_RB_BWD")) {
         const int x = atoi(v);
         if (x == 2 || x == 4) rb = x;

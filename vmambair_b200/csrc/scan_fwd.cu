@@ -1,7 +1,7 @@
-// Selective-scan forward for sm_100a -- replaces selective_scan_fwd_kernel
+// Selective-scan forward for sm_90a -- replaces selective_scan_fwd_kernel
 // (reference: Mamba/kernels/selective_scan/csrc/selective_scan/cus/selective_scan_fwd_kernel.cuh:61-172).
 //
-// Design (B200-first, not a port of the CUB block-scan kernel):
+// Design (not a port of the CUB block-scan kernel):
 //   * one WARP owns RB rows (channels d of one (batch, group)) and walks the sequence in chunks of
 //     (32/RB) segments x T=16 positions; lane -> (row = lane % RB, segment = lane / RB).  The WPC warps
 //     of a CTA own different rows of the SAME group and share one staged B/C tile; they only meet at
@@ -352,8 +352,7 @@ static void pick_cfg(const ScanFwdParams& p, int& rb, int& wpc) {
     int env_rb = 0, env_wpc = 0;
     if (const char* e = getenv("VMB_SCAN_RB")) env_rb = atoi(e);
     if (const char* e = getenv("VMB_SCAN_WPC")) env_wpc = atoi(e);
-    // measured on B200 (bf16, C=96, L=4096; tools/scan_sustained.py): rows=384 -> RB=1, rows=3072 -> RB=2,
-    // rows=12288 -> RB=4..8 (all within 2 %); i.e. aim for >= ~1500 warps, then grow RB for cheaper scans.
+    // aim for >= ~1500 warps, then grow RB for cheaper scans (tools/scan_sustained.py sweeps RB per shape)
     rb = rows < 1536 ? 1 : rows < 8192 ? 2 : rows < 32768 ? 4 : 8;
     while (rb > 1 && rpg % rb) rb >>= 1;
     // short sequences: a warp-chunk should not be much longer than L

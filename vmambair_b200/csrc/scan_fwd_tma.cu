@@ -1,4 +1,4 @@
-// Selective-scan forward, TMA-staged variant (sm_100a) -- the fast path of vmb_selective_scan_fwd[_grouped].
+// Selective-scan forward, TMA-staged variant (sm_90a) -- the fast path of vmb_selective_scan_fwd[_grouped].
 // Replaces selective_scan_fwd_kernel (reference: Mamba/kernels/selective_scan/csrc/selective_scan/cus/selective_scan_fwd_kernel.cuh:61-172).
 //
 // Same recurrence mapping as scan_fwd.cu (lane = (row, segment of T positions), two register passes per state pair in packed
@@ -393,9 +393,9 @@ static int launch_tma5(const ScanFwdParams& p, const ScanTmaMaps& maps, cudaStre
     return VMB_OK;
 }
 
-// POLY = 1 (6 of 16 decay factors per lane-chunk by exp2_poly2 on the FMA pipe) is an EXPERIMENT that lost: 18.0 vs 15.6 us/img at
-// (8, 384, 4096) bf16, 14.8 vs 13.1 at batch 32 (profiles/scan_fwd_r2.md) -- the FMA pipe / issue slots have less slack than the
-// pipe-utilisation counters suggest.  Build with -DVMB_SCAN_POLY_VARIANT and set VMB_SCAN_POLY=1 to reproduce the measurement.
+// POLY = 1 (6 of 16 decay factors per lane-chunk by exp2_poly2 on the FMA pipe) is an EXPERIMENT, off by default: the FMA pipe /
+// issue slots have less slack than the pipe-utilisation counters suggest.  Build with -DVMB_SCAN_POLY_VARIANT and set
+// VMB_SCAN_POLY=1 to measure it.
 template <typename in_t, int RB, int NW, int SS, int MODE>
 static int launch_tma4(const ScanFwdParams& p, const ScanTmaMaps& maps, cudaStream_t stream) {
 #ifdef VMB_SCAN_POLY_VARIANT
@@ -411,7 +411,7 @@ static int launch_tma3(const ScanFwdParams& p, const ScanTmaMaps& maps, cudaStre
     return p.ckpt ? launch_tma4<in_t, RB, NW, SS, 1>(p, maps, stream) : launch_tma4<in_t, RB, NW, SS, 0>(p, maps, stream);
 }
 
-// 4-warp CTAs, three resident per SM: 384 CTAs at (8, 384, 4096) spread 2-3 per SM (8-warp CTAs: 192 on 148 SMs, 1-2 per SM)
+// 4-warp CTAs, three resident per SM: 384 CTAs at (8, 384, 4096) spread 2-3 per SM (8-warp CTAs: 192 on 132 SMs, 1-2 per SM)
 constexpr int kTmaWarps = 4;
 
 template <typename in_t, int RB>
@@ -437,9 +437,9 @@ bool scan_fwd_tma_pick(const ScanFwdParams& p, int& rb, int& ss) {
     if (p.ndesc && p.N != 16) return false;  // grouped sources: the B/C boxes are 16 rows of a wider tensor
     const int rpg = p.rows_per_group;
     const long rows = (long)p.batch * p.dim;
-    const long want = 1184;  // >= 2 warps per scheduler on 148 SMs
-    // measured (tools/scan_sweep.py, profiles/scan_sweep_r2.md): rb = 2 wins at every batch size -- with more rows per warp the
-    // B/C tile reads shrink but the warp count drops, and the MUFU + LDS + SHFL instructions of a warp all queue on one path
+    const long want = 8L * num_sms();  // >= 2 warps per scheduler
+    // rb = 2 at every batch size (tools/scan_sweep.py sweeps it): with more rows per warp the B/C tile reads shrink but the warp
+    // count drops, and the MUFU + LDS + SHFL instructions of a warp all queue on one path
     rb = 2;
     ss = 1;
     while (ss < 4 && rows / rb * ss < want) ss <<= 1;
@@ -454,12 +454,7 @@ bool scan_fwd_tma_pick(const ScanFwdParams& p, int& rb, int& ss) {
 int scan_fwd_tma_launch(const ScanFwdParams& p_in, int dtype, int rb, int ss, cudaStream_t stream) {
     ScanFwdParams p = p_in;
     {
-        static const int sms = [] {
-            int dev = 0, n = 148;
-            if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-            return n > 0 ? n : 148;
-        }();
-        p.num_sms = sms;
+        p.num_sms = num_sms();
     }
     ScanTmaMaps maps;
     const uint32_t chunk = 32 / rb * T, rows = rb * kTmaWarps / ss;

@@ -1,6 +1,6 @@
-// TMA (cp.async.bulk.tensor) + mbarrier helpers for sm_100a, and the host-side tensor-map encoder.
+// TMA (cp.async.bulk.tensor) + mbarrier helpers for sm_90a, and the host-side tensor-map encoder.
 // The library links only cudart: cuTensorMapEncodeTiled is fetched at run time through cudaGetDriverEntryPoint
-// (there is no libcuda in the build container; on a GPU box the driver is always present).
+// (the library builds on hosts without a driver; where it runs, the driver is present).
 #pragma once
 #include <cuda.h>
 

@@ -610,7 +610,7 @@ __global__ void adam_step_inc_kernel(float* state) {
 }
 
 int fused_adam_launch(const AdamParams& p, cudaStream_t stream) {
-    const int blocks = (int)((p.n + 255) / 256 < 148 * 8 ? (p.n + 255) / 256 : 148 * 8);
+    const int blocks = (int)((p.n + 255) / 256 < num_sms() * 8 ? (p.n + 255) / 256 : num_sms() * 8);
     if (p.max_norm > 0.f) sqsum_kernel<<<blocks, 256, 0, stream>>>(p.grad, p.n, p.state);
     fused_adam_kernel<<<blocks, 256, 0, stream>>>(p);
     adam_step_inc_kernel<<<1, 1, 0, stream>>>(p.state);
@@ -861,7 +861,7 @@ extern "C" int vmb_sum4_add(const void* x4, const void* add, void* out, int batc
     VMB_CHECK(per_dir % v == 0 && ((reinterpret_cast<uintptr_t>(x4) | reinterpret_cast<uintptr_t>(add) | reinterpret_cast<uintptr_t>(out)) & 15) == 0,
               "sum4_add: 16 B aligned contiguous tensors");
     const long total = (long)batch * per_dir;
-    const int blocks = (int)((total / v + 255) / 256 < 148 * 8 ? (total / v + 255) / 256 : 148 * 8);
+    const int blocks = (int)((total / v + 255) / 256 < num_sms() * 8 ? (total / v + 255) / 256 : num_sms() * 8);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     switch (dtype) {
         case VMB_F32: VMB_CUDA(launch_pdl(sum4_add_kernel<float>, dim3(blocks), dim3(256), 0, st, (const float*)x4, (const float*)add, (float*)out, per_dir, 4 * per_dir, total)); break;

@@ -4,7 +4,7 @@
 // kernel is split over pixels: CTA (m-tile 64, k-tile 64, pixel range), mma.sync m16n8k16 (bf16 / fp16 in, fp32 accumulate) from
 // cp.async double-buffered [64 rows][32 pixels] tiles, fp32 atomicAdd of the 64 x 64 partial into dW (the caller zero-fills).
 // Tensor cores are the right unit here (a dense contraction) but the shape is tiny and reduction-dominated: the legacy mma.sync
-// path is used on purpose -- a tcgen05 pipeline needs >= 128 x 64 tiles and its setup cost exceeds these 2-10 us launches.
+// path is used on purpose -- a wgmma pipeline needs 64-row warpgroup tiles and a persistent set-up that these short launches cannot amortise.
 #include "common.cuh"
 #include "train_params.h"
 
@@ -159,7 +159,7 @@ extern "C" int vmb_pixlin_wgrad(const vmb_wgrad_args* a, void* stream) {
     WgradParams p{a->dy, a->x, a->out, a->batch, a->M, a->K, a->L, a->dy_bs, a->dy_cs, a->x_bs, a->x_cs, 1, a->per_batch, a->dbias};
     // pixel splits: enough CTAs for ~2 waves, at least 512 pixels per CTA
     const long tiles = (long)((a->M + WG_TM - 1) / WG_TM) * ((a->K + WG_TN - 1) / WG_TN) * a->batch;
-    int splits = (int)((2 * 148 + tiles - 1) / tiles);
+    int splits = (int)((2 * num_sms() + tiles - 1) / tiles);
     const int max_splits = (a->L + 511) / 512;
     p.splits = splits < 1 ? 1 : (splits > max_splits ? max_splits : splits);
     return wgrad_launch(p, a->dtype, static_cast<cudaStream_t>(stream));

@@ -1,7 +1,7 @@
 """`selective_scan_fn` -- drop-in for the reference's SelectiveScanFn / selective_scan_fn_v1
 (SRGAN/VmambaIR/archs/MambaSISR6_arch.py:24-96, same in the Deraining / RealSR archs): same
 argument order, same contiguity / dim fix-ups, same returned gradients; the kernels underneath are
-the sm_100a ones of this repository (through the C-ABI).
+the sm_90a ones of this repository (through the C-ABI).
 """
 from __future__ import annotations
 

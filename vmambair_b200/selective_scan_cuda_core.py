@@ -2,7 +2,7 @@
 (Mamba/kernels/selective_scan/csrc/selective_scan/cus/selective_scan.cpp:351-354): exposes
 `fwd(u, delta, A, B, C, D, delta_bias, delta_softplus, nrows) -> [out, x]` and
 `bwd(u, delta, A, B, C, D, delta_bias, dout, x, delta_softplus, nrows) -> [du, ddelta, dA, dB, dC, dD, ddelta_bias]`
-with the same arity / return order, so the UNMODIFIED reference archs run on the sm_100a kernels:
+with the same arity / return order, so the UNMODIFIED reference archs run on the sm_90a kernels:
 
     import sys, vmambair_b200.selective_scan_cuda_core as m
     sys.modules["selective_scan_cuda_core"] = m          # before importing the reference arch

@@ -7,7 +7,7 @@ Reference behaviour mirrored:
   * tile_process: RealESRGANer.tile_process (RealSR/VmambaIR/utils.py:97-160): tiles of `tile_size` with `tile_pad` pixels of
     context on every side that exists, each upscaled on its own, the un-padded centre written into the output.
 
-B200-first difference: tiles of equal shape are independent units of the path, so they are stacked on the batch axis and go through
+GPU-first difference: tiles of equal shape are independent units of the path, so they are stacked on the batch axis and go through
 the network in batches of `max_batch` tiles instead of one forward per tile; the stitched result is the reference's.
 """
 from __future__ import annotations

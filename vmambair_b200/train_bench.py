@@ -18,7 +18,8 @@ H = W = 64
 
 
 def run_train(args, build_net, ClockSampler, env_rank, dist_max, barrier, peaks, sample_clocks=True):
-    """-> the JSON record (dict) of the training workload on this rank's GPU; the process group is the caller's."""
+    """-> (the JSON record (dict) of the training workload on this rank's GPU, {name: tensor} of what the last timed step
+    computed); the process group is the caller's."""
     from . import archs, ops
     from .optim import FlatAdam
     rank, local, world = env_rank()
@@ -114,10 +115,13 @@ def run_train(args, build_net, ClockSampler, env_rank, dist_max, barrier, peaks,
     s, e = torch.cuda.Event(True), torch.cuda.Event(True)
     s.record()
     for _ in range(K):
-        step(lq, gt)
+        loss_last = step(lq, gt)
     e.record()
     torch.cuda.synchronize(dev)
     barrier(world)
+    # what the last timed step computed: its loss and a seeded sample of the parameters it left (fp32 flat buffer)
+    idx = torch.randint(0, opt.n, (1 << 20,), generator=torch.Generator().manual_seed(5)).to(dev)
+    outputs = {"train_loss": loss_last.detach().float().view(1).clone(), "train_params_sample": opt.flat_param[idx]}
     total_ms = dist_max(s.elapsed_time(e), world, dev)
     # collective share: the all-reduce alone, timed on the device
     ar_ms = 0.0
@@ -185,4 +189,4 @@ def run_train(args, build_net, ClockSampler, env_rank, dist_max, barrier, peaks,
                      "share_of_step": round((fw[1] + bw[1]) / ms_step, 3)},
         "clocks": clocks,
     }
-    return out
+    return out, outputs

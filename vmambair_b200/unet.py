@@ -13,7 +13,7 @@ separate pass over HBM (and, on cuDNN, an NCHW<->NHWC transform either side of e
     the same way.
 
 The two middle convs of the SR tail (96 -> 384 at 64x64 and 128x128: 22 + 87 GFLOP per 8-image batch, compute-bound) stay on the
-library convolution (cuDNN's sm_100 kernels, NHWC) with this library's NHWC PixelShuffle between them.
+library convolution (cuDNN's sm_90 kernels, NHWC) with this library's NHWC PixelShuffle between them.
 
 Inference only: with gradients enabled the modules' nn.Conv2d / torch.cat path (autograd) is used.  VMB_UNET=torch restores that
 path for inference as well (cross-checks, tests).
