@@ -118,9 +118,6 @@ typedef struct {
     int64_t x_bs, x_cs, r_bs, r_cs, o_bs, o_cs, g_bs;
     int64_t w_ld;                           /* row stride of w (0: = K); rows padded to a multiple of 16 elements load vectorised */
     int dtype, out_dtype;                   /* x / w / residual dtype; out dtype (same, or VMB_F32) */
-    int w_static;                           /* 1: w / bias / ln_w / ln_b were final before the preceding kernel of the stream was launched
-                                             * (cached inference weights): the kernel may stage them while that kernel still runs
-                                             * (programmatic dependent launch); 0: they may be its output -- fetched after it completes */
 } vmb_pixlin_args;
 int vmb_pixlin(const vmb_pixlin_args* a, void* stream);
 

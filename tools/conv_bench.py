@@ -75,7 +75,7 @@ def main():
         cat = torch.cat([u, e], 1)
         wq = ops.pad_weight(w1.view(c, 2 * c))
         t_ref = timeit(lambda: F.conv2d(torch.cat([u, e], 1), w1))
-        t_our = timeit(lambda: ops.pixlin(cat.view(B, 2 * c, hw * hw), wq, static_w=True))
+        t_our = timeit(lambda: ops.pixlin(cat.view(B, 2 * c, hw * hw), wq))
         print(json.dumps({"site": name, "torch_us": round(t_ref, 1), "vmb_us": round(t_our, 1)}))
 
 

@@ -1,6 +1,5 @@
-"""Per-shape sustained timing of the 1x1-conv GEMM (vmb_pixlin) on the shapes of the light SISR net at B=8, 64x64:
-mma.sync kernel (VMB_PIXLIN_TC=0) against the wgmma kernel (VMB_PIXLIN_TC=2).  Four rotating buffer sets
-(> L2 together for the big shapes), 10 launches per CUDA graph, 20 replays."""
+"""Per-shape sustained timing of the 1x1-conv GEMM (vmb_pixlin) on the shapes of the light SISR net at B=8, 64x64.
+Four rotating buffer sets (> L2 together for the big shapes), 12 launches per CUDA graph, 20 replays."""
 import sys, os, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -42,22 +41,19 @@ for name, K, M, kind in SHAPES:
 
     nbytes = 2 * B * P * (K + M + (M if "res" in kind else 0))
     row = dict(shape=name, K=K, M=M, kind=kind, MB=round(nbytes / 1e6, 1))
-    for mode in ("0", "2"):
-        os.environ["VMB_PIXLIN_TC"] = mode
-        call(sets[0]); torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            for i in range(12):
-                call(sets[i % 4])
-        for _ in range(3):
-            g.replay()
-        torch.cuda.synchronize()
-        s, e = torch.cuda.Event(True), torch.cuda.Event(True)
-        s.record()
-        for _ in range(20):
-            g.replay()
-        e.record(); torch.cuda.synchronize()
-        us = s.elapsed_time(e) / (20 * 12) * 1e3
-        tag = "mma" if mode == "0" else "tc"
-        row[tag + "_us"] = round(us, 2); row[tag + "_GBs"] = round(nbytes / us / 1e3, 0)
+    call(sets[0]); torch.cuda.synchronize()
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        for i in range(12):
+            call(sets[i % 4])
+    for _ in range(3):
+        g.replay()
+    torch.cuda.synchronize()
+    s, e = torch.cuda.Event(True), torch.cuda.Event(True)
+    s.record()
+    for _ in range(20):
+        g.replay()
+    e.record(); torch.cuda.synchronize()
+    us = s.elapsed_time(e) / (20 * 12) * 1e3
+    row["us"] = round(us, 2); row["GBs"] = round(nbytes / us / 1e3, 0)
     print(json.dumps(row), flush=True)

@@ -1,4 +1,4 @@
-"""A few launches of one pixlin shape (for ncu): PB_SHAPE in {pin96,in_conv96,w_big96,pout96}, VMB_PIXLIN_TC selects kernel."""
+"""A few launches of one pixlin shape (for ncu): PB_SHAPE in {pin96,in_conv96,w_big96,pout96}."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

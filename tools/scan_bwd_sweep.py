@@ -1,4 +1,4 @@
-"""rows-per-warp sweep of the selective-scan backward (VMB_SCAN_RB_BWD) at the north-star shape, next to the reference kernel."""
+"""state-split sweep of the TMA selective-scan backward (VMB_SCAN_SS_BWD) at the north-star shape, next to the reference kernel."""
 import json, os, sys, importlib.util
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -24,11 +24,11 @@ for dt in (torch.bfloat16,):
         if refm is not None:
             o_r, x_r = refm.fwd(u, delta, A, Bm, Cm, Dv, bias, True, 1)
             rec["ref_us_per_img"] = round(bench(lambda: refm.bwd(u, delta, A, Bm, Cm, Dv, bias, dout, x_r, True, 1), flush=flush) * 1e3 / B, 1)
-        for rb in (0, 1, 2, 4, 8):
-            if rb:
-                os.environ["VMB_SCAN_RB_BWD"] = str(rb)
+        for ss in (0, 1, 2, 4):
+            if ss:
+                os.environ["VMB_SCAN_SS_BWD"] = str(ss)
             else:
-                os.environ.pop("VMB_SCAN_RB_BWD", None)
+                os.environ.pop("VMB_SCAN_SS_BWD", None)
             ms = bench(lambda: ops.selective_scan_bwd(u, delta, A, Bm, Cm, Dv, bias, dout, ck, True), flush=flush)
-            rec[f"rb{rb}" if rb else "auto"] = round(ms * 1e3 / B, 1)
+            rec[f"ss{ss}" if ss else "auto"] = round(ms * 1e3 / B, 1)
         print(json.dumps(rec), flush=True)

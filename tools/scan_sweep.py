@@ -19,7 +19,6 @@ def main():
     ap.add_argument("--L", type=int, default=4096)
     ap.add_argument("--dtype", default="bf16")
     ap.add_argument("--ckpt", action="store_true")
-    ap.add_argument("--skew", type=int, nargs="*", default=None, help="sweep VMB_SCAN_SKEW_NS over these values (auto launch config)")
     a = ap.parse_args()
     dev = "cuda"
     dt = {"bf16": torch.bfloat16, "fp32": torch.float32}[a.dtype]
@@ -46,12 +45,7 @@ def main():
         print(json.dumps(dict(B=B, cfg="generic", us_per_img=round(ms0 * 1e3 / B, 2), GBps=round(byts / ms0 / 1e6, 1))), flush=True)
         os.environ["VMB_SCAN_TMA"] = "1"
         cfgs = [(0, 0), (2, 1), (2, 2), (2, 4), (4, 1), (4, 2), (4, 4), (8, 1), (8, 2), (8, 4)]
-        if a.skew:
-            cfgs = [(0, 0)]
-        for skew in (a.skew or [None]):
-          if skew is not None:
-            os.environ["VMB_SCAN_SKEW_NS"] = str(skew)
-          for rb, ss in cfgs:
+        for rb, ss in cfgs:
             if rb:
                 os.environ["VMB_SCAN_RB"], os.environ["VMB_SCAN_SS"] = str(rb), str(ss)
             try:
@@ -62,7 +56,7 @@ def main():
                 continue
             err = float((out.float() - ref.float()).abs().max())
             ms = bench(run, flush=flush)
-            print(json.dumps(dict(B=B, cfg=f"rb{rb}ss{ss}" if rb else "auto", skew_ns=skew, us_per_img=round(ms * 1e3 / B, 2),
+            print(json.dumps(dict(B=B, cfg=f"rb{rb}ss{ss}" if rb else "auto", us_per_img=round(ms * 1e3 / B, 2),
                                   GBps=round(byts / ms / 1e6, 1), frac=round(byts / ms / 1e6 / 6486.5, 4),
                                   speedup_vs_generic=round(ms0 / ms, 2), max_abs_diff_vs_generic=err)), flush=True)
 

@@ -47,7 +47,7 @@ class PixlinArgs(C.Structure):
         ("ln_mode", C.c_int), ("gate_mode", C.c_int), ("act_from", C.c_int), ("act_to", C.c_int),
         ("batch", C.c_int), ("K", C.c_int), ("M", C.c_int), ("P", C.c_int),
         ("x_bs", i64), ("x_cs", i64), ("r_bs", i64), ("r_cs", i64), ("o_bs", i64), ("o_cs", i64), ("g_bs", i64), ("w_ld", i64),
-        ("dtype", C.c_int), ("out_dtype", C.c_int), ("w_static", C.c_int),
+        ("dtype", C.c_int), ("out_dtype", C.c_int),
     ]
 
 

@@ -345,9 +345,6 @@ class Upsampler(nn.Sequential):
         super().__init__(*m)
 
 
-_DEFER_TAIL_BIAS = os.environ.get("VMB_TAIL_BIAS", "deferred") == "deferred"
-
-
 def fused_f32(t):
     from . import fused
     return fused._f32(t)
@@ -463,7 +460,7 @@ class MambaSISR6(_MamberUNet):
                 # a conv followed by PixelShuffle(2) runs without its bias: the permutation kernel adds it (the library conv would
                 # otherwise spend a separate elementwise pass over its (B,4C,H,W) output on the bias)
                 defer = (m.bias is not None and isinstance(nxt, nn.PixelShuffle) and nxt.upscale_factor == 2 and
-                         m.out_channels % 8 == 0 and _DEFER_TAIL_BIAS)
+                         m.out_channels % 8 == 0)
                 x = F.conv2d(x, wcl[id(m)], None if defer else m.bias, m.stride, m.padding)
                 pending_bias = fused_f32(m.bias) if defer else None
             elif isinstance(m, nn.PixelShuffle) and m.upscale_factor == 2 and x.shape[1] % 8 == 0:

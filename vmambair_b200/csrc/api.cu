@@ -125,7 +125,7 @@ extern "C" int vmb_pixlin(const vmb_pixlin_args* a, void* stream) {
     VMB_CHECK(a->gate_mode == 0 || a->gate, "pixlin: gate missing");
     PixlinParams p{a->x, a->w, a->bias, a->residual, a->out, a->ln_w, a->ln_b, a->gate, a->ln_mode, a->gate_mode,
                    a->act_from, a->act_to, a->batch, a->K, a->M, a->P, a->x_bs, a->x_cs, a->r_bs, a->r_cs, a->o_bs, a->o_cs,
-                   a->g_bs, a->w_ld > 0 ? a->w_ld : a->K, false, false, false, 2, a->w_static};
+                   a->g_bs, a->w_ld > 0 ? a->w_ld : a->K, false, false, false, 2};
     {
         const int vw = 16 / elt_size(a->dtype);
         const int64_t kpad = (a->K + 15) / 16 * 16;

@@ -81,109 +81,11 @@ __global__ void __launch_bounds__(256) dwconv3x3_kernel(const DwParams p) {
 }
 
 // Row-block version (W a power of two in [8, 256], H % 4 == 0, 16 B aligned rows): one thread = an 8-pixel strip of FOUR
-// consecutive output rows, so six 16 B row loads feed four outputs (v1: three loads per output), and the left / right halo
-// pixels come from the neighbouring lanes' vectors by shuffle instead of two scalar loads per row.  Same fmaf order as v1
-// (dy ascending, dx ascending; out-of-image taps contribute fmaf(k, 0, acc) = acc), so the results are bit-identical.
-template <typename in_t>
-__device__ __forceinline__ void dw_rows4(const in_t* __restrict__ xc, const float* __restrict__ w9, int h0, int w0, int s, int S,
-                                         int H, int W, float bias, float (*acc)[8]) {
-    constexpr int V = Vec<in_t>::N;
-#pragma unroll
-    for (int o = 0; o < 4; ++o)
-#pragma unroll
-        for (int i = 0; i < 8; ++i) acc[o][i] = bias;
-#pragma unroll
-    for (int r = 0; r < 6; ++r) {
-        const int hh = h0 - 1 + r;
-        float v[10];
-        if (hh >= 0 && hh < H) {
-            const in_t* __restrict__ row = xc + (int64_t)hh * W + w0;
-#pragma unroll
-            for (int j = 0; j < 8 / V; ++j) load_vec<in_t>(row + j * V, v + 1 + j * V, V, true);
-        } else {
-#pragma unroll
-            for (int i = 1; i <= 8; ++i) v[i] = 0.f;
-        }
-        const float left = __shfl_up_sync(0xffffffffu, v[8], 1, S), right = __shfl_down_sync(0xffffffffu, v[1], 1, S);
-        v[0] = s > 0 ? left : 0.f;
-        v[9] = s < S - 1 ? right : 0.f;
-#pragma unroll
-        for (int o = 0; o < 4; ++o) {
-            const int dy = r - 1 - o;  // input row r feeds output row o with tap row dy
-            if (dy >= -1 && dy <= 1) {
-                const float k0 = w9[(dy + 1) * 3], k1 = w9[(dy + 1) * 3 + 1], k2 = w9[(dy + 1) * 3 + 2];
-#pragma unroll
-                for (int i = 0; i < 8; ++i) acc[o][i] = fmaf(k2, v[i + 2], fmaf(k1, v[i + 1], fmaf(k0, v[i], acc[o][i])));
-            }
-        }
-    }
-}
-
-template <typename in_t>
-__global__ void __launch_bounds__(256) dwconv3x3_rows4_kernel(const DwParams p, const int S, const int log2_tpp, const long total) {
-    pdl_trigger();
-    pdl_wait();
-    constexpr int V = Vec<in_t>::N;
-    const long gt = (long)blockIdx.x * blockDim.x + threadIdx.x;
-    const bool valid = gt < total;
-    const long g = valid ? gt : total - 1;      // clamped: every lane takes part in the shuffles
-    const int plane = (int)(g >> log2_tpp), t = (int)(g & ((1L << log2_tpp) - 1));
-    const int c = plane % p.Cout, b = plane / p.Cout;
-    const int s = t & (S - 1), h0 = (t / S) * 4, w0 = s * 8;
-    const in_t* __restrict__ xb = reinterpret_cast<const in_t*>(p.x) + (int64_t)b * p.x_bs;
-    in_t* __restrict__ ob = reinterpret_cast<in_t*>(p.out) + (int64_t)b * p.o_bs + (int64_t)c * p.o_cs;
-    float w0k[9];
-#pragma unroll
-    for (int i = 0; i < 9; ++i) w0k[i] = p.w[c * 9 + i];
-    float a0[4][8];
-    dw_rows4<in_t>(xb + (int64_t)c * p.x_cs, w0k, h0, w0, s, S, p.H, p.W, p.bias ? p.bias[c] : 0.f, a0);
-    if (p.mode == 0) {
-#pragma unroll
-        for (int o = 0; o < 4; ++o)
-#pragma unroll
-            for (int i = 0; i < 8; ++i) a0[o][i] = silu2(a0[o][i]);
-    } else if (p.mode == 1) {
-#pragma unroll
-        for (int o = 0; o < 4; ++o)
-#pragma unroll
-            for (int i = 0; i < 8; ++i) a0[o][i] = gelu_exact(a0[o][i]);
-        float w1k[9];
-#pragma unroll
-        for (int i = 0; i < 9; ++i) w1k[i] = p.w[(c + p.Cout) * 9 + i];
-        float a1[4][8];
-        dw_rows4<in_t>(xb + (int64_t)(c + p.Cout) * p.x_cs, w1k, h0, w0, s, S, p.H, p.W, p.bias ? p.bias[c + p.Cout] : 0.f, a1);
-#pragma unroll
-        for (int o = 0; o < 4; ++o)
-#pragma unroll
-            for (int i = 0; i < 8; ++i) a0[o][i] *= a1[o][i];
-    }
-    if (!valid) return;
-#pragma unroll
-    for (int o = 0; o < 4; ++o)
-#pragma unroll
-        for (int j = 0; j < 8 / V; ++j) store_vec<in_t>(ob + (int64_t)(h0 + o) * p.W + w0 + j * V, a0[o] + j * V, V, true);
-    if (p.out_t != nullptr) {
-        // transposed copy: this thread's 4 rows x 8 columns are 8 runs of 4 consecutive h in the (W, H) plane; the four row blocks
-        // of a warp that share a strip fill whole 32 B sectors
-        in_t* __restrict__ ot = reinterpret_cast<in_t*>(p.out_t) + ((int64_t)b * p.Cout + c) * ((int64_t)p.H * p.W);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-            in_t* q = ot + (int64_t)(w0 + i) * p.H + h0;
-            if constexpr (sizeof(in_t) == 2) {
-                uint2 v;
-                v.x = pack2<in_t>(a0[0][i], a0[1][i]);
-                v.y = pack2<in_t>(a0[2][i], a0[3][i]);
-                *reinterpret_cast<uint2*>(q) = v;
-            } else {
-                *reinterpret_cast<float4*>(q) = make_float4(a0[0][i], a0[1][i], a0[2][i], a0[3][i]);
-            }
-        }
-    }
-}
-
-// The same row block with the loads split from the arithmetic: all six 16 B row vectors (twelve in the gated mode: both channel sets)
-// are requested before the first use, so one thread has 6-12 loads in flight instead of one row at a time (the interleaved version
-// stalls on each row load in turn).  Identical fmaf order: bit-identical results.
+// consecutive output rows, so six 16 B row loads feed four outputs (the strip kernel: three loads per output), and the left / right
+// halo pixels come from the neighbouring lanes' vectors by shuffle instead of two scalar loads per row.  The loads are split from the
+// arithmetic: all six row vectors (twelve in the gated mode: both channel sets) are requested before the first use, so one thread
+// has 6-12 loads in flight instead of stalling on each row load in turn.  Same fmaf order as the strip kernel (dy ascending, dx
+// ascending; out-of-image taps contribute fmaf(k, 0, acc) = acc), so the results are bit-identical.
 template <typename in_t>
 __device__ __forceinline__ void dw_rows4_load(const in_t* __restrict__ xc, int h0, int w0, int H, int W,
                                               uint4 (&raw)[6][8 / Vec<in_t>::N]) {
@@ -278,6 +180,8 @@ __global__ void __launch_bounds__(256, 2) dwconv3x3_rows4_pre_kernel(const DwPar
 #pragma unroll
         for (int j = 0; j < 8 / V; ++j) store_vec<in_t>(ob + (int64_t)(h0 + o) * p.W + w0 + j * V, a0[o] + j * V, V, true);
     if (p.out_t != nullptr) {
+        // transposed copy: this thread's 4 rows x 8 columns are 8 runs of 4 consecutive h in the (W, H) plane; the four row blocks
+        // of a warp that share a strip fill whole 32 B sectors
         in_t* __restrict__ ot = reinterpret_cast<in_t*>(p.out_t) + ((int64_t)b * p.Cout + c) * ((int64_t)p.H * p.W);
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
@@ -294,38 +198,30 @@ __global__ void __launch_bounds__(256, 2) dwconv3x3_rows4_pre_kernel(const DwPar
     }
 }
 
-template <typename in_t, bool PRE>
+template <typename in_t>
 static int dwconv_rows4_launch(const DwParams& p, cudaStream_t stream) {
     const int S = p.W / 8;
     const long tpp = (long)S * (p.H / 4);
     int lg = 0;
     while ((1L << lg) < tpp) ++lg;
     const long total = tpp * p.B * p.Cout;
-    if (PRE) {
-        VMB_CUDA(launch_pdl(dwconv3x3_rows4_pre_kernel<in_t>, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, stream, p, S, lg, total));
-    } else {
-        VMB_CUDA(launch_pdl(dwconv3x3_rows4_kernel<in_t>, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, stream, p, S, lg, total));
-    }
+    VMB_CUDA(launch_pdl(dwconv3x3_rows4_pre_kernel<in_t>, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, stream, p, S, lg, total));
     VMB_CUDA(cudaGetLastError());
     return VMB_OK;
 }
 
 int dwconv_launch(const DwParams& p, int dtype, cudaStream_t stream) {
     const int L = p.H * p.W;
-    {
-        const char* ve = getenv("VMB_DW_V");
-        const int version = ve ? atoi(ve) : 3;  // 1: strip kernel, 2: row-block kernel, 3 (default): row-block kernel, loads issued first
-        const int S = p.W / 8;
-        const long tpp = (long)S * (p.H / 4);
-        // W and the threads per plane powers of two (plane index by shift, halo shuffles inside one row of strips)
-        if (version >= 2 && p.vec_ok && p.W >= 8 && p.W <= 256 && (p.W & (p.W - 1)) == 0 && p.H % 4 == 0 && (tpp & (tpp - 1)) == 0) {
-            const bool pre = version == 3;  // loads of the whole row block issued before the arithmetic (VMB_DW_V=3)
-            switch (dtype) {
-                case VMB_F32: return pre ? dwconv_rows4_launch<float, true>(p, stream) : dwconv_rows4_launch<float, false>(p, stream);
-                case VMB_BF16: return pre ? dwconv_rows4_launch<__nv_bfloat16, true>(p, stream) : dwconv_rows4_launch<__nv_bfloat16, false>(p, stream);
-                case VMB_F16: return pre ? dwconv_rows4_launch<__half, true>(p, stream) : dwconv_rows4_launch<__half, false>(p, stream);
-                default: set_error("dwconv: unsupported dtype %d", dtype); return VMB_ERR_INVALID;
-            }
+    const int S = p.W / 8;
+    const long tpp = (long)S * (p.H / 4);
+    // row-block kernel where it applies: W and the threads per plane powers of two (plane index by shift, halo shuffles inside one
+    // row of strips); every other geometry takes the strip kernel
+    if (p.vec_ok && p.W >= 8 && p.W <= 256 && (p.W & (p.W - 1)) == 0 && p.H % 4 == 0 && (tpp & (tpp - 1)) == 0) {
+        switch (dtype) {
+            case VMB_F32: return dwconv_rows4_launch<float>(p, stream);
+            case VMB_BF16: return dwconv_rows4_launch<__nv_bfloat16>(p, stream);
+            case VMB_F16: return dwconv_rows4_launch<__half>(p, stream);
+            default: set_error("dwconv: unsupported dtype %d", dtype); return VMB_ERR_INVALID;
         }
     }
     const int per_thread = p.vec_ok ? 8 : 1;
@@ -497,8 +393,7 @@ int cross_scan_multi_launch(const CrossScanMulti& m, int dtype, cudaStream_t str
         vec = vec && cross_scan_vec_ok(p, dtype) && p.B == m.seg[0].B && p.H == m.seg[0].H && p.W == m.seg[0].W;
         all_same = all_same && p.src[0] == p.src[1] && p.src[0] == p.src[2] && p.src[0] == p.src[3];
     }
-    const char* ve = getenv("VMB_CROSS_SCAN_MULTI");
-    if (!vec || m.nseg == 1 || m.row_end[m.nseg - 1] > 65535 || (ve && atoi(ve) == 0)) {  // one launch per segment: same values
+    if (!vec || m.nseg == 1 || m.row_end[m.nseg - 1] > 65535) {  // one launch per segment: same values
         for (int i = 0; i < m.nseg; ++i) {
             const int rc = cross_scan_launch(m.seg[i], dtype, stream);
             if (rc != VMB_OK) return rc;
@@ -528,32 +423,26 @@ int cross_scan_multi_launch(const CrossScanMulti& m, int dtype, cudaStream_t str
 int cross_scan_launch(const CrossScanParams& p, int dtype, cudaStream_t stream) {
     dim3 grid(((p.H + 31) / 32) * ((p.W + 31) / 32), p.rows, p.B);
     VMB_CHECK(p.rows <= 65535 && p.B <= 65535, "cross_scan: too many rows / batch");
-    {
-        const int v = dtype == VMB_F32 ? 4 : 8;
-        auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
-        const char* ve = getenv("VMB_CROSS_SCAN_V");
-        const bool want = !ve || atoi(ve) != 1;
-        if (want && p.H % v == 0 && p.W % v == 0 && al16(p.src[0]) && al16(p.src[1]) && al16(p.src[2]) && al16(p.src[3]) && al16(p.out) &&
-            p.src_bs % v == 0 && p.src_rs % v == 0 && p.out_bs % v == 0 && p.out_ks % v == 0) {
-            const bool same = p.src[0] == p.src[1] && p.src[0] == p.src[2] && p.src[0] == p.src[3];
-            const size_t smem = sizeof(float) * (same ? 1 : 4) * 64 * 65;
-            dim3 gv(((p.H + 63) / 64) * ((p.W + 63) / 64), p.rows, p.B);
+    if (cross_scan_vec_ok(p, dtype)) {
+        const bool same = p.src[0] == p.src[1] && p.src[0] == p.src[2] && p.src[0] == p.src[3];
+        const size_t smem = sizeof(float) * (same ? 1 : 4) * 64 * 65;
+        dim3 gv(((p.H + 63) / 64) * ((p.W + 63) / 64), p.rows, p.B);
 #define VMB_CSV(T)                                                                                                        \
     {                                                                                                                     \
         if (smem > 48 * 1024) VMB_CUDA(cudaFuncSetAttribute(cross_scan_vec_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
         VMB_CUDA(launch_pdl(cross_scan_vec_kernel<T>, gv, dim3(256), smem, stream, p));                                    \
     }
-            switch (dtype) {
-                case VMB_F32: VMB_CSV(float) break;
-                case VMB_BF16: VMB_CSV(__nv_bfloat16) break;
-                case VMB_F16: VMB_CSV(__half) break;
-                default: set_error("cross_scan: unsupported dtype %d", dtype); return VMB_ERR_INVALID;
-            }
-#undef VMB_CSV
-            VMB_CUDA(cudaGetLastError());
-            return VMB_OK;
+        switch (dtype) {
+            case VMB_F32: VMB_CSV(float) break;
+            case VMB_BF16: VMB_CSV(__nv_bfloat16) break;
+            case VMB_F16: VMB_CSV(__half) break;
+            default: set_error("cross_scan: unsupported dtype %d", dtype); return VMB_ERR_INVALID;
         }
+#undef VMB_CSV
+        VMB_CUDA(cudaGetLastError());
+        return VMB_OK;
     }
+    // per-element kernel: H or W not a multiple of the vector width, or unaligned rows
     switch (dtype) {
         case VMB_F32: VMB_CUDA(launch_pdl(cross_scan_kernel<float>, grid, dim3(256), 0, stream, p)); break;
         case VMB_BF16: VMB_CUDA(launch_pdl(cross_scan_kernel<__nv_bfloat16>, grid, dim3(256), 0, stream, p)); break;
@@ -1160,16 +1049,9 @@ __global__ void __launch_bounds__(256) channel_branch_kernel(const ChannelParams
 // carries only the h recurrence -- exp / dt*u*B are independent of h and are hoisted eight positions ahead, the
 // per-position sum over the 16 states (a 4-stage shuffle chain per position in v1) becomes a store of h*C into
 // shared memory and one parallel reduction afterwards.
-// debug trace (VMB_CH_TRACE=1): %globaltimer of CTA 0 after each phase
-__device__ long long g_ch_trace[16];
-__device__ __forceinline__ long long ch_gtimer() {
-    long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
-}
 constexpr int CH2_THREADS = 512;
 
-__global__ void __launch_bounds__(CH2_THREADS) channel_branch_v2_kernel(const ChannelParams p, const int trace) {
+__global__ void __launch_bounds__(CH2_THREADS) channel_branch_v2_kernel(const ChannelParams p) {
     pdl_trigger();
     extern __shared__ float sm[];
     const int C = p.C, dc = p.dc, Rc = p.Rc, N = p.N, RN = Rc + 2 * N;
@@ -1188,8 +1070,6 @@ __global__ void __launch_bounds__(CH2_THREADS) channel_branch_v2_kernel(const Ch
     float* sHC = sCio + 3 * dc + 1;       // [rows][16][CP]  h * C per state
     const int b = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     constexpr int NW = CH2_THREADS / 32;
-    long long* tr = (trace && b == 0 && tid == 0) ? g_ch_trace : nullptr;
-    if (tr) tr[0] = ch_gtimer();
     for (int i = tid; i < 2 * RN * dc; i += CH2_THREADS) sXp[i] = p.xc_proj[i];
     for (int i = tid; i < 2 * dc * Rc; i += CH2_THREADS) sDw[i] = p.dtc_w[i];
     if (tid < 2 * dc) sDb[tid] = p.dtc_b[tid];
@@ -1205,12 +1085,10 @@ __global__ void __launch_bounds__(CH2_THREADS) channel_branch_v2_kernel(const Ch
     const float A2 = sact ? -__expf(p.Ac_logs[srow * N + n]) * kLog2e : 0.f;
     pdl_wait();  // the parameter staging above overlaps the tail of the merge kernels; `pooled` is read from here on
     __syncthreads();
-    if (tr) tr[1] = ch_gtimer();
     // xc = conv_cin(pool)  (per-channel affine of the pooled mean): warp j-strided rows, lanes over the sequence
     for (int j = warp; j < dc; j += NW)
         for (int l = lane; l < C; l += 32) sSeq[j * C + l] = fmaf(p.pooled[(int64_t)b * C + l] * p.inv_count, sCio[j], sCio[dc + j]);
     __syncthreads();
-    if (tr) tr[2] = ch_gtimer();
     // xc_dbl[k][c][l] = sum_j W[k][c][j] * xs[k][j][l],  xs[1] = flipped sequence
     for (int kc = warp; kc < 2 * RN; kc += NW) {
         const int k = kc >= RN;
@@ -1223,7 +1101,6 @@ __global__ void __launch_bounds__(CH2_THREADS) channel_branch_v2_kernel(const Ch
         }
     }
     __syncthreads();
-    if (tr) tr[3] = ch_gtimer();
     // dt[k][j][l] = softplus(sum_r Wdt[k][j][r] * dbl[k][r][l] + bias)
     for (int kj = warp; kj < rows; kj += NW) {
         const int k = kj / dc;
@@ -1234,7 +1111,6 @@ __global__ void __launch_bounds__(CH2_THREADS) channel_branch_v2_kernel(const Ch
         }
     }
     __syncthreads();
-    if (tr) tr[4] = ch_gtimer();
     // sequential scan: thread = (row, state n)
     if (srow < rows) {
         const int k = srow / dc, j = srow - k * dc;
@@ -1269,7 +1145,6 @@ __global__ void __launch_bounds__(CH2_THREADS) channel_branch_v2_kernel(const Ch
         }
     }
     __syncthreads();
-    if (tr) tr[5] = ch_gtimer();
     // y[row][l] = D u + sum over the 16 state slots
     for (int row = warp; row < rows; row += NW) {
         const int k = row / dc, j = row - k * dc;
@@ -1282,7 +1157,6 @@ __global__ void __launch_bounds__(CH2_THREADS) channel_branch_v2_kernel(const Ch
         }
     }
     __syncthreads();
-    if (tr) tr[6] = ch_gtimer();
     // merge directions, conv_cout, channel_norm over the C positions
     float part = 0.f;
     for (int l = tid; l < C; l += CH2_THREADS) {
@@ -1312,7 +1186,6 @@ __global__ void __launch_bounds__(CH2_THREADS) channel_branch_v2_kernel(const Ch
     }
     const float rstd = rsqrtf(block_sum(vp) / C + 1e-5f);
     for (int l = tid; l < C; l += CH2_THREADS) p.c_out[(int64_t)b * C + l] = (sOut[l] - mu) * rstd * p.cn_w[l] + p.cn_b[l];
-    if (tr) tr[7] = ch_gtimer();
 }
 
 int channel_launch(const ChannelParams& p, cudaStream_t stream) {
@@ -1324,11 +1197,9 @@ int channel_launch(const ChannelParams& p, cudaStream_t stream) {
     const int version = ve ? atoi(ve) : 2;
     const size_t smem2 = base + sizeof(float) * (size_t)2 * p.dc * 16 * (p.C | 1);
     if (version == 2 && 2 * p.dc * 16 <= CH2_THREADS && smem2 <= 227 * 1024) {
-        const char* te = getenv("VMB_CH_TRACE");
-        const int trace = te ? atoi(te) : 0;
         if (smem2 > 48 * 1024)
             VMB_CUDA(cudaFuncSetAttribute(channel_branch_v2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
-        VMB_CUDA(launch_pdl(channel_branch_v2_kernel, dim3(p.B), dim3(CH2_THREADS), smem2, stream, p, trace));
+        VMB_CUDA(launch_pdl(channel_branch_v2_kernel, dim3(p.B), dim3(CH2_THREADS), smem2, stream, p));
         VMB_CUDA(cudaGetLastError());
         return VMB_OK;
     }
@@ -1342,8 +1213,3 @@ int channel_launch(const ChannelParams& p, cudaStream_t stream) {
 }
 
 }  // namespace vmb
-
-// debug only (not part of the public header): phase stamps of CTA 0 of the last traced channel-branch launch
-extern "C" int vmb_debug_ch_trace(long long* dst, int n) {
-    return cudaMemcpyFromSymbol(dst, vmb::g_ch_trace, sizeof(long long) * (size_t)n) == cudaSuccess ? 0 : 1;
-}

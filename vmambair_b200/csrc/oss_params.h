@@ -11,7 +11,6 @@ struct PixlinParams {
     int64_t x_bs, x_cs, r_bs, r_cs, o_bs, o_cs, g_bs, w_ld;
     bool vec_ok, w_vec, w_all;
     int w_tiles;  // weight-tile buffers in smem (2 = double buffer, or every tile of the CTA when w_all)
-    int w_static; // weights / parameters may be fetched before griddepcontrol.wait (not produced by the preceding kernel)
 };
 struct DwParams {
     const void* x; const float* w; const float* bias; void* out;
@@ -65,8 +64,6 @@ struct Conv3Params {
 };
 int conv3x3_launch(const Conv3Params& p, int dtype, cudaStream_t stream);
 int pixlin_launch(const PixlinParams& p, int dtype, int out_dtype, cudaStream_t stream);
-bool pixlin_tc_applicable(const PixlinParams& p, int dtype, int out_dtype);
-int pixlin_tc_launch(const PixlinParams& p, int dtype, cudaStream_t stream);
 int dwconv_launch(const DwParams& p, int dtype, cudaStream_t stream);
 int cross_scan_launch(const CrossScanParams& p, int dtype, cudaStream_t stream);
 int cross_scan_multi_launch(const CrossScanMulti& m, int dtype, cudaStream_t stream);

@@ -565,8 +565,7 @@ static int launch2(K kern, PixlinParams p, int PT, cudaStream_t stream) {
 template <typename in_t>
 static int launch_mma(const PixlinParams& p, int out_dtype, cudaStream_t stream) {
     // 128-pixel tiles when there are enough pixels to fill the GPU with them, else 64
-    bool big = (long)((p.P + 127) / 128) * p.B >= num_sms() && pixlin_smem(p.K, 2, 128, 2) <= 100 * 1024;
-    if (const char* e = getenv("VMB_PL_PT")) big = big && atoi(e) == 128;  // tuning override
+    const bool big = (long)((p.P + 127) / 128) * p.B >= num_sms() && pixlin_smem(p.K, 2, 128, 2) <= 100 * 1024;
     const int PT = big ? 128 : 64;
     if (out_dtype == VMB_F32)
         return big ? launch2(pixlin_mma_kernel<in_t, float, 128>, p, PT, stream)
@@ -580,13 +579,13 @@ static int launch_mma(const PixlinParams& p, int out_dtype, cudaStream_t stream)
 // The data gradients W^T dY of the EFFN (2h = 510 -> C = 96) and of the folded x_proj / dt_proj (4(C + 2N) = 512 -> 96) in the
 // training path: the input (K x P) is the big operand, the output small.  The resident-K kernel above re-stages its activation tile
 // per output-channel tile and K chunk without overlap; here a CTA owns 128 output channels x 64 pixels
-// and walks K in 32-row stages through a 4-deep cp.async ring (W stage [128][32], X stage [32][64]), mma.sync m16n8k16,
-// bias / SiLU range / residual straight from the accumulators.
-constexpr int KS_MT = 128, KS_PT = 64, KS_KC = 32, KS_THREADS = 128;
+// and walks K in 32-row stages through a 6-deep cp.async ring (W stage [128][32], X stage [32][64]; the depth sets the bytes in
+// flight per SM), mma.sync m16n8k16, bias / SiLU range / residual straight from the accumulators.
+constexpr int KS_MT = 128, KS_PT = 64, KS_KC = 32, KS_THREADS = 128, KS_ST = 6;
 constexpr int KS_WP = KS_KC + 8, KS_XP = KS_PT + 8;
-constexpr size_t ks_smem(int stages) { return (size_t)stages * (KS_MT * KS_WP + KS_KC * KS_XP) * 2; }
+constexpr size_t KS_SMEM = (size_t)KS_ST * (KS_MT * KS_WP + KS_KC * KS_XP) * 2;
 
-template <typename in_t, int KS_ST>
+template <typename in_t>
 __global__ void __launch_bounds__(KS_THREADS) pixlin_kstream_kernel(const PixlinParams p) {
     pdl_trigger();
     pdl_wait();
@@ -694,21 +693,15 @@ __global__ void __launch_bounds__(KS_THREADS) pixlin_kstream_kernel(const Pixlin
         }
 }
 
-template <typename in_t, int ST>
-static int launch_kstream2(const PixlinParams& p, cudaStream_t stream) {
-    auto kern = pixlin_kstream_kernel<in_t, ST>;
-    VMB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ks_smem(ST)));
-    dim3 grid((p.P + KS_PT - 1) / KS_PT, (p.M + KS_MT - 1) / KS_MT, p.B);
-    VMB_CHECK(grid.y <= 65535, "pixlin: too many output channels");
-    VMB_CUDA(launch_pdl(kern, grid, dim3(KS_THREADS), ks_smem(ST), stream, p));
-    VMB_CUDA(cudaGetLastError());
-    return VMB_OK;
-}
 template <typename in_t>
 static int launch_kstream(const PixlinParams& p, cudaStream_t stream) {
-    int st = 6;  // ring depth: bytes in flight per SM
-    if (const char* e = getenv("VMB_KS_ST")) st = atoi(e);
-    return st == 4 ? launch_kstream2<in_t, 4>(p, stream) : launch_kstream2<in_t, 6>(p, stream);
+    auto kern = pixlin_kstream_kernel<in_t>;
+    VMB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)KS_SMEM));
+    dim3 grid((p.P + KS_PT - 1) / KS_PT, (p.M + KS_MT - 1) / KS_MT, p.B);
+    VMB_CHECK(grid.y <= 65535, "pixlin: too many output channels");
+    VMB_CUDA(launch_pdl(kern, grid, dim3(KS_THREADS), KS_SMEM, stream, p));
+    VMB_CUDA(cudaGetLastError());
+    return VMB_OK;
 }
 
 static bool kstream_applicable(const PixlinParams& p, int dtype, int out_dtype) {
@@ -736,7 +729,6 @@ int pixlin_launch(const PixlinParams& p, int dtype, int out_dtype, cudaStream_t 
     VMB_CHECK(p.ln_mode == 0 || p.K <= (dtype == VMB_F32 ? PL_KC / 2 : PL2_KC), "pixlin: LayerNorm prologue needs K <= %d",
               dtype == VMB_F32 ? PL_KC / 2 : PL2_KC);
     VMB_CHECK(p.gate_mode == 0 || p.K <= (dtype == VMB_F32 ? PL_KC / 2 : PL2_KC), "pixlin: gate prologue needs resident K");
-    if (pixlin_tc_applicable(p, dtype, out_dtype)) return pixlin_tc_launch(p, dtype, stream);  // wgmma path
     if (kstream_applicable(p, dtype, out_dtype))
         return dtype == VMB_BF16 ? launch_kstream<__nv_bfloat16>(p, stream) : launch_kstream<__half>(p, stream);
     const size_t smem = pixlin_smem(p.K, dtype == VMB_F32 ? 4 : 2);

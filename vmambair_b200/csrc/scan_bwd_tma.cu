@@ -415,8 +415,8 @@ static int launch_bt2(const ScanBwdParams& p, const ScanBwdTmaMaps& maps, int ss
 }
 
 template <typename in_t>
-static int launch_bt1(const ScanBwdParams& p, const ScanBwdTmaMaps& maps, int rb, int ss, cudaStream_t stream) {
-    return rb == 4 ? launch_bt2<in_t, 4>(p, maps, ss, stream) : launch_bt2<in_t, 2>(p, maps, ss, stream);
+static int launch_bt1(const ScanBwdParams& p, const ScanBwdTmaMaps& maps, int ss, cudaStream_t stream) {
+    return launch_bt2<in_t, 2>(p, maps, ss, stream);  // rows per warp: 2 (scan_bwd_tma_pick)
 }
 
 // (rows per warp, state split): the 255-register kernel keeps 2 CTAs x 4 warps per SM resident (2 x SMs CTAs per wave)
@@ -427,19 +427,14 @@ bool scan_bwd_tma_pick(const ScanBwdParams& p, int dtype, int& rb, int& ss) {
     if (!p.vec_ok || p.npad != 16 || p.L < 512 || p.ckpt == nullptr) return false;
     const int rpg = p.rows_per_group;
     const long rows = (long)p.batch * p.dim;
-    // RB = 2 at every batch; the state split while the CTAs still fit one resident wave (tools/scan_bwd_sweep.py sweeps both)
+    // RB = 2 at every batch; the state split while the CTAs still fit one resident wave (tools/scan_bwd_sweep.py sweeps it)
     rb = 2;
     ss = 1;
     while (ss < 4 && rows / (rb * 4 / ss) * 2 <= 2L * num_sms()) ss <<= 1;
-    if (const char* v = getenv("VMB_SCAN_RB_BWD")) {
-        const int x = atoi(v);
-        if (x == 2 || x == 4) rb = x;
-    }
     if (const char* v = getenv("VMB_SCAN_SS_BWD")) {
         const int x = atoi(v);
         if (x == 1 || x == 2 || x == 4) ss = x;
     }
-    while (rb > 2 && rpg % (rb * 4 / ss) != 0) rb >>= 1;
     return rpg % (rb * 4 / ss) == 0;
 }
 
@@ -458,9 +453,9 @@ int scan_bwd_tma_launch(const ScanBwdParams& p, int dtype, int rb, int ss, cudaS
     if ((rc = make_tmap_4d(&maps.b, dtype, p.Bm, dbc, sb, box_bc)) != VMB_OK) return rc;
     if ((rc = make_tmap_4d(&maps.c, dtype, p.Cm, dbc, sc, box_bc)) != VMB_OK) return rc;
     switch (dtype) {
-        case VMB_F32: return launch_bt1<float>(p, maps, rb, ss, stream);  // 130 KB of tiles: one CTA per SM
-        case VMB_BF16: return launch_bt1<__nv_bfloat16>(p, maps, rb, ss, stream);
-        case VMB_F16: return launch_bt1<__half>(p, maps, rb, ss, stream);
+        case VMB_F32: return launch_bt1<float>(p, maps, ss, stream);  // 130 KB of tiles: one CTA per SM
+        case VMB_BF16: return launch_bt1<__nv_bfloat16>(p, maps, ss, stream);
+        case VMB_F16: return launch_bt1<__half>(p, maps, ss, stream);
     }
     set_error("selective_scan_bwd: unsupported dtype %d", dtype);
     return VMB_ERR_INVALID;

@@ -35,28 +35,7 @@ struct TmaCfg {
 };
 
 // MODE 0: plain operator   1: plain + checkpoints (training forward)   2: per-group sources, reversed walk (fused OSS block)
-// 2^x for a packed pair on the FMA pipe (x <= 0): magic-number split x = n + f, |f| <= 0.5, degree-5 minimax polynomial
-// (max relative error 2.3e-7 in fp32 Horner form -- the level of MUFU.EX2's 2 ulp), exponent patched in by integer add.
-// MUFU, LDS and SHFL instructions queue on one dispatch path (tools/microbench.cu) which bounds this kernel; the FMA pipe has
-// slack, so a fixed subset of the decay factors is evaluated here instead of on the XU.
-__device__ __forceinline__ float2 exp2_poly2(float2 x) {
-    x.x = fmaxf(x.x, -126.f);
-    x.y = fmaxf(x.y, -126.f);
-    const float2 t = add2(x, make_float2(12582912.f, 12582912.f));       // 1.5 * 2^23: round(x) lands in the low mantissa bits
-    const float2 n = add2(t, make_float2(-12582912.f, -12582912.f));
-    const float2 f = fma2(n, make_float2(-1.f, -1.f), x);
-    float2 q = fma2(f, make_float2(0.00132763443980366f, 0.00132763443980366f), make_float2(0.009675498120486736f, 0.009675498120486736f));
-    q = fma2(q, f, make_float2(0.05550713092088699f, 0.05550713092088699f));
-    q = fma2(q, f, make_float2(0.24022120237350464f, 0.24022120237350464f));
-    q = fma2(q, f, make_float2(0.6931469440460205f, 0.6931469440460205f));
-    q = fma2(q, f, make_float2(1.0000001192092896f, 1.0000001192092896f));
-    return make_float2(__int_as_float(__float_as_int(q.x) + (__float_as_int(t.x) << 23)),
-                       __int_as_float(__float_as_int(q.y) + (__float_as_int(t.y) << 23)));
-}
-// positions of a lane's 16 whose decay factors take the polynomial (6 of 16) when POLY is set
-__host__ __device__ constexpr bool poly_pos(int poly, int t) { return poly && (t % 8 == 2 || t % 8 == 5 || t % 8 == 7); }
-
-template <typename in_t, int RB, int NW, int SS, int MODE, int POLY>
+template <typename in_t, int RB, int NW, int SS, int MODE>
 __global__ void __launch_bounds__(32 * NW, NW == 8 ? 2 : 3)
     scan_fwd_tma_kernel(const ScanFwdParams p, const __grid_constant__ ScanTmaMaps maps) {
     pdl_trigger();
@@ -227,8 +206,8 @@ __global__ void __launch_bounds__(32 * NW, NW == 8 ? 2 : 3)
                 const float4 Bq = bq[t / 2];
                 const float2 e0 = mul2(A2, make_float2(dt[t], dt[t]));
                 const float2 e1 = mul2(A2, make_float2(dt[t + 1], dt[t + 1]));
-                a2[t] = poly_pos(POLY, t) ? exp2_poly2(e0) : make_float2(ex2(e0.x), ex2(e0.y));
-                a2[t + 1] = poly_pos(POLY, t + 1) ? exp2_poly2(e1) : make_float2(ex2(e1.x), ex2(e1.y));
+                a2[t] = make_float2(ex2(e0.x), ex2(e0.y));
+                a2[t + 1] = make_float2(ex2(e1.x), ex2(e1.y));
                 hend = fma2(a2[t], hend, mul2(make_float2(dtu[t], dtu[t]), make_float2(Bq.x, Bq.y)));
                 hend = fma2(a2[t + 1], hend, mul2(make_float2(dtu[t + 1], dtu[t + 1]), make_float2(Bq.z, Bq.w)));
             }
@@ -273,12 +252,12 @@ __global__ void __launch_bounds__(32 * NW, NW == 8 ? 2 : 3)
                     h = fma2(a2[t], h, mul2(du0, make_float2(Bq.x, Bq.y)));
                     y[t] = fmaf(h.y, Cq.y, fmaf(h.x, Cq.x, y[t]));
                     const float2 e0 = mul2(A2n, make_float2(dt[t], dt[t]));
-                    a2[t] = poly_pos(POLY, t) ? exp2_poly2(e0) : make_float2(ex2(e0.x), ex2(e0.y));
+                    a2[t] = make_float2(ex2(e0.x), ex2(e0.y));
                     hn = fma2(a2[t], hn, mul2(du0, make_float2(Bn.x, Bn.y)));
                     h = fma2(a2[t + 1], h, mul2(du1, make_float2(Bq.z, Bq.w)));
                     y[t + 1] = fmaf(h.y, Cq.w, fmaf(h.x, Cq.z, y[t + 1]));
                     const float2 e1 = mul2(A2n, make_float2(dt[t + 1], dt[t + 1]));
-                    a2[t + 1] = poly_pos(POLY, t + 1) ? exp2_poly2(e1) : make_float2(ex2(e1.x), ex2(e1.y));
+                    a2[t + 1] = make_float2(ex2(e1.x), ex2(e1.y));
                     hn = fma2(a2[t + 1], hn, mul2(du1, make_float2(Bn.z, Bn.w)));
                 }
                 hend = hn;
@@ -380,10 +359,10 @@ int make_tmap_4d(CUtensorMap* map, int dtype, const void* base, const uint64_t d
     return VMB_OK;
 }
 
-template <typename in_t, int RB, int NW, int SS, int MODE, int POLY>
-static int launch_tma5(const ScanFwdParams& p, const ScanTmaMaps& maps, cudaStream_t stream) {
+template <typename in_t, int RB, int NW, int SS, int MODE>
+static int launch_tma4(const ScanFwdParams& p, const ScanTmaMaps& maps, cudaStream_t stream) {
     using K = TmaCfg<in_t, RB, NW, SS>;
-    auto kern = scan_fwd_tma_kernel<in_t, RB, NW, SS, MODE, POLY>;
+    auto kern = scan_fwd_tma_kernel<in_t, RB, NW, SS, MODE>;
     constexpr size_t smem = K::smem_bytes + 128;  // + alignment slack
     static_assert(smem <= 227 * 1024, "scan_fwd_tma: shared memory");
     VMB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -391,18 +370,6 @@ static int launch_tma5(const ScanFwdParams& p, const ScanTmaMaps& maps, cudaStre
     VMB_CUDA(launch_pdl(kern, dim3((unsigned)blocks), dim3(32 * NW), smem, stream, p, maps));
     VMB_CUDA(cudaGetLastError());
     return VMB_OK;
-}
-
-// POLY = 1 (6 of 16 decay factors per lane-chunk by exp2_poly2 on the FMA pipe) is an EXPERIMENT, off by default: the FMA pipe /
-// issue slots have less slack than the pipe-utilisation counters suggest.  Build with -DVMB_SCAN_POLY_VARIANT and set
-// VMB_SCAN_POLY=1 to measure it.
-template <typename in_t, int RB, int NW, int SS, int MODE>
-static int launch_tma4(const ScanFwdParams& p, const ScanTmaMaps& maps, cudaStream_t stream) {
-#ifdef VMB_SCAN_POLY_VARIANT
-    const char* e = getenv("VMB_SCAN_POLY");
-    if (e && atoi(e) == 1) return launch_tma5<in_t, RB, NW, SS, MODE, 1>(p, maps, stream);
-#endif
-    return launch_tma5<in_t, RB, NW, SS, MODE, 0>(p, maps, stream);
 }
 
 template <typename in_t, int RB, int NW, int SS>
@@ -424,8 +391,8 @@ static int launch_tma2(const ScanFwdParams& p, const ScanTmaMaps& maps, int ss, 
 }
 
 template <typename in_t>
-static int launch_tma1(const ScanFwdParams& p, const ScanTmaMaps& maps, int rb, int ss, cudaStream_t stream) {
-    (void)rb;  // rows per warp: 2 (tools/scan_sweep.py: RB = 4 / 8 lose at every batch size; not instantiated)
+static int launch_tma1(const ScanFwdParams& p, const ScanTmaMaps& maps, int ss, cudaStream_t stream) {
+    // rows per warp: 2 (scan_fwd_tma_pick; tools/scan_sweep.py: RB = 4 / 8 lose at every batch size, not instantiated)
     return launch_tma2<in_t, 2>(p, maps, ss, stream);
 }
 
@@ -447,7 +414,6 @@ bool scan_fwd_tma_pick(const ScanFwdParams& p, int& rb, int& ss) {
         const int x = atoi(v);
         if (x == 1 || x == 2 || x == 4) ss = x;
     }
-    while (rb > 2 && rpg % (rb * kTmaWarps / ss) != 0) rb >>= 1;
     return rpg % (rb * kTmaWarps / ss) == 0;
 }
 
@@ -481,9 +447,9 @@ int scan_fwd_tma_launch(const ScanFwdParams& p_in, int dtype, int rb, int ss, cu
         if ((rc = make_tmap_4d(&maps.c[0], dtype, p.Cm, dbc, sc, box_bc)) != VMB_OK) return rc;
     }
     switch (dtype) {
-        case VMB_F32: return launch_tma1<float>(p, maps, rb, ss, stream);
-        case VMB_BF16: return launch_tma1<__nv_bfloat16>(p, maps, rb, ss, stream);
-        case VMB_F16: return launch_tma1<__half>(p, maps, rb, ss, stream);
+        case VMB_F32: return launch_tma1<float>(p, maps, ss, stream);
+        case VMB_BF16: return launch_tma1<__nv_bfloat16>(p, maps, ss, stream);
+        case VMB_F16: return launch_tma1<__half>(p, maps, ss, stream);
     }
     set_error("selective_scan_fwd: unsupported dtype %d", dtype);
     return VMB_ERR_INVALID;

@@ -12,8 +12,6 @@ No CPU path, no silent fallback: every stage goes through the C-ABI and raises o
 """
 from __future__ import annotations
 
-import os
-
 import torch
 
 from . import ops
@@ -22,7 +20,6 @@ _DTYPES = (torch.float32, torch.bfloat16, torch.float16)
 
 
 _warned = set()
-_DW_T = os.environ.get("VMB_DW_T", "1") == "1"  # depthwise conv writes the transposed copy itself (0: separate vmb_transpose_hw pass)
 
 
 def unsupported_reason(block, x: torch.Tensor):
@@ -121,26 +118,22 @@ def block_forward(block, x: torch.Tensor, out: torch.Tensor = None) -> torch.Ten
     N = c["N"]
     x3 = x.contiguous().view(B, C, L)
     # norm1 + in_conv; SiLU on the z half
-    xz = ops.pixlin(x3, c["w_in"], c["b_in"], ln=c["ln1"], act=(C, 2 * C), static_w=True)
-    grouped = L % 8 == 0 and os.environ.get("VMB_FUSED_SCAN", "grouped") == "grouped"
-    if grouped and _DW_T:
+    xz = ops.pixlin(x3, c["w_in"], c["b_in"], ln=c["ln1"], act=(C, 2 * C))
+    if L % 8 == 0:
         xc, xt = ops.dwconv3x3_t(xz[:, :C], c["dw"], c["dw_b"], C, H, W)  # x and its (W,H) copy from one launch
-    else:
-        xc = ops.dwconv3x3(xz[:, :C], c["dw"], c["dw_b"], C, H, W, 0)
-    if grouped:
         # direction-aware scan: directions 0/2 read x and the GEMM on x, 1/3 read the transposed copies; reversed
         # directions walk the same memory backwards -- no gathered / flipped (B,4C,L) operands exist
-        if not _DW_T:
-            xt = ops.transpose_hw(xc, H, W)
-        d02 = ops.pixlin(xc, c["w_big02"], static_w=True).view(B, 2, C + 2 * N, L)
-        d13 = ops.pixlin(xt, c["w_big13"], static_w=True).view(B, 2, C + 2 * N, L)
+        d02 = ops.pixlin(xc, c["w_big02"]).view(B, 2, C + 2 * N, L)
+        d13 = ops.pixlin(xt, c["w_big13"]).view(B, 2, C + 2 * N, L)
         src = [(xc, d02[:, 0]), (xt, d13[:, 0]), (xc, d02[:, 1]), (xt, d13[:, 1])]
         ys = ops.selective_scan_fwd_grouped([s[0] for s in src], [s[1][:, :C] for s in src], [s[1][:, C:C + N] for s in src],
                                             [s[1][:, C + N:] for s in src], [0, 0, 1, 1], c["A"], c["Ds"], c["dt_bias"], True)
         y2, pooled = ops.merge_norm_gate(ys, xz[:, C:], c["on_w"], c["on_b"], C, H, W, in_place_order=True)
         return _block_tail(c, x3, y2, pooled, B, C, H, W, out)
+    # L % 8 != 0: the gathered path
+    xc = ops.dwconv3x3(xz[:, :C], c["dw"], c["dw_b"], C, H, W, 0)
     # delta (dt_proj o x_proj), B, C of the four directions from one GEMM on the un-permuted x
-    dbl = ops.pixlin(xc, c["w_big"], static_w=True)  # (B, 4*(C+2N), L)
+    dbl = ops.pixlin(xc, c["w_big"])  # (B, 4*(C+2N), L)
     dbl4 = dbl.view(B, 4, C + 2 * N, L)
     xs = ops.cross_scan([xc] * 4, C, H, W)
     dts = ops.cross_scan([dbl4[:, k, :C] for k in range(4)], C, H, W)
@@ -154,12 +147,12 @@ def block_forward(block, x: torch.Tensor, out: torch.Tensor = None) -> torch.Ten
 def _block_tail(c, x3, y2, pooled, B, C, H, W, dst=None):
     L = H * W
     cg = ops.channel_branch(pooled, 1.0 / L, c["ch"], C)
-    x1 = ops.pixlin(y2, c["w_out"], c["b_out"], residual=x3, gate=cg, gate_mode=c["gate_mode"], static_w=True)
-    t = ops.pixlin(x1, c["w_pin"], c["b_pin"], ln=c["ln2"], static_w=True)
+    x1 = ops.pixlin(y2, c["w_out"], c["b_out"], residual=x3, gate=cg, gate_mode=c["gate_mode"])
+    t = ops.pixlin(x1, c["w_pin"], c["b_pin"], ln=c["ln2"])
     g = ops.dwconv3x3(t, c["fdw"], c["fdw_b"], c["h"], H, W, 1)
     if dst is not None:
         assert dst.shape == (B, C, H, W) and dst.stride(3) == 1 and dst.stride(2) == W and dst.stride(1) == L
-        ops.pixlin(g, c["w_pout"], c["b_pout"], residual=x1, static_w=True, out=dst.view(B, C, L))
+        ops.pixlin(g, c["w_pout"], c["b_pout"], residual=x1, out=dst.view(B, C, L))
         return dst
-    out = ops.pixlin(g, c["w_pout"], c["b_pout"], residual=x1, static_w=True)
+    out = ops.pixlin(g, c["w_pout"], c["b_pout"], residual=x1)
     return out.view(B, C, H, W)

@@ -151,12 +151,10 @@ def _run(name, args, t, tag, nbytes=0, kernels=1):
         _lib.check(fn(C.byref(args), _stream(t)), name)
 
 
-def pixlin(x, w, bias=None, residual=None, ln=None, gate=None, gate_mode=0, act=(0, 0), out_dtype=None, out=None, static_w=False):
+def pixlin(x, w, bias=None, residual=None, ln=None, gate=None, gate_mode=0, act=(0, 0), out_dtype=None, out=None):
     """out[b,m,p] = epi(sum_k w[m,k] pro(x)[b,k,p]).  x: (B,K,P) view with stride(-1)==1; w: (M,>=K) x.dtype, rows may be
     zero-padded to a multiple of 16 (pad_weight) for vector loads.
-    ln = (mode, weight_fp32, bias_fp32|None); gate: (B,K) fp32; residual: (B,M,P) view.
-    static_w: w / bias / ln parameters were written long before this call (cached inference weights), so the kernel may fetch them
-    while the preceding kernel of the stream is still running; leave False when they are that kernel's output."""
+    ln = (mode, weight_fp32, bias_fp32|None); gate: (B,K) fp32; residual: (B,M,P) view."""
     B, K, P = x.shape
     M = w.shape[0]
     assert w.shape[1] >= K and w.dtype == x.dtype and w.stride(1) == 1 and x.stride(2) == 1
@@ -169,7 +167,7 @@ def pixlin(x, w, bias=None, residual=None, ln=None, gate=None, gate_mode=0, act=
         ln_mode, gate_mode if gate is not None else 0, act[0], act[1], B, K, M, P,
         x.stride(0), x.stride(1), residual.stride(0) if residual is not None else 0,
         residual.stride(1) if residual is not None else 0, out.stride(0), out.stride(1),
-        gate.stride(0) if gate is not None else 0, w.stride(0), _DT[x.dtype], _DT[out_dtype], int(static_w))
+        gate.stride(0) if gate is not None else 0, w.stride(0), _DT[x.dtype], _DT[out_dtype])
     _run("vmb_pixlin", a, x, "pixlin", 0)
     return out
 

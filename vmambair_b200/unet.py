@@ -73,7 +73,7 @@ def conv1x1(conv: nn.Conv2d, x):
     """reduce_chan_level*: 1x1 conv over the (contiguous) concatenation buffer"""
     w, bias = _cached(conv, x.dtype, "1x1")
     B, K, H, W = x.shape
-    return ops.pixlin(x.contiguous().view(B, K, H * W), w, bias, static_w=True).view(B, conv.out_channels, H, W)
+    return ops.pixlin(x.contiguous().view(B, K, H * W), w, bias).view(B, conv.out_channels, H, W)
 
 
 def run_stage(stage: nn.Sequential, x, out=None):
