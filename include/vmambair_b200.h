@@ -64,7 +64,11 @@ int vmb_selective_scan_fwd(const vmb_scan_fwd_args* a, void* stream);
  * L-1-l for u, delta, B, C and out), so the four scan orders of cross_scan_2d
  * (SRGAN/VmambaIR/archs/MambaSISR6_arch.py:401-404) need no flipped / gathered copies: directions 0,2 read the
  * natural (H,W) tensors, directions 1,3 the (W,H)-transposed ones.  Strides are shared by the groups; u/delta/out
- * rows are indexed inside the group.  Requires 16 B-aligned rows (seqlen % 8 == 0 for 16-bit I/O), dstate <= 16. */
+ * rows are indexed inside the group.  Requires 16 B-aligned rows (seqlen % 8 == 0 for 16-bit I/O), dstate <= 16.
+ *   ckpt : NULL (inference), or fp32 (batch, dim, n_ckpt, dstate) as written by vmb_selective_scan_fwd, indexed by SEQUENCE
+ *          position: a reversed group's checkpoints equal the flat forward's on the flipped copy (`out` is the same as without
+ *          checkpoints, except that shapes left to the generic kernel run it at <= 2 rows per warp, which may change rounding).  Training forward of
+ *          cross_selective_scan (RealSR/VmambaIR/archs/MambaRealSR11_arch.py:371-434; CrossScan :325-343 + SelectiveScan fwd). */
 typedef struct {
     const void* u[4]; const void* delta[4]; const void* Bm[4]; const void* Cm[4]; void* out[4]; int rev[4];
     const float* A; const float* D; const float* delta_bias;   /* (dim, dstate), (dim), (dim): indexed by g*rows+r */
@@ -72,6 +76,7 @@ typedef struct {
     int64_t u_bs, u_ds, delta_bs, delta_ds, out_bs, out_ds, B_bs, B_ns, C_bs, C_ns;
     int delta_softplus;
     int dtype;
+    float* ckpt;
 } vmb_scan_grouped_args;
 int vmb_selective_scan_fwd_grouped(const vmb_scan_grouped_args* a, void* stream);
 
@@ -99,6 +104,29 @@ typedef struct {
 } vmb_scan_bwd_args;
 int vmb_selective_scan_bwd(const vmb_scan_bwd_args* a, void* stream);
 int64_t vmb_scan_bwd_workspace_bytes(int batch, int ngroups, int dstate, int seqlen);
+
+/* Direction-aware backward, the adjoint of vmb_selective_scan_fwd_grouped: group g (<= 4) reads u, delta, Bm, Cm, dout from its own
+ * tensors and writes du, ddelta (batch, rows, seqlen) and dB, dC (batch, dstate, seqlen) to its own destinations, every one in the
+ * memory order of that group's sources (rev[g] != 0: sequence position l <-> memory index L-1-l).  Same values as
+ * vmb_selective_scan_bwd on the gathered / flipped copies followed by scattering the results back -- what CrossScan.backward +
+ * SelectiveScan.backward compute (RealSR/VmambaIR/archs/MambaRealSR11_arch.py:295-343) without the four gathered copies.
+ *   dA (dim,dstate), dD (dim), ddelta_bias (dim): fp32, indexed by g*rows+r, ACCUMULATED into (caller zero-fills)
+ *   workspace : vmb_scan_bwd_workspace_bytes(batch, ngroups, dstate, seqlen) bytes, 16 B aligned, zero-filled by the library
+ *   ckpt : as written by vmb_selective_scan_fwd_grouped (required when seqlen > interval)
+ * Strides are shared by the groups.  Requires 16 B-aligned rows of u, delta, Bm, Cm, dout, du, ddelta (seqlen % 8 == 0 for
+ * 16-bit I/O, % 4 for fp32) and dstate <= 16; dB / dC need no alignment.  Anything else returns VMB_ERR_INVALID. */
+typedef struct {
+    const void* u[4]; const void* delta[4]; const void* Bm[4]; const void* Cm[4]; const void* dout[4];
+    void* du[4]; void* ddelta[4]; void* dB[4]; void* dC[4]; int rev[4];
+    const float* A; const float* D; const float* delta_bias; const float* ckpt;
+    float* dA; float* dD; float* ddelta_bias; void* workspace;
+    int batch, dim, seqlen, dstate, ngroups;
+    int64_t u_bs, u_ds, delta_bs, delta_ds, dout_bs, dout_ds, du_bs, du_ds, ddelta_bs, ddelta_ds;
+    int64_t B_bs, B_ns, C_bs, C_ns, dB_bs, dB_ns, dC_bs, dC_ns;
+    int delta_softplus;
+    int dtype;
+} vmb_scan_grouped_bwd_args;
+int vmb_selective_scan_bwd_grouped(const vmb_scan_grouped_bwd_args* a, void* stream);
 
 
 /* ---- B1 module boundary: fused stages of one OSS block (inference) -------------------------------
@@ -214,6 +242,10 @@ typedef struct {
 } vmb_merge_args;
 int vmb_merge_norm_gate(const vmb_merge_args* a, void* stream);
 int64_t vmb_merge_workspace_bytes(int batch, int C, int H, int W);
+/* the inverse orders + 4-way fp32 sum alone (CrossMerge.forward, RealSR/VmambaIR/archs/MambaRealSR11_arch.py:346-355): out fp32 (batch,
+ * C, H*W) dense, same values as the merged sum of vmb_merge_norm_gate.  Uses a->ys, batch, C, H, W, in_place_order, dtype and the
+ * workspace (per-pixel statistics); z, ln_w, ln_b, y2, pooled are ignored. */
+int vmb_merge_sum(const vmb_merge_args* a, float* out, void* stream);
 
 /* the channel-direction OSS for one image per CTA (cforward_corev1 :438-483; Mamber32/33 and RealSR variants):
  * pooled means -> conv_cin -> xc_proj / dtc_proj -> bidirectional selective scan over L=C -> conv_cout ->

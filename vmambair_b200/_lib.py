@@ -101,6 +101,20 @@ class ScanGroupedArgs(C.Structure):
         ("batch", C.c_int), ("dim", C.c_int), ("seqlen", C.c_int), ("dstate", C.c_int), ("ngroups", C.c_int),
         ("u_bs", i64), ("u_ds", i64), ("delta_bs", i64), ("delta_ds", i64), ("out_bs", i64), ("out_ds", i64),
         ("B_bs", i64), ("B_ns", i64), ("C_bs", i64), ("C_ns", i64),
+        ("delta_softplus", C.c_int), ("dtype", C.c_int), ("ckpt", vp),
+    ]
+
+
+class ScanGroupedBwdArgs(C.Structure):
+    _fields_ = [
+        ("u", vp * 4), ("delta", vp * 4), ("Bm", vp * 4), ("Cm", vp * 4), ("dout", vp * 4),
+        ("du", vp * 4), ("ddelta", vp * 4), ("dB", vp * 4), ("dC", vp * 4), ("rev", C.c_int * 4),
+        ("A", vp), ("D", vp), ("delta_bias", vp), ("ckpt", vp),
+        ("dA", vp), ("dD", vp), ("ddelta_bias", vp), ("workspace", vp),
+        ("batch", C.c_int), ("dim", C.c_int), ("seqlen", C.c_int), ("dstate", C.c_int), ("ngroups", C.c_int),
+        ("u_bs", i64), ("u_ds", i64), ("delta_bs", i64), ("delta_ds", i64), ("dout_bs", i64), ("dout_ds", i64),
+        ("du_bs", i64), ("du_ds", i64), ("ddelta_bs", i64), ("ddelta_ds", i64),
+        ("B_bs", i64), ("B_ns", i64), ("C_bs", i64), ("C_ns", i64), ("dB_bs", i64), ("dB_ns", i64), ("dC_bs", i64), ("dC_ns", i64),
         ("delta_softplus", C.c_int), ("dtype", C.c_int),
     ]
 
@@ -193,6 +207,8 @@ SYMBOLS = {
     "vmb_cross_scan_multi": (C.c_int, [C.POINTER(CrossScanArgs), C.c_int, vp]),
     "vmb_dwconv3x3_t": (C.c_int, [C.POINTER(DwconvArgs), vp, vp]),
     "vmb_selective_scan_fwd_grouped": (C.c_int, [C.POINTER(ScanGroupedArgs), vp]),
+    "vmb_selective_scan_bwd_grouped": (C.c_int, [C.POINTER(ScanGroupedBwdArgs), vp]),
+    "vmb_merge_sum": (C.c_int, [C.POINTER(MergeArgs), vp, vp]),
     "vmb_channel_branch": (C.c_int, [C.POINTER(ChannelArgs), vp]),
     "vmb_layernorm_fwd": (C.c_int, [C.POINTER(LnFwdArgs), vp]),
     "vmb_layernorm_bwd": (C.c_int, [C.POINTER(LnBwdArgs), vp]),

@@ -262,6 +262,16 @@ class SS2D_1(nn.Module):
         y2 = y2 * c + y2 if self.gate == "mul" else y2 + c
         return self.out_conv(y2)
 
+    def forward_corev2(self, x: torch.Tensor, nrows=-1, channel_first=False):
+        """the four-direction scan of this module as the reference's forward_corev2 (RealSR/VmambaIR/archs/MambaRealSR11_arch.py:791-804):
+        x (B,H,W,D) channels-last, or (B,D,H,W) when channel_first -> out_norm(merged scan output) (B,D,H,W), differentiable, on the
+        library's direction-aware kernels (cross_scan.cross_selective_scan).  Nothing calls it by default, as in the reference."""
+        from .cross_scan import cross_selective_scan
+        if not channel_first:
+            x = x.permute(0, 3, 1, 2).contiguous()
+        return cross_selective_scan(x, self.x_proj_weight, None, self.dt_projs_weight, self.dt_projs_bias, self.A_logs, self.Ds,
+                                    self.out_norm, self.softmax_version, nrows=nrows, delta_softplus=True)
+
     def forward(self, x: torch.Tensor, **kwargs):
         return self.forward_compose(x)
 

@@ -206,6 +206,15 @@ extern "C" int vmb_merge_norm_gate(const vmb_merge_args* a, void* stream) {
     return merge_launch(p, a->dtype, static_cast<cudaStream_t>(stream));
 }
 
+extern "C" int vmb_merge_sum(const vmb_merge_args* a, float* out, void* stream) {
+    VMB_CHECK(a && a->ys && out, "merge_sum: null pointer");
+    VMB_CHECK(dt_ok(a->dtype), "merge_sum: bad dtype");
+    VMB_CHECK(a->batch > 0 && a->batch <= 65535 && a->C > 0 && a->H > 0 && a->W > 0, "merge_sum: bad sizes");
+    VMB_CHECK(a->workspace && aligned16(a->workspace), "merge_sum: 16 B-aligned workspace of vmb_merge_workspace_bytes() required");
+    MergeParams p{a->ys, nullptr, nullptr, nullptr, nullptr, nullptr, a->batch, a->C, a->H, a->W, 0, 0, a->in_place_order, a->workspace, 0, 0};
+    return merge_sum_launch(p, out, a->dtype, static_cast<cudaStream_t>(stream));
+}
+
 extern "C" int vmb_channel_branch(const vmb_channel_args* a, void* stream) {
     VMB_CHECK(a && a->pooled && a->xc_proj && a->dtc_w && a->dtc_b && a->Ac_logs && a->Dsc && a->cn_w && a->cn_b && a->c_out,
               "channel_branch: null pointer");
@@ -267,11 +276,11 @@ extern "C" int vmb_selective_scan_fwd_grouped(const vmb_scan_grouped_args* a, vo
               "scan_fwd_grouped: bad sizes (dstate <= 16)");
     VMB_CHECK(a->A != nullptr, "scan_fwd_grouped: A missing");
     ScanFwdParams p{};
-    p.A = a->A; p.D = a->D; p.bias = a->delta_bias; p.ckpt = nullptr;
+    p.A = a->A; p.D = a->D; p.bias = a->delta_bias; p.ckpt = a->ckpt;
     p.batch = a->batch; p.dim = a->dim; p.L = a->seqlen; p.N = a->dstate; p.G = a->ngroups;
     p.npad = 16;
     p.rows_per_group = a->dim / a->ngroups;
-    p.n_ckpt = 0;
+    p.n_ckpt = (a->seqlen + kScanCkpt - 1) / kScanCkpt;
     p.u_bs = a->u_bs; p.u_ds = a->u_ds; p.dl_bs = a->delta_bs; p.dl_ds = a->delta_ds; p.o_bs = a->out_bs; p.o_ds = a->out_ds;
     p.B_bs = a->B_bs; p.B_gs = 0; p.B_ns = a->B_ns; p.C_bs = a->C_bs; p.C_gs = 0; p.C_ns = a->C_ns;
     p.softplus = a->delta_softplus;
@@ -287,4 +296,49 @@ extern "C" int vmb_selective_scan_fwd_grouped(const vmb_scan_grouped_args* a, vo
     }
     p.vec_ok = ok;
     return scan_fwd_launch(p, a->dtype, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vmb_selective_scan_bwd_grouped(const vmb_scan_grouped_bwd_args* a, void* stream) {
+    VMB_CHECK(a != nullptr, "selective_scan_bwd_grouped: null args");
+    VMB_CHECK(dt_ok(a->dtype), "selective_scan_bwd_grouped: dtype must be f32/bf16/f16 (got %d)", a->dtype);
+    VMB_CHECK(a->ngroups >= 1 && a->ngroups <= 4 && a->dim % a->ngroups == 0, "selective_scan_bwd_grouped: 1..4 groups dividing dim");
+    VMB_CHECK(a->batch > 0 && a->batch <= 65535 && a->dim > 0 && a->seqlen > 0 && a->dstate > 0 && a->dstate <= 16,
+              "selective_scan_bwd_grouped: bad sizes (dstate <= 16)");
+    VMB_CHECK(a->A && a->dA && a->workspace, "selective_scan_bwd_grouped: A, dA or workspace missing");
+    VMB_CHECK(a->ckpt != nullptr || a->seqlen <= kScanCkpt,
+              "selective_scan_bwd_grouped: forward checkpoints required when seqlen > %d", kScanCkpt);
+    VMB_CHECK(aligned16(a->workspace), "selective_scan_bwd_grouped: workspace must be 16-byte aligned");
+    VMB_CHECK((a->D == nullptr) == (a->dD == nullptr), "selective_scan_bwd_grouped: D and dD must both be given or both be NULL");
+    VMB_CHECK((a->delta_bias == nullptr) == (a->ddelta_bias == nullptr),
+              "selective_scan_bwd_grouped: delta_bias and ddelta_bias must both be given or both be NULL");
+    ScanBwdParams p{};
+    p.A = a->A; p.D = a->D; p.bias = a->delta_bias; p.ckpt = a->ckpt;
+    p.dA = a->dA; p.dD = a->dD; p.dbias = a->ddelta_bias; p.dBC = static_cast<float*>(a->workspace);
+    p.batch = a->batch; p.dim = a->dim; p.L = a->seqlen; p.N = a->dstate; p.G = a->ngroups;
+    p.npad = 16;
+    p.rows_per_group = a->dim / a->ngroups;
+    p.n_ckpt = (a->seqlen + kScanCkpt - 1) / kScanCkpt;
+    p.u_bs = a->u_bs; p.u_ds = a->u_ds; p.dl_bs = a->delta_bs; p.dl_ds = a->delta_ds; p.do_bs = a->dout_bs; p.do_ds = a->dout_ds;
+    p.du_bs = a->du_bs; p.du_ds = a->du_ds; p.dd_bs = a->ddelta_bs; p.dd_ds = a->ddelta_ds;
+    p.B_bs = a->B_bs; p.B_ns = a->B_ns; p.C_bs = a->C_bs; p.C_ns = a->C_ns;
+    p.softplus = a->delta_softplus;
+    const int v = 16 / elt_size(a->dtype);
+    auto mult = [v](int64_t s) { return s % v == 0; };
+    bool ok = mult(a->u_bs) && mult(a->u_ds) && mult(a->delta_bs) && mult(a->delta_ds) && mult(a->dout_bs) && mult(a->dout_ds) &&
+              mult(a->du_bs) && mult(a->du_ds) && mult(a->ddelta_bs) && mult(a->ddelta_ds) && mult(a->B_bs) && mult(a->B_ns) &&
+              mult(a->C_bs) && mult(a->C_ns) && a->seqlen % v == 0;
+    ScanBwdGroups gr{};
+    gr.ndesc = a->ngroups;
+    gr.dB_bs = a->dB_bs; gr.dB_ns = a->dB_ns; gr.dC_bs = a->dC_bs; gr.dC_ns = a->dC_ns;
+    for (int g = 0; g < a->ngroups; ++g) {
+        VMB_CHECK(a->u[g] && a->delta[g] && a->Bm[g] && a->Cm[g] && a->dout[g] && a->du[g] && a->ddelta[g] && a->dB[g] && a->dC[g],
+                  "selective_scan_bwd_grouped: null tensor pointer (group %d)", g);
+        ok = ok && aligned16(a->u[g]) && aligned16(a->delta[g]) && aligned16(a->Bm[g]) && aligned16(a->Cm[g]) && aligned16(a->dout[g]) &&
+             aligned16(a->du[g]) && aligned16(a->ddelta[g]);
+        gr.grp[g] = ScanBwdGroupDesc{a->u[g], a->delta[g], a->Bm[g], a->Cm[g], a->dout[g], a->du[g], a->ddelta[g], a->dB[g], a->dC[g], a->rev[g]};
+    }
+    VMB_CHECK(ok, "selective_scan_bwd_grouped: needs 16 B-aligned rows (base pointers, batch / row strides, seqlen %% %d == 0)", v);
+    p.vec_ok = true;
+    VMB_CHECK((long)p.batch * p.dim < (1L << 31), "selective_scan_bwd_grouped: batch*dim too large");
+    return scan_bwd_grouped_launch(p, gr, a->dtype, static_cast<cudaStream_t>(stream));
 }

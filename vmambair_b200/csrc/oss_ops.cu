@@ -909,6 +909,25 @@ int merge_launch(const MergeParams& p, int dtype, cudaStream_t stream) {
     return VMB_OK;
 }
 
+// the four-way fp32 sum alone (merge_sum_kernel into `out`, its per-pixel statistics into the workspace): cross_selective_scan's merge
+// (forward) and its adjoint of the direction-aware backward (du of every direction + the x_proj data gradients, in the groups' orders)
+int merge_sum_launch(const MergeParams& p, float* out, int dtype, cudaStream_t stream) {
+    VMB_CHECK(p.ws != nullptr && out != nullptr, "merge_sum: workspace / output missing");
+    const int L = p.H * p.W;
+    float* stats = reinterpret_cast<float*>(p.ws) + (size_t)p.B * p.C * L;
+    VMB_CUDA(cudaMemsetAsync(stats, 0, sizeof(float) * 2 * (size_t)p.B * L, stream));
+    dim3 gridA(((p.H + 15) / 16) * ((p.W + 15) / 16), (p.C + MG_CH - 1) / MG_CH, p.B);
+    VMB_CHECK(gridA.y <= 65535 && p.B <= 65535, "merge_sum: grid too large");
+    switch (dtype) {
+        case VMB_F32: merge_sum_kernel<float><<<gridA, 256, 0, stream>>>(p, out, stats); break;
+        case VMB_BF16: merge_sum_kernel<__nv_bfloat16><<<gridA, 256, 0, stream>>>(p, out, stats); break;
+        case VMB_F16: merge_sum_kernel<__half><<<gridA, 256, 0, stream>>>(p, out, stats); break;
+        default: set_error("merge_sum: unsupported dtype %d", dtype); return VMB_ERR_INVALID;
+    }
+    VMB_CUDA(cudaGetLastError());
+    return VMB_OK;
+}
+
 // ------------------------------------------------------------------------------------------ channel branch
 // One CTA (256 threads) per image.  Sequence = the C pooled channel means, dc rows, 2 directions, N states.
 

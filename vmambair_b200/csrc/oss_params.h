@@ -68,6 +68,7 @@ int dwconv_launch(const DwParams& p, int dtype, cudaStream_t stream);
 int cross_scan_launch(const CrossScanParams& p, int dtype, cudaStream_t stream);
 int cross_scan_multi_launch(const CrossScanMulti& m, int dtype, cudaStream_t stream);
 int merge_launch(const MergeParams& p, int dtype, cudaStream_t stream);
+int merge_sum_launch(const MergeParams& p, float* out, int dtype, cudaStream_t stream);
 int transpose_launch(const TransposeParams& p, int dtype, cudaStream_t stream);
 int pixel_shuffle_launch(const PixelShuffleParams& p, int dtype, cudaStream_t stream);
 int channel_launch(const ChannelParams& p, cudaStream_t stream);

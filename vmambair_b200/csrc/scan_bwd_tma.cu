@@ -15,13 +15,22 @@
 //     red.global.add.v4.f32 per (pair, position, CTA).
 #include <stdlib.h>
 
+#include <type_traits>
+
 #include "scan_tma_common.cuh"
 
 namespace vmb {
 
-struct ScanBwdTmaMaps {
-    CUtensorMap u, d, g, b, c;
+// plain operator: index 0 only (B/C group = z coordinate); grouped (NM = 4): one map per group and operand
+template <int NM>
+struct ScanBwdTmaMapsN {
+    CUtensorMap u[NM], d[NM], g[NM], b[NM], c[NM];
 };
+struct ScanBwdTmaMapsG : ScanBwdTmaMapsN<4> {
+    ScanBwdGroups gr;
+};
+template <bool GRP>
+using BwdMaps = typename std::conditional<GRP, ScanBwdTmaMapsG, ScanBwdTmaMapsN<1>>::type;
 
 template <typename in_t, int RB, int SS>
 struct BwdTmaCfg {
@@ -60,8 +69,11 @@ __device__ __forceinline__ void named_bar_sync(int idx, int count) {
     }
 }
 
-template <typename in_t, int RB, int SS>
-__global__ void __launch_bounds__(128, sizeof(in_t) == 4 ? 1 : 2) scan_bwd_tma_kernel(const ScanBwdParams p, const __grid_constant__ ScanBwdTmaMaps maps) {
+// GRP: per-group sources and destinations (vmb_selective_scan_bwd_grouped); a reversed group loads mirrored boxes (m0 = L - c0 - CHUNK,
+// underflow zero-filled as in the forward), reads them back to front and stores du / ddelta at memory index L-1-l.
+template <typename in_t, int RB, int SS, bool GRP>
+__global__ void __launch_bounds__(128, sizeof(in_t) == 4 ? 1 : 2)
+    scan_bwd_tma_kernel(const ScanBwdParams p, const __grid_constant__ BwdMaps<GRP> maps) {
     pdl_wait();
     using K = BwdTmaCfg<in_t, RB, SS>;
     using Cfg = FwdCfg<RB>;
@@ -98,19 +110,42 @@ __global__ void __launch_bounds__(128, sizeof(in_t) == 4 ? 1 : 2) scan_bwd_tma_k
     const int d0 = dc0 + rs * RB, d = d0 + r;
     const int N = p.N, L = p.L;
 
-    in_t* __restrict__ durow = reinterpret_cast<in_t*>(p.du) + (int64_t)b * p.du_bs + (int64_t)d * p.du_ds;
-    in_t* __restrict__ ddrow = reinterpret_cast<in_t*>(p.ddelta) + (int64_t)b * p.dd_bs + (int64_t)d * p.dd_ds;
+    // grouped: group g's own tensors, rows indexed inside the group
+    const void *du_base = p.du, *dd_base = p.ddelta;
+    bool rev = false;
+    int gi = 0, zbc = g, urow0 = dc0, dg = d;
+    if constexpr (GRP) {
+        const ScanBwdGroupDesc& gd = maps.gr.grp[g];
+        urow0 = dc0 - g * p.rows_per_group;
+        dg = urow0 + rs * RB + r;
+        du_base = gd.du;
+        dd_base = gd.ddelta;
+        rev = gd.rev != 0;
+        gi = g;
+        zbc = 0;
+    }
+    in_t* __restrict__ durow = reinterpret_cast<in_t*>(const_cast<void*>(du_base)) + (int64_t)b * p.du_bs + (int64_t)dg * p.du_ds;
+    in_t* __restrict__ ddrow = reinterpret_cast<in_t*>(const_cast<void*>(dd_base)) + (int64_t)b * p.dd_bs + (int64_t)dg * p.dd_ds;
     float4* __restrict__ scratch = reinterpret_cast<float4*>(p.dBC) + ((int64_t)b * p.G + g) * 8 * (int64_t)L;
     const float* __restrict__ ckrow = p.ckpt + ((int64_t)b * p.dim + d0) * p.n_ckpt * N;
 
     const int nchunks = (L + CHUNK - 1) / CHUNK;
     auto issue = [&](int c0) {
         mbarrier_expect_tx(bar, K::tx_bytes);
-        tma_load_4d(rawU, &maps.u, bar, c0, dc0, 0, b);
-        tma_load_4d(rawD, &maps.d, bar, c0, dc0, 0, b);
-        tma_load_4d(rawG, &maps.g, bar, c0, dc0, 0, b);
-        tma_load_4d(rawB, &maps.b, bar, c0, 0, g, b);
-        tma_load_4d(rawC, &maps.c, bar, c0, 0, g, b);
+        if constexpr (!GRP) {
+            tma_load_4d(rawU, &maps.u[0], bar, c0, dc0, 0, b);
+            tma_load_4d(rawD, &maps.d[0], bar, c0, dc0, 0, b);
+            tma_load_4d(rawG, &maps.g[0], bar, c0, dc0, 0, b);
+            tma_load_4d(rawB, &maps.b[0], bar, c0, 0, g, b);
+            tma_load_4d(rawC, &maps.c[0], bar, c0, 0, g, b);
+        } else {
+            const int m0 = rev ? L - c0 - CHUNK : c0;  // reversed walk: mirrored box, may start below 0 (zero-filled)
+            tma_load_4d(rawU, &maps.u[gi], bar, m0, urow0, 0, b);
+            tma_load_4d(rawD, &maps.d[gi], bar, m0, urow0, 0, b);
+            tma_load_4d(rawG, &maps.g[gi], bar, m0, urow0, 0, b);
+            tma_load_4d(rawB, &maps.b[gi], bar, m0, 0, zbc, b);
+            tma_load_4d(rawC, &maps.c[gi], bar, m0, 0, zbc, b);
+        }
     };
     if (tid == 0) {
         mbarrier_init(bar, 1);
@@ -138,15 +173,32 @@ __global__ void __launch_bounds__(128, sizeof(in_t) == 4 ? 1 : 2) scan_bwd_tma_k
         mbarrier_wait(bar, phase);
         phase ^= 1;
         if (ci < nchunks - 1) __syncthreads();  // every warp is done with the previous fp32 tile
-        convert_bc_dense<in_t, RB, NT>(sB, rawB, tid, false);
-        convert_bc_dense<in_t, RB, NT>(sC, rawC, tid, false);
+        convert_bc_dense<in_t, RB, NT>(sB, rawB, tid, GRP && rev);
+        convert_bc_dense<in_t, RB, NT>(sC, rawC, tid, GRP && rev);
         {
             const int row = rs * RB + r;
+            if (!GRP || !rev) {
 #pragma unroll
-            for (int v = 0; v < T / V; ++v) {
-                load_vec_smem<in_t>(rawU + row * CHUNK + sl * T + v * V, uv + v * V);
-                load_vec_smem<in_t>(rawD + row * CHUNK + sl * T + v * V, dt + v * V);
-                load_vec_smem<in_t>(rawG + row * CHUNK + sl * T + v * V, go + v * V);
+                for (int v = 0; v < T / V; ++v) {
+                    load_vec_smem<in_t>(rawU + row * CHUNK + sl * T + v * V, uv + v * V);
+                    load_vec_smem<in_t>(rawD + row * CHUNK + sl * T + v * V, dt + v * V);
+                    load_vec_smem<in_t>(rawG + row * CHUNK + sl * T + v * V, go + v * V);
+                }
+            } else {  // sequence position sl*T+t lives at raw index CHUNK-1-(sl*T+t)
+#pragma unroll
+                for (int v = 0; v < T / V; ++v) {
+                    float tu[V], td[V], tg[V];
+                    const int o = row * CHUNK + CHUNK - (sl + 1) * T + v * V;
+                    load_vec_smem<in_t>(rawU + o, tu);
+                    load_vec_smem<in_t>(rawD + o, td);
+                    load_vec_smem<in_t>(rawG + o, tg);
+#pragma unroll
+                    for (int i = 0; i < V; ++i) {
+                        uv[T - 1 - (v * V + i)] = tu[i];
+                        dt[T - 1 - (v * V + i)] = td[i];
+                        go[T - 1 - (v * V + i)] = tg[i];
+                    }
+                }
             }
         }
         __syncthreads();  // tile complete, raw buffers consumed
@@ -368,10 +420,31 @@ __global__ void __launch_bounds__(128, sizeof(in_t) == 4 ? 1 : 2) scan_bwd_tma_k
             ddo[t] = dd;
             dbias_acc += dd;
         }
+        if (!GRP || !rev) {
 #pragma unroll
-        for (int v = 0; v < T / V; ++v) {
-            store_vec<in_t>(durow + l0 + v * V, duo + v * V, valid - v * V, true);
-            store_vec<in_t>(ddrow + l0 + v * V, ddo + v * V, valid - v * V, true);
+            for (int v = 0; v < T / V; ++v) {
+                store_vec<in_t>(durow + l0 + v * V, duo + v * V, valid - v * V, true);
+                store_vec<in_t>(ddrow + l0 + v * V, ddo + v * V, valid - v * V, true);
+            }
+        } else if (valid == T) {  // sequence l0+t -> memory L-1-l0-t: one reversed contiguous block
+#pragma unroll
+            for (int v = 0; v < T / V; ++v) {
+                float ur[V], dr[V];
+#pragma unroll
+                for (int i = 0; i < V; ++i) {
+                    ur[i] = duo[T - 1 - (v * V + i)];
+                    dr[i] = ddo[T - 1 - (v * V + i)];
+                }
+                store_vec<in_t>(durow + (L - l0 - T) + v * V, ur, V, true);
+                store_vec<in_t>(ddrow + (L - l0 - T) + v * V, dr, V, true);
+            }
+        } else {
+#pragma unroll
+            for (int t = 0; t < T; ++t)
+                if (t < valid) {
+                    durow[L - 1 - l0 - t] = from_f32<in_t>(duo[t]);
+                    ddrow[L - 1 - l0 - t] = from_f32<in_t>(ddo[t]);
+                }
         }
     }
     // ---- per-row parameter gradients ----
@@ -392,10 +465,10 @@ __global__ void __launch_bounds__(128, sizeof(in_t) == 4 ? 1 : 2) scan_bwd_tma_k
 }
 
 // ---------------------------------------------------------------------------------------------------- host
-template <typename in_t, int RB, int SS>
-static int launch_bt3(const ScanBwdParams& p, const ScanBwdTmaMaps& maps, cudaStream_t stream) {
+template <typename in_t, int RB, int SS, bool GRP>
+static int launch_bt3(const ScanBwdParams& p, const BwdMaps<GRP>& maps, cudaStream_t stream) {
     using K = BwdTmaCfg<in_t, RB, SS>;
-    auto kern = scan_bwd_tma_kernel<in_t, RB, SS>;
+    auto kern = scan_bwd_tma_kernel<in_t, RB, SS, GRP>;
     constexpr size_t smem = K::smem_bytes + 128;
     static_assert(sizeof(in_t) == 4 ? smem <= 227 * 1024 : smem <= 113 * 1024, "scan_bwd_tma: two CTAs per SM (one for fp32 I/O)");
     VMB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -405,41 +478,46 @@ static int launch_bt3(const ScanBwdParams& p, const ScanBwdTmaMaps& maps, cudaSt
     return VMB_OK;
 }
 
-template <typename in_t, int RB>
-static int launch_bt2(const ScanBwdParams& p, const ScanBwdTmaMaps& maps, int ss, cudaStream_t stream) {
+template <typename in_t, int RB, bool GRP>
+static int launch_bt2(const ScanBwdParams& p, const BwdMaps<GRP>& maps, int ss, cudaStream_t stream) {
     switch (ss) {
-        case 4: return launch_bt3<in_t, RB, 4>(p, maps, stream);
-        case 2: return launch_bt3<in_t, RB, 2>(p, maps, stream);
-        default: return launch_bt3<in_t, RB, 1>(p, maps, stream);
+        case 4: return launch_bt3<in_t, RB, 4, GRP>(p, maps, stream);
+        case 2: return launch_bt3<in_t, RB, 2, GRP>(p, maps, stream);
+        default: return launch_bt3<in_t, RB, 1, GRP>(p, maps, stream);
     }
 }
 
-template <typename in_t>
-static int launch_bt1(const ScanBwdParams& p, const ScanBwdTmaMaps& maps, int ss, cudaStream_t stream) {
-    return launch_bt2<in_t, 2>(p, maps, ss, stream);  // rows per warp: 2 (scan_bwd_tma_pick)
+template <typename in_t, bool GRP>
+static int launch_bt1(const ScanBwdParams& p, const BwdMaps<GRP>& maps, int ss, cudaStream_t stream) {
+    return launch_bt2<in_t, 2, GRP>(p, maps, ss, stream);  // rows per warp: 2 (scan_bwd_tma_pick)
 }
 
-// (rows per warp, state split): the 255-register kernel keeps 2 CTAs x 4 warps per SM resident (2 x SMs CTAs per wave)
-bool scan_bwd_tma_pick(const ScanBwdParams& p, int dtype, int& rb, int& ss) {
-    const char* e = getenv("VMB_SCAN_BWD_TMA");
-    if (e && atoi(e) == 0) return false;
-    if (dtype == VMB_F32 && getenv("VMB_SCAN_BWD_TMA_F32") && atoi(getenv("VMB_SCAN_BWD_TMA_F32")) == 0) return false;
-    if (!p.vec_ok || p.npad != 16 || p.L < 512 || p.ckpt == nullptr) return false;
-    const int rpg = p.rows_per_group;
+// state split at RB = 2: the 255-register kernel keeps 2 CTAs x 4 warps per SM resident (2 x SMs CTAs per wave)
+static int bwd_tma_ss(const ScanBwdParams& p, int rb) {
     const long rows = (long)p.batch * p.dim;
-    // RB = 2 at every batch; the state split while the CTAs still fit one resident wave (tools/scan_bwd_sweep.py sweeps it)
-    rb = 2;
-    ss = 1;
+    int ss = 1;
     while (ss < 4 && rows / (rb * 4 / ss) * 2 <= 2L * num_sms()) ss <<= 1;
     if (const char* v = getenv("VMB_SCAN_SS_BWD")) {
         const int x = atoi(v);
         if (x == 1 || x == 2 || x == 4) ss = x;
     }
-    return rpg % (rb * 4 / ss) == 0;
+    return ss;
+}
+
+// (rows per warp, state split): RB = 2 at every batch; the state split while the CTAs still fit one resident wave
+// (tools/scan_bwd_sweep.py sweeps it)
+bool scan_bwd_tma_pick(const ScanBwdParams& p, int dtype, int& rb, int& ss) {
+    const char* e = getenv("VMB_SCAN_BWD_TMA");
+    if (e && atoi(e) == 0) return false;
+    if (dtype == VMB_F32 && getenv("VMB_SCAN_BWD_TMA_F32") && atoi(getenv("VMB_SCAN_BWD_TMA_F32")) == 0) return false;
+    if (!p.vec_ok || p.npad != 16 || p.L < 512 || p.ckpt == nullptr) return false;
+    rb = 2;
+    ss = bwd_tma_ss(p, rb);
+    return p.rows_per_group % (rb * 4 / ss) == 0;
 }
 
 int scan_bwd_tma_launch(const ScanBwdParams& p, int dtype, int rb, int ss, cudaStream_t stream) {
-    ScanBwdTmaMaps maps;
+    ScanBwdTmaMapsN<1> maps;
     const uint32_t chunk = 32 / rb * T, rows = rb * 4 / ss;
     const uint32_t box_io[4] = {chunk, rows, 1, 1}, box_bc[4] = {chunk, 16, 1, 1};
     const uint64_t dio[4] = {(uint64_t)p.L, (uint64_t)p.dim, 1, (uint64_t)p.batch};
@@ -447,17 +525,90 @@ int scan_bwd_tma_launch(const ScanBwdParams& p, int dtype, int rb, int ss, cudaS
     const int64_t su[3] = {p.u_ds, 0, p.u_bs}, sd[3] = {p.dl_ds, 0, p.dl_bs}, sg[3] = {p.do_ds, 0, p.do_bs};
     const int64_t sb[3] = {p.B_ns, p.B_gs, p.B_bs}, sc[3] = {p.C_ns, p.C_gs, p.C_bs};
     int rc;
-    if ((rc = make_tmap_4d(&maps.u, dtype, p.u, dio, su, box_io)) != VMB_OK) return rc;
-    if ((rc = make_tmap_4d(&maps.d, dtype, p.delta, dio, sd, box_io)) != VMB_OK) return rc;
-    if ((rc = make_tmap_4d(&maps.g, dtype, p.dout, dio, sg, box_io)) != VMB_OK) return rc;
-    if ((rc = make_tmap_4d(&maps.b, dtype, p.Bm, dbc, sb, box_bc)) != VMB_OK) return rc;
-    if ((rc = make_tmap_4d(&maps.c, dtype, p.Cm, dbc, sc, box_bc)) != VMB_OK) return rc;
+    if ((rc = make_tmap_4d(&maps.u[0], dtype, p.u, dio, su, box_io)) != VMB_OK) return rc;
+    if ((rc = make_tmap_4d(&maps.d[0], dtype, p.delta, dio, sd, box_io)) != VMB_OK) return rc;
+    if ((rc = make_tmap_4d(&maps.g[0], dtype, p.dout, dio, sg, box_io)) != VMB_OK) return rc;
+    if ((rc = make_tmap_4d(&maps.b[0], dtype, p.Bm, dbc, sb, box_bc)) != VMB_OK) return rc;
+    if ((rc = make_tmap_4d(&maps.c[0], dtype, p.Cm, dbc, sc, box_bc)) != VMB_OK) return rc;
     switch (dtype) {
-        case VMB_F32: return launch_bt1<float>(p, maps, ss, stream);  // 130 KB of tiles: one CTA per SM
-        case VMB_BF16: return launch_bt1<__nv_bfloat16>(p, maps, ss, stream);
-        case VMB_F16: return launch_bt1<__half>(p, maps, ss, stream);
+        case VMB_F32: return launch_bt1<float, false>(p, maps, ss, stream);  // 130 KB of tiles: one CTA per SM
+        case VMB_BF16: return launch_bt1<__nv_bfloat16, false>(p, maps, ss, stream);
+        case VMB_F16: return launch_bt1<__half, false>(p, maps, ss, stream);
     }
     set_error("selective_scan_bwd: unsupported dtype %d", dtype);
+    return VMB_ERR_INVALID;
+}
+
+// scratch [b][g][npad/2][L][4] fp32 (sequence order) -> every group's dB, dC (B,N,L) in the I/O dtype, in that group's memory order
+template <typename in_t>
+__global__ void scan_bwd_finalize_grouped_kernel(const float4* __restrict__ scratch, const ScanBwdGroups gr, int N, int L, long total) {
+    const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;  // over (b, g, np, l)
+    if (i >= total) return;
+    const int l = (int)(i % L);
+    const long t = i / L;
+    const int np = (int)(t % 8);
+    const long bg = t / 8;
+    const int g = (int)(bg % gr.ndesc);
+    const int64_t b = bg / gr.ndesc;
+    const ScanBwdGroupDesc& gd = gr.grp[g];
+    const int m = gd.rev ? L - 1 - l : l;
+    in_t* __restrict__ dB = reinterpret_cast<in_t*>(gd.dB) + b * gr.dB_bs + m;
+    in_t* __restrict__ dC = reinterpret_cast<in_t*>(gd.dC) + b * gr.dC_bs + m;
+    const float4 v = scratch[i];
+    const int n0 = 2 * np;
+    if (n0 < N) {
+        dB[n0 * gr.dB_ns] = from_f32<in_t>(v.x);
+        dC[n0 * gr.dC_ns] = from_f32<in_t>(v.z);
+    }
+    if (n0 + 1 < N) {
+        dB[(n0 + 1) * gr.dB_ns] = from_f32<in_t>(v.y);
+        dC[(n0 + 1) * gr.dC_ns] = from_f32<in_t>(v.w);
+    }
+}
+
+template <typename in_t>
+static int launch_grouped_t(const ScanBwdParams& p, const ScanBwdTmaMapsG& maps, int ss, cudaStream_t stream) {
+    int rc = launch_bt1<in_t, true>(p, maps, ss, stream);
+    if (rc != VMB_OK) return rc;
+    const long total = (long)p.batch * p.G * (p.npad / 2) * p.L;
+    scan_bwd_finalize_grouped_kernel<in_t><<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(reinterpret_cast<const float4*>(p.dBC), maps.gr,
+                                                                                                 p.N, p.L, total);
+    VMB_CUDA(cudaGetLastError());
+    return VMB_OK;
+}
+
+// the grouped mode always runs the TMA kernel (any seqlen: tails and the reversed walk's underflow are zero-filled boxes); the state
+// split grows until the CTA's rows divide the group
+int scan_bwd_grouped_launch(const ScanBwdParams& p, const ScanBwdGroups& gr, int dtype, cudaStream_t stream) {
+    VMB_CHECK(gr.ndesc == p.G && p.G >= 1 && p.G <= 4 && p.vec_ok && p.npad == 16, "selective_scan_bwd_grouped: needs 16 B-aligned rows and dstate <= 16");
+    const int rb = 2;
+    int ss = bwd_tma_ss(p, rb);
+    while (ss < 4 && p.rows_per_group % (rb * 4 / ss)) ss <<= 1;
+    VMB_CHECK(p.rows_per_group % (rb * 4 / ss) == 0, "selective_scan_bwd_grouped: rows per group (%d) must be even", p.rows_per_group);
+    ScanBwdTmaMapsG maps;
+    maps.gr = gr;
+    const uint32_t chunk = 32 / rb * T, rows = rb * 4 / ss;
+    const uint32_t box_io[4] = {chunk, rows, 1, 1}, box_bc[4] = {chunk, 16, 1, 1};
+    const uint64_t dio[4] = {(uint64_t)p.L, (uint64_t)p.rows_per_group, 1, (uint64_t)p.batch};
+    const uint64_t dbc[4] = {(uint64_t)p.L, (uint64_t)p.N, 1, (uint64_t)p.batch};
+    const int64_t su[3] = {p.u_ds, 0, p.u_bs}, sd[3] = {p.dl_ds, 0, p.dl_bs}, sg[3] = {p.do_ds, 0, p.do_bs};
+    const int64_t sb[3] = {p.B_ns, 0, p.B_bs}, sc[3] = {p.C_ns, 0, p.C_bs};
+    for (int g = 0; g < gr.ndesc; ++g) {
+        const ScanBwdGroupDesc& gd = gr.grp[g];
+        int rc;
+        if ((rc = make_tmap_4d(&maps.u[g], dtype, gd.u, dio, su, box_io)) != VMB_OK) return rc;
+        if ((rc = make_tmap_4d(&maps.d[g], dtype, gd.delta, dio, sd, box_io)) != VMB_OK) return rc;
+        if ((rc = make_tmap_4d(&maps.g[g], dtype, gd.dout, dio, sg, box_io)) != VMB_OK) return rc;
+        if ((rc = make_tmap_4d(&maps.b[g], dtype, gd.Bm, dbc, sb, box_bc)) != VMB_OK) return rc;
+        if ((rc = make_tmap_4d(&maps.c[g], dtype, gd.Cm, dbc, sc, box_bc)) != VMB_OK) return rc;
+    }
+    VMB_CUDA(cudaMemsetAsync(p.dBC, 0, sizeof(float4) * (size_t)p.batch * p.G * (p.npad / 2) * p.L, stream));
+    switch (dtype) {
+        case VMB_F32: return launch_grouped_t<float>(p, maps, ss, stream);
+        case VMB_BF16: return launch_grouped_t<__nv_bfloat16>(p, maps, ss, stream);
+        case VMB_F16: return launch_grouped_t<__half>(p, maps, ss, stream);
+    }
+    set_error("selective_scan_bwd_grouped: unsupported dtype %d", dtype);
     return VMB_ERR_INVALID;
 }
 

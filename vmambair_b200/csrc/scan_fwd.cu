@@ -116,7 +116,7 @@ __device__ __forceinline__ void stage_bc_cta(float4* __restrict__ dst, const in_
 }
 
 // MODE 0: plain operator, no checkpoints (inference)   1: plain operator + checkpoints (training forward)
-//      2: direction-aware grouped sources (per-group bases, reversed walk), no checkpoints.
+//      2: direction-aware grouped sources (per-group bases, reversed walk), no checkpoints   3: 2 + checkpoints.
 // Each mode only compiles what it needs: the state loop sits at the 128-register limit.
 template <typename in_t, int RB, int WPC, int MODE>
 __global__ void __launch_bounds__(32 * WPC, 12 / WPC) scan_fwd_kernel(const ScanFwdParams p) {
@@ -145,12 +145,12 @@ __global__ void __launch_bounds__(32 * WPC, 12 / WPC) scan_fwd_kernel(const Scan
     const int g = d0 / p.rows_per_group;  // same for every warp of the CTA (RB*WPC divides the group)
     const int N = p.N, L = p.L, npad = p.npad;
     const bool async_ok = p.vec_ok;
-    constexpr bool HAS_REV = MODE == 2;
+    constexpr bool HAS_REV = MODE >= 2;
 
     const in_t *Bg, *Cg, *ublk, *dblk;
     in_t* orow;
     bool rev = false;
-    if (MODE != 2) {
+    if (MODE < 2) {
         Bg = reinterpret_cast<const in_t*>(p.Bm) + (int64_t)b * p.B_bs + (int64_t)g * p.B_gs;
         Cg = reinterpret_cast<const in_t*>(p.Cm) + (int64_t)b * p.C_bs + (int64_t)g * p.C_gs;
         ublk = reinterpret_cast<const in_t*>(p.u) + (int64_t)b * p.u_bs + (int64_t)d0 * p.u_ds;
@@ -298,7 +298,7 @@ __global__ void __launch_bounds__(32 * WPC, 12 / WPC) scan_fwd_kernel(const Scan
                     h = fma2(a2[t + 1], h, mul2(make_float2(dtu[t + 1], dtu[t + 1]), make_float2(Bq.z, Bq.w)));
                     y[t + 1] = fmaf(h.y, Cq.w, fmaf(h.x, Cq.z, y[t + 1]));
                 }
-                if (MODE == 1 && l0 < L && ((l0 + T) % kScanCkpt) == 0) {
+                if ((MODE == 1 || MODE == 3) && l0 < L && ((l0 + T) % kScanCkpt) == 0) {
                     float* ck = p.ckpt + (((int64_t)b * p.dim + d) * p.n_ckpt + ((l0 + T) / kScanCkpt - 1)) * N + n0;
                     if (n0 < N) ck[0] = h.x;
                     if (n0 + 1 < N) ck[1] = h.y;
@@ -340,7 +340,13 @@ static int launch_cfg2(const ScanFwdParams& p, cudaStream_t stream) {
 
 template <typename in_t, int RB, int WPC>
 static int launch_cfg(const ScanFwdParams& p, cudaStream_t stream) {
-    if (p.ndesc) return launch_cfg2<in_t, RB, WPC, 2>(p, stream);
+    if (p.ndesc) {
+        if constexpr (RB <= 2) {
+            if (p.ckpt) return launch_cfg2<in_t, RB, WPC, 3>(p, stream);
+        }
+        VMB_CHECK(p.ckpt == nullptr, "grouped scan: checkpoints need RB <= 2 (pick_cfg)");
+        return launch_cfg2<in_t, RB, WPC, 2>(p, stream);
+    }
     return p.ckpt ? launch_cfg2<in_t, RB, WPC, 1>(p, stream) : launch_cfg2<in_t, RB, WPC, 0>(p, stream);
 }
 
@@ -358,6 +364,7 @@ static void pick_cfg(const ScanFwdParams& p, int& rb, int& wpc) {
     // short sequences: a warp-chunk should not be much longer than L
     while (rb < 8 && rpg % (rb * 2) == 0 && (32 / rb) * T >= 2 * p.L) rb *= 2;
     if (env_rb > 0 && env_rb <= 8 && (env_rb & (env_rb - 1)) == 0 && rpg % env_rb == 0) rb = env_rb;
+    if (p.ndesc && p.ckpt && rb > 2) rb = 2;  // grouped + checkpoints (MODE 3) is instantiated at RB <= 2 only: RB 4 / 8 spill
     wpc = 4;
     while (wpc > 1 && (rpg % (rb * wpc) != 0)) wpc >>= 1;
     if (env_wpc > 0 && (env_wpc & (env_wpc - 1)) == 0 && rpg % (rb * env_wpc) == 0 && env_wpc <= 4) wpc = env_wpc;
@@ -392,7 +399,6 @@ int scan_fwd_launch(const ScanFwdParams& p, int dtype, cudaStream_t stream) {
     }
     if (p.ndesc) {
         VMB_CHECK(p.vec_ok && p.npad == 16, "grouped scan: needs 16 B-aligned rows (L %% 8 == 0) and dstate <= 16");
-        VMB_CHECK(p.ckpt == nullptr, "grouped scan: inference only (no checkpoints)");
     }
     switch (dtype) {
         case VMB_F32: return launch_t<float>(p, stream);

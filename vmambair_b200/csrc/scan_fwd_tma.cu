@@ -35,6 +35,7 @@ struct TmaCfg {
 };
 
 // MODE 0: plain operator   1: plain + checkpoints (training forward)   2: per-group sources, reversed walk (fused OSS block)
+//      3: per-group sources + checkpoints (cross_selective_scan forward; indexed by sequence position, like MODE 1 on gathered copies)
 template <typename in_t, int RB, int NW, int SS, int MODE>
 __global__ void __launch_bounds__(32 * NW, NW == 8 ? 2 : 3)
     scan_fwd_tma_kernel(const ScanFwdParams p, const __grid_constant__ ScanTmaMaps maps) {
@@ -72,7 +73,7 @@ __global__ void __launch_bounds__(32 * NW, NW == 8 ? 2 : 3)
     in_t* orow;
     bool rev = false;
     int gi = 0, zbc = g, urow0 = dc0;
-    if (MODE != 2) {
+    if (MODE < 2) {
         orow = reinterpret_cast<in_t*>(p.out) + (int64_t)b * p.o_bs + (int64_t)d * p.o_ds;
     } else {
         const ScanGroupDesc& gd = p.grp[g];
@@ -112,12 +113,12 @@ __global__ void __launch_bounds__(32 * NW, NW == 8 ? 2 : 3)
         mbarrier_wait(bar, phase);
         phase ^= 1;
         if (c0 > 0) __syncthreads();  // every warp is done with the previous fp32 tile
-        convert_bc_dense<in_t, RB, NT>(sB, rawB, tid, MODE == 2 && rev);
-        convert_bc_dense<in_t, RB, NT>(sC, rawC, tid, MODE == 2 && rev);
+        convert_bc_dense<in_t, RB, NT>(sB, rawB, tid, MODE >= 2 && rev);
+        convert_bc_dense<in_t, RB, NT>(sC, rawC, tid, MODE >= 2 && rev);
         {
             const in_t* ur = rawU + (rs * RB + r) * CHUNK;
             const in_t* dr = rawD + (rs * RB + r) * CHUNK;
-            if (MODE != 2 || !rev) {
+            if (MODE < 2 || !rev) {
 #pragma unroll
                 for (int v = 0; v < T / V; ++v) {
                     load_vec_smem<in_t>(ur + sl * T + v * V, uv + v * V);
@@ -275,7 +276,7 @@ __global__ void __launch_bounds__(32 * NW, NW == 8 ? 2 : 3)
                     y[t + 1] = fmaf(h.y, Cq.w, fmaf(h.x, Cq.z, y[t + 1]));
                 }
             }
-            if (MODE == 1 && l0 < L && ((l0 + T) % kScanCkpt) == 0) {
+            if ((MODE == 1 || MODE == 3) && l0 < L && ((l0 + T) % kScanCkpt) == 0) {
                 float* ck = p.ckpt + (((int64_t)b * p.dim + d) * p.n_ckpt + ((l0 + T) / kScanCkpt - 1)) * N + n0;
                 if (n0 < N) ck[0] = h.x;
                 if (n0 + 1 < N) ck[1] = h.y;
@@ -295,7 +296,7 @@ __global__ void __launch_bounds__(32 * NW, NW == 8 ? 2 : 3)
 #pragma unroll
                 for (int t = 0; t < T; ++t) y[t] += yp[(s * T + t) * 32 + lane];
         }
-        if (MODE != 2 || !rev) {
+        if (MODE < 2 || !rev) {
 #pragma unroll
             for (int v = 0; v < T / V; ++v) store_vec<in_t>(orow + l0 + v * V, y + v * V, valid - v * V, true);
         } else if (valid == T) {  // sequence l0+t -> memory L-1-l0-t: one reversed contiguous block
@@ -374,7 +375,7 @@ static int launch_tma4(const ScanFwdParams& p, const ScanTmaMaps& maps, cudaStre
 
 template <typename in_t, int RB, int NW, int SS>
 static int launch_tma3(const ScanFwdParams& p, const ScanTmaMaps& maps, cudaStream_t stream) {
-    if (p.ndesc) return launch_tma4<in_t, RB, NW, SS, 2>(p, maps, stream);
+    if (p.ndesc) return p.ckpt ? launch_tma4<in_t, RB, NW, SS, 3>(p, maps, stream) : launch_tma4<in_t, RB, NW, SS, 2>(p, maps, stream);
     return p.ckpt ? launch_tma4<in_t, RB, NW, SS, 1>(p, maps, stream) : launch_tma4<in_t, RB, NW, SS, 0>(p, maps, stream);
 }
 

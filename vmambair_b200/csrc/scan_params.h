@@ -31,6 +31,14 @@ struct ScanFwdParams {
     int num_sms;
 };
 
+// Per-group operands of the direction-aware backward: the forward's sources, the incoming gradient and the four gradient
+// outputs of group g, all in the memory order of that group's sources (rev: sequence position l <-> memory index L-1-l).
+struct ScanBwdGroupDesc {
+    const void *u, *delta, *Bm, *Cm, *dout;
+    void *du, *ddelta, *dB, *dC;
+    int rev;
+};
+
 struct ScanBwdParams {
     const void *u, *delta, *Bm, *Cm, *dout;
     const float *A, *D, *bias, *ckpt;
@@ -45,11 +53,20 @@ struct ScanBwdParams {
     int debug_nored;  // profiling only (VMB_BWD_NORED=1): skip the dB/dC global reductions
 };
 
+// Grouped backward (vmb_selective_scan_bwd_grouped): G = ndesc <= 4 group descriptors; strides are the ScanBwdParams ones, shared by
+// the groups, rows indexed inside the group.  Kept out of ScanBwdParams so that the flat kernels' parameter layout is unchanged.
+struct ScanBwdGroups {
+    int ndesc;
+    ScanBwdGroupDesc grp[4];
+    int64_t dB_bs, dB_ns, dC_bs, dC_ns;  // strides of every group's dB / dC (B,N,L) destination
+};
+
 int scan_fwd_launch(const ScanFwdParams& p, int dtype, cudaStream_t stream);
 bool scan_fwd_tma_pick(const ScanFwdParams& p, int& rb, int& ss);
 int scan_fwd_tma_launch(const ScanFwdParams& p, int dtype, int rb, int ss, cudaStream_t stream);
 int scan_bwd_launch(const ScanBwdParams& p, int dtype, cudaStream_t stream);
 bool scan_bwd_tma_pick(const ScanBwdParams& p, int dtype, int& rb, int& ss);
 int scan_bwd_tma_launch(const ScanBwdParams& p, int dtype, int rb, int ss, cudaStream_t stream);
+int scan_bwd_grouped_launch(const ScanBwdParams& p, const ScanBwdGroups& gr, int dtype, cudaStream_t stream);
 
 }  // namespace vmb

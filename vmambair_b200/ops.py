@@ -316,9 +316,10 @@ def transpose_hw(x, H, W):
     return out
 
 
-def selective_scan_fwd_grouped(us, deltas, Bs, Cs, revs, A, D, delta_bias, delta_softplus=True):
+def selective_scan_fwd_grouped(us, deltas, Bs, Cs, revs, A, D, delta_bias, delta_softplus=True, need_ckpt=False):
     """Direction-aware forward: group g reads us[g] (B,R,L), deltas[g] (B,R,L), Bs[g]/Cs[g] (B,N,L) (views sharing
-    strides) and walks them backwards when revs[g]; returns (B, G, R, L) with group g written in ITS SOURCE's memory order."""
+    strides) and walks them backwards when revs[g]; returns (B, G, R, L) with group g written in ITS SOURCE's memory order.
+    need_ckpt: -> (out, ckpt) with the fp32 checkpoints (B, G*R, n_ckpt, N) that selective_scan_bwd_grouped consumes."""
     G = len(us)
     b, R, L = us[0].shape
     N = A.shape[1]
@@ -326,17 +327,84 @@ def selective_scan_fwd_grouped(us, deltas, Bs, Cs, revs, A, D, delta_bias, delta
         for t in lst:
             assert t.stride() == lst[0].stride() and t.stride(2) == 1 and t.dtype == us[0].dtype
     out = torch.empty((b, G, R, L), dtype=us[0].dtype, device=us[0].device)
+    ck = ckpt_interval()
+    ckpt = torch.empty((b, G * R, (L + ck - 1) // ck, N), dtype=torch.float32, device=us[0].device) if need_ckpt else None
     arr = lambda lst: (C.c_void_p * 4)(*([t.data_ptr() for t in lst] + [0] * (4 - G)))
     outs = [out[:, g] for g in range(G)]
     a = _lib.ScanGroupedArgs(
         arr(us), arr(deltas), arr(Bs), arr(Cs), arr(outs), (C.c_int * 4)(*(list(map(int, revs)) + [0] * (4 - G))),
         _ptr(A), _ptr(D), _ptr(delta_bias), b, G * R, L, N, G,
         us[0].stride(0), us[0].stride(1), deltas[0].stride(0), deltas[0].stride(1), out.stride(0), out.stride(2),
-        Bs[0].stride(0), Bs[0].stride(1), Cs[0].stride(0), Cs[0].stride(1), int(bool(delta_softplus)), _DT[us[0].dtype])
+        Bs[0].stride(0), Bs[0].stride(1), Cs[0].stride(0), Cs[0].stride(1), int(bool(delta_softplus)), _DT[us[0].dtype], _ptr(ckpt))
     es = us[0].element_size()
     n_u = len({t.data_ptr() for t in us})  # forward and reversed directions share one source tensor: counted once
     nbytes = es * b * L * (n_u * R + G * R + G * R + 2 * G * N) + 4 * (G * R * N + 2 * G * R)  # every unique operand / result once
+    if ckpt is not None:
+        nbytes += 4 * ckpt.numel()
     _run("vmb_selective_scan_fwd_grouped", a, us[0], "scan_fwd", nbytes)
+    return (out, ckpt) if need_ckpt else out
+
+
+def selective_scan_bwd_grouped(us, deltas, Bs, Cs, douts, revs, A, D, delta_bias, ckpt, delta_softplus=True, zeroed=None, out=None):
+    """Backward of selective_scan_fwd_grouped (checkpoints from its need_ckpt=True call): douts[g] (B,R,L) is the gradient of group
+    g's output in that group's memory order.  -> (dus, ddeltas, dA, dBs, dCs, dD, ddelta_bias): dus / ddeltas lists of (B,R,L), dBs / dCs
+    lists of (B,N,L), every one in the memory order of group g's sources; dA (G*R,N), dD, ddelta_bias (G*R) fp32.
+    zeroed: optional (dA, dD, dbias) pre-zeroed fp32 accumulators.  out: optional (dus, ddeltas, dBs, dCs) destination views (each list
+    sharing strides, rows contiguous), e.g. slices of the buffers the next kernels read."""
+    G = len(us)
+    b, R, L = us[0].shape
+    N = A.shape[1]
+    dev, dt = us[0].device, us[0].dtype
+    for lst in (us, deltas, Bs, Cs, douts):
+        for t in lst:
+            assert t.stride() == lst[0].stride() and t.stride(2) == 1 and t.dtype == dt and t.is_cuda
+    if out is None:
+        du = torch.empty((b, G, R, L), dtype=dt, device=dev)
+        ddelta = torch.empty((b, G, R, L), dtype=dt, device=dev)
+        dBm = torch.empty((b, G, N, L), dtype=dt, device=dev)
+        dCm = torch.empty((b, G, N, L), dtype=dt, device=dev)
+        out = ([du[:, g] for g in range(G)], [ddelta[:, g] for g in range(G)], [dBm[:, g] for g in range(G)], [dCm[:, g] for g in range(G)])
+    dus, dds, dBs, dCs = out
+    for lst in out:
+        for t in lst:
+            assert t.stride() == lst[0].stride() and t.stride(2) == 1 and t.dtype == dt
+    Lb = _lib.lib()
+    dA = torch.zeros_like(A) if zeroed is None else zeroed[0]
+    dD = (torch.zeros_like(D) if zeroed is None else zeroed[1]) if D is not None else None
+    dbias = (torch.zeros_like(delta_bias) if zeroed is None else zeroed[2]) if delta_bias is not None else None
+    ws = torch.empty(Lb.vmb_scan_bwd_workspace_bytes(b, G, N, L), dtype=torch.uint8, device=dev)
+    arr = lambda lst: (C.c_void_p * 4)(*([t.data_ptr() for t in lst] + [0] * (4 - G)))
+    a = _lib.ScanGroupedBwdArgs(
+        arr(us), arr(deltas), arr(Bs), arr(Cs), arr(douts), arr(dus), arr(dds), arr(dBs), arr(dCs),
+        (C.c_int * 4)(*(list(map(int, revs)) + [0] * (4 - G))),
+        _ptr(A), _ptr(D), _ptr(delta_bias), _ptr(ckpt), _ptr(dA), _ptr(dD), _ptr(dbias), _ptr(ws),
+        b, G * R, L, N, G,
+        us[0].stride(0), us[0].stride(1), deltas[0].stride(0), deltas[0].stride(1), douts[0].stride(0), douts[0].stride(1),
+        dus[0].stride(0), dus[0].stride(1), dds[0].stride(0), dds[0].stride(1),
+        Bs[0].stride(0), Bs[0].stride(1), Cs[0].stride(0), Cs[0].stride(1),
+        dBs[0].stride(0), dBs[0].stride(1), dCs[0].stride(0), dCs[0].stride(1), int(bool(delta_softplus)), _DT[dt])
+    es = us[0].element_size()
+    uniq = lambda lst: len({t.data_ptr() for t in lst})  # directions that share a source tensor read it once
+    nbytes = es * b * L * (R * (uniq(us) + G + uniq(douts) + 2 * G) + 4 * G * N) + (4 * ckpt.numel() if ckpt is not None else 0)
+    with torch.cuda.device(dev), _timed("scan_bwd", nbytes, dev, 2):
+        _lib.check(Lb.vmb_selective_scan_bwd_grouped(C.byref(a), _stream(us[0])), "selective_scan_bwd_grouped")
+    return dus, dds, dA, dBs, dCs, dD, dbias
+
+
+def merge_sum(ys, C_, H, W, in_place_order=False, out=None):
+    """ys: (B,4,C,L) contiguous, four scan directions -> fp32 (B,C,L): (y0 + y2') + T y1' + T y3' in pixel order, where ' is the
+    inverse order of the direction (in_place_order: ys[0], ys[2] hold natural (H,W) pixel order and ys[1], ys[3] the transposed (W,H)
+    order, as the grouped scan writes them; else every ys[k] is in scan order, k = 2, 3 reversed).  out: optional fp32 (B,C,L) dense."""
+    B = ys.shape[0]
+    assert ys.is_contiguous() and ys.shape == (B, 4, C_, H * W)
+    if out is None:
+        out = torch.empty((B, C_, H * W), dtype=torch.float32, device=ys.device)
+    assert out.dtype == torch.float32 and out.is_contiguous()
+    ws = torch.empty(_lib.lib().vmb_merge_workspace_bytes(B, C_, H, W), dtype=torch.uint8, device=ys.device)
+    a = _lib.MergeArgs(_ptr(ys), None, None, None, None, None, B, C_, H, W, 0, 0, _DT[ys.dtype], _ptr(ws), int(in_place_order), 0, 0)
+    fn = _lib.lib().vmb_merge_sum
+    with torch.cuda.device(ys.device), _timed("merge", ys.element_size() * ys.numel() + 4 * out.numel(), ys.device, 1):
+        _lib.check(fn(C.byref(a), _ptr(out), _stream(ys)), "vmb_merge_sum")
     return out
 
 
