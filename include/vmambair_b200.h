@@ -337,6 +337,43 @@ int vmb_channel_branch_bwd(const vmb_channel_bwd_args* a, void* stream);
 int64_t vmb_channel_branch_bwd_smem_bytes(int C, int dc, int Rc, int N);
 int64_t vmb_channel_branch_bwd_scratch_bytes(int batch, int dc, int C);
 
+/* Two-direction channel selective scan, cross_selective_scanC (RealSR/VmambaIR/archs/MambaRealSR11_arch.py:438-534: CrossScanC,
+ * the x_proj / dt_proj einsums, SelectiveScan, CrossMergeC), one CTA per image, everything in fp32 shared memory:
+ *   xs_0 = x[b] (D, L), xs_1 = flip_L(x[b]);  x_dbl_k = W_k xs_k (+ bias_k);  dt_k = softplus?(Wdt_k x_dbl_k[:R] + dt_bias_k)
+ *   y_k = selective scan of (u = xs_k, dt_k, A_k = -exp(A_logs[k]), B = x_dbl_k[R:R+N], C = x_dbl_k[R+N:], D = Ds[k])
+ *   y[b][l][d] = y_0[d][l] + y_1[d][L-1-l]
+ *   x : (batch, D, L) in `dtype`, element strides x_bs / x_ds, last stride 1
+ *   x_proj_weight (2, R+2N, D), x_proj_bias (2, R+2N) or NULL, dt_projs_weight (2, D, R), dt_projs_bias (2D), A_logs (2D, N),
+ *   Ds (2D): fp32 contiguous
+ *   y : forward output, fp32 (batch, L, D) dense (the reference's (B, L, 1, D))
+ * Bounds: d_state N <= 16, D <= 16 and vmb_cross_selective_scan_c_smem_bytes(D, L, R, N) <= 227 KB (every RealSR channel call:
+ * D = 1, N = 16, L = C <= 384, R = ceil(C/16)); anything else returns VMB_ERR_INVALID. */
+typedef struct {
+    const void* x;
+    const float* x_proj_weight; const float* x_proj_bias; const float* dt_projs_weight; const float* dt_projs_bias;
+    const float* A_logs; const float* Ds;
+    float* y;
+    int batch, D, L, R, N;
+    int64_t x_bs, x_ds;
+    int delta_softplus;
+    int dtype;
+} vmb_cross_scan_c_args;
+int vmb_cross_selective_scan_c_fwd(const vmb_cross_scan_c_args* a, void* stream);
+/* backward: recomputes the forward per image and walks the recurrence backwards.  fwd: the forward's arguments (y unused).
+ *   dy : fp32 (batch, L, D) dense, gradient w.r.t. y;  dx : (batch, D, L) dense, x's dtype, fully written
+ *   d_params : fp32, fully written (not accumulated), packed as x_proj_weight (2(R+2N)D), x_proj_bias (2(R+2N); written even when
+ *              the bias is NULL), dt_projs_weight (2DR), dt_projs_bias (2D), A_logs (2DN), Ds (2D)
+ *   workspace : vmb_cross_selective_scan_c_workspace_bytes(batch, D, R, N) bytes: the per-image gradients, which a second kernel
+ *               sums over the batch in a fixed order (no atomics: bitwise reproducible) */
+typedef struct {
+    vmb_cross_scan_c_args fwd;
+    const float* dy; void* dx; float* d_params; float* workspace;
+} vmb_cross_scan_c_bwd_args;
+int vmb_cross_selective_scan_c_bwd(const vmb_cross_scan_c_bwd_args* a, void* stream);
+/* shared-memory bytes the backward (the larger of the two kernels) needs at (D, L, R, N); -1 when N > 16 or D > 16 */
+int64_t vmb_cross_selective_scan_c_smem_bytes(int D, int L, int R, int N);
+int64_t vmb_cross_selective_scan_c_workspace_bytes(int batch, int D, int R, int N);
+
 /* weight gradient of a 1x1 conv: out[m][k] += sum_{b,p} dy[b][m][p] * x[b][k][p]  (out fp32 (M,K), accumulated: the caller zero-fills;
  * per_batch != 0: out is (B,M,K) and batches are not summed -- the channel gate in front of out_conv scales them per image).
  * dy (B,M,L), x (B,K,L): bf16 / fp16 views with 16 B aligned, pixel-contiguous rows.  mma.sync tensor-core kernel, split over

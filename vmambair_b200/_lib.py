@@ -171,6 +171,17 @@ class ChannelBwdArgs(C.Structure):
                 ("d_cout_w", vp), ("d_cout_b", vp), ("d_cn_w", vp), ("d_cn_b", vp), ("scratch", vp)]
 
 
+class CrossScanCArgs(C.Structure):
+    _fields_ = [("x", vp), ("x_proj_weight", vp), ("x_proj_bias", vp), ("dt_projs_weight", vp), ("dt_projs_bias", vp),
+                ("A_logs", vp), ("Ds", vp), ("y", vp),
+                ("batch", C.c_int), ("D", C.c_int), ("L", C.c_int), ("R", C.c_int), ("N", C.c_int),
+                ("x_bs", i64), ("x_ds", i64), ("delta_softplus", C.c_int), ("dtype", C.c_int)]
+
+
+class CrossScanCBwdArgs(C.Structure):
+    _fields_ = [("fwd", CrossScanCArgs), ("dy", vp), ("dx", vp), ("d_params", vp), ("workspace", vp)]
+
+
 class PrepJob(C.Structure):
     _fields_ = [("src", vp), ("src2", vp), ("dst", vp), ("dst2", vp), ("type", C.c_int), ("M", C.c_int), ("K", C.c_int),
                 ("N2", C.c_int), ("ld", C.c_int), ("ld2", C.c_int)]
@@ -220,6 +231,10 @@ SYMBOLS = {
     "vmb_channel_branch_bwd": (C.c_int, [C.POINTER(ChannelBwdArgs), vp]),
     "vmb_channel_branch_bwd_smem_bytes": (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int]),
     "vmb_channel_branch_bwd_scratch_bytes": (C.c_int64, [C.c_int, C.c_int, C.c_int]),
+    "vmb_cross_selective_scan_c_fwd": (C.c_int, [C.POINTER(CrossScanCArgs), vp]),
+    "vmb_cross_selective_scan_c_bwd": (C.c_int, [C.POINTER(CrossScanCBwdArgs), vp]),
+    "vmb_cross_selective_scan_c_smem_bytes": (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int]),
+    "vmb_cross_selective_scan_c_workspace_bytes": (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int]),
     "vmb_prep_block_weights": (C.c_int, [C.POINTER(PrepArgs), vp]),
     "vmb_sum4_add": (C.c_int, [vp, vp, vp, C.c_int, C.c_long, C.c_int, vp]),
 }

@@ -272,6 +272,21 @@ class SS2D_1(nn.Module):
         return cross_selective_scan(x, self.x_proj_weight, None, self.dt_projs_weight, self.dt_projs_bias, self.A_logs, self.Ds,
                                     self.out_norm, self.softmax_version, nrows=nrows, delta_softplus=True)
 
+    def cforward_corev2(self, xc: torch.Tensor, nrows=-1, channel_first=False):
+        """the channel-direction scan of this module as the reference's cforward_corev2 (RealSR/VmambaIR/archs/MambaRealSR11_arch.py:806-817):
+        xc (B,H,W,D) channels-last, or (B,D,H,W) when channel_first -> AdaptiveAvgPool2d(1) -> channel_norm(cross_selective_scanC(...))
+        (B,D,1,1), differentiable, on the library's fused channel-scan kernels.  variant="realsr" only; nothing calls it by default."""
+        if self.variant != "realsr":
+            raise NotImplementedError(f"cforward_corev2 exists for variant='realsr' only: the '{self.variant}' channel parameters have "
+                                      f"dc_inner = {self.dc_inner} rows and a conv_cin in front of the scan (use cforward_core)")
+        from .cross_scan import cross_selective_scanC
+        if not channel_first:
+            xc = xc.permute(0, 3, 1, 2).contiguous()
+        b, d, h, w = xc.shape
+        xc = self.pooling(xc).view(b, -1, d)  # (b, 1, d)
+        return cross_selective_scanC(xc, self.xc_proj_weight, None, self.dtc_projs_weight, self.dtc_projs_bias, self.Ac_logs, self.Dsc,
+                                     self.channel_norm, self.softmax_version, nrows=nrows, delta_softplus=True)
+
     def forward(self, x: torch.Tensor, **kwargs):
         return self.forward_compose(x)
 

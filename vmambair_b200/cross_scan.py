@@ -1,4 +1,5 @@
-"""Four-direction 2-D selective scan as a differentiable operator: `cross_selective_scan`, `CrossScan`, `CrossMerge`.
+"""Four-direction 2-D selective scan as a differentiable operator: `cross_selective_scan`, `CrossScan`, `CrossMerge`; and the
+two-direction channel scan next to it: `cross_selective_scanC`, `CrossScanC`, `CrossMergeC` (at the end of this module).
 
 Reference: RealSR/VmambaIR/archs/MambaRealSR11_arch.py:325-434 (CrossScan, CrossMerge, cross_selective_scan), called by
 SS2D_1.forward_corev2 (:791-804) and by VMamba-style code directly.
@@ -233,6 +234,170 @@ def cross_selective_scan(x: torch.Tensor = None, x_proj_weight: torch.Tensor = N
                            "dt_projs_bias (4,D), A_logs (4D,N), Ds (4D)")
     with torch.autocast("cuda", enabled=False):
         y = _CrossSelectiveScan.apply(x, x_proj_weight, x_proj_bias, dt_projs_weight, dt_projs_bias, A_logs, Ds, bool(delta_softplus))
+    y = out_norm(y)
+    if to_dtype:
+        y = y.to(x.dtype)
+    return y
+
+
+# ----------------------------------------------------------------------------- the two-direction channel scan
+# Reference: RealSR/VmambaIR/archs/MambaRealSR11_arch.py:438-534 (CrossScanC, CrossMergeC, cross_selective_scanC), called by
+# SS2D_1.cforward_corev2 (:806-817) on the pooled (B, 1, C) descriptor.
+#
+#   forward   vmb_cross_selective_scan_c_fwd: one CTA per image loads x once and runs both projections, softplus, both scan
+#             directions and the merge in fp32 shared memory -> y (B, L, 1, D) fp32
+#   backward  vmb_cross_selective_scan_c_bwd: one CTA per image recomputes the forward, walks the recurrence backwards and writes dx
+#             and its own parameter gradients; a second kernel sums those over the batch in a fixed order (bitwise reproducible)
+#
+# Shapes the kernels reject (cross_scan_c_supported: d_state > 16, D > 16, or a state history beyond one CTA's shared memory) take
+# the composed path inside the same Function: fp32 torch einsums around the flat vmb_selective_scan_fwd / _bwd.
+
+
+class CrossScanC(torch.autograd.Function):
+    """x (B,D,L) -> xs (B,2,D,L) = [x, flip_L x] (reference :438-456).  Backward: ys[:,0] + flip_L ys[:,1], i.e. CrossMergeC's
+    forward.  Plain torch indexing: the fused operator does not use it."""
+
+    @staticmethod
+    def forward(ctx, x):
+        B, D, L = x.shape
+        xs = x.new_empty((B, 2, D, L))
+        xs[:, 0] = x
+        xs[:, 1] = torch.flip(x, dims=[-1])
+        return xs
+
+    @staticmethod
+    def backward(ctx, ys):
+        return ys[:, 0] + ys[:, 1].flip(dims=[-1])
+
+
+class CrossMergeC(torch.autograd.Function):
+    """ys (B,2,D,L) -> ys[:,0] + flip_L ys[:,1] (reference :459-475).  Backward: [g, flip_L g], i.e. CrossScanC's forward."""
+
+    @staticmethod
+    def forward(ctx, ys):
+        return ys[:, 0] + ys[:, 1].flip(dims=[-1])
+
+    @staticmethod
+    def backward(ctx, g):
+        B, D, L = g.shape
+        xs = g.new_empty((B, 2, D, L))
+        xs[:, 0] = g
+        xs[:, 1] = torch.flip(g, dims=[-1])
+        return xs
+
+
+def _csc_composed_fwd(x, xw, xb, dtw, dtb, A, Df, softplus):
+    """fp32 composition for shapes the kernels reject -> (y (B, L, D), saved tensors)"""
+    B, D, L = x.shape
+    N = A.shape[1]
+    R = xw.shape[1] - 2 * N
+    xf = x.float()
+    xs = torch.stack([xf, xf.flip(-1)], 1)  # (B, 2, D, L)
+    dbl = torch.einsum("bkdl,kcd->bkcl", xs, xw)
+    if xb is not None:
+        dbl = dbl + xb.view(1, 2, -1, 1)
+    dtr, Bs, Cs = dbl[:, :, :R], dbl[:, :, R:R + N].contiguous(), dbl[:, :, R + N:].contiguous()
+    dts = torch.einsum("bkrl,kdr->bkdl", dtr, dtw).reshape(B, 2 * D, L).contiguous()
+    u = xs.view(B, 2 * D, L)
+    ys, ckpt = ops.selective_scan_fwd(u, dts, A, Bs, Cs, Df, dtb, softplus, need_ckpt=True)
+    ys = ys.view(B, 2, D, L)
+    y = (ys[:, 0] + ys[:, 1].flip(-1)).transpose(1, 2).contiguous()
+    return y, (u, dtr.contiguous(), dts, Bs, Cs, ckpt)
+
+
+def _csc_composed_bwd(saved, dy, xw, dtw, A, Df, dtb, softplus, has_bias):
+    u, dtr, dts, Bs, Cs, ckpt = saved
+    B, D2, L = u.shape
+    D = D2 // 2
+    dm = dy.transpose(1, 2)  # (B, D, L)
+    dys = torch.stack([dm, dm.flip(-1)], 1).reshape(B, 2 * D, L).contiguous()
+    du, ddelta, dA, dB, dC, dD, dbias = ops.selective_scan_bwd(u, dts, A, Bs, Cs, Df, dtb, dys, ckpt, softplus)
+    dd = ddelta.view(B, 2, D, L)
+    d_dtw = torch.einsum("bkdl,bkrl->kdr", dd, dtr)
+    ddbl = torch.cat([torch.einsum("bkdl,kdr->bkrl", dd, dtw), dB, dC], 2)  # (B, 2, R+2N, L)
+    xs = u.view(B, 2, D, L)
+    d_xw = torch.einsum("bkcl,bkdl->kcd", ddbl, xs)
+    d_xb = ddbl.sum((0, 3)) if has_bias else None
+    dxs = du.view(B, 2, D, L) + torch.einsum("bkcl,kcd->bkdl", ddbl, xw)
+    dx = dxs[:, 0] + dxs[:, 1].flip(-1)
+    g = {"x_proj_weight": d_xw, "dt_projs_weight": d_dtw, "dt_projs_bias": dbias, "A_logs": dA * A, "Ds": dD}
+    if has_bias:
+        g["x_proj_bias"] = d_xb
+    return dx, g
+
+
+class _CrossSelectiveScanC(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, x_proj_weight, x_proj_bias, dt_projs_weight, dt_projs_bias, A_logs, Ds, delta_softplus):
+        B, D, L = x.shape
+        N = A_logs.shape[1]
+        R = x_proj_weight.shape[1] - 2 * N
+        f32 = lambda t: None if t is None else t.detach().float().contiguous()
+        xw, dtw, A_logs32 = f32(x_proj_weight), f32(dt_projs_weight), f32(A_logs)
+        xb = f32(x_proj_bias).view(2, -1) if x_proj_bias is not None else None
+        dtb, Df = f32(dt_projs_bias).view(-1), f32(Ds).view(-1)
+        fused = ops.cross_scan_c_supported(D, L, R, N)
+        xd = x.detach()
+        if xd.stride(-1) != 1:
+            xd = xd.contiguous()
+        if fused:
+            y = ops.cross_selective_scan_c_fwd(xd, xw, xb, dtw, dtb, A_logs32, Df, delta_softplus)
+            ctx.save_for_backward(xd, xw, xb, dtw, dtb, A_logs32, Df)
+        else:
+            A = (-torch.exp(A_logs32)).contiguous()
+            y, saved = _csc_composed_fwd(xd, xw, xb, dtw, dtb, A, Df, delta_softplus)
+            ctx.save_for_backward(xw, dtw, dtb, A, Df, *saved)
+        ctx.geom = (B, D, L, fused, bool(delta_softplus), x.dtype, x_proj_bias is not None)
+        ctx.param_meta = {k: (t.shape, t.dtype) for k, t in (("x_proj_weight", x_proj_weight), ("x_proj_bias", x_proj_bias),
+                                                             ("dt_projs_weight", dt_projs_weight), ("dt_projs_bias", dt_projs_bias),
+                                                             ("A_logs", A_logs), ("Ds", Ds)) if t is not None}
+        return y.view(B, L, 1, D)
+
+    @staticmethod
+    def backward(ctx, dy):
+        B, D, L, fused, softplus, x_dtype, has_bias = ctx.geom
+        dy = dy.float().contiguous().view(B, L, D)
+        if fused:
+            xd, xw, xb, dtw, dtb, A_logs32, Df = ctx.saved_tensors
+            dx, g = ops.cross_selective_scan_c_bwd(xd, xw, xb, dtw, dtb, A_logs32, Df, dy, softplus)
+        else:
+            xw, dtw, dtb, A, Df, *saved = ctx.saved_tensors
+            dx, g = _csc_composed_bwd(saved, dy, xw, dtw, A, Df, dtb, softplus, has_bias)
+        meta = ctx.param_meta
+        cast = lambda k: g[k].to(meta[k][1]).view(meta[k][0]) if k in meta else None
+        return (dx.to(x_dtype), cast("x_proj_weight"), cast("x_proj_bias"), cast("dt_projs_weight"), cast("dt_projs_bias"),
+                cast("A_logs"), cast("Ds"), None)
+
+
+def cross_selective_scanC(x: torch.Tensor = None, x_proj_weight: torch.Tensor = None, x_proj_bias: torch.Tensor = None,
+                          dt_projs_weight: torch.Tensor = None, dt_projs_bias: torch.Tensor = None, A_logs: torch.Tensor = None,
+                          Ds: torch.Tensor = None, out_norm: torch.nn.Module = None, softmax_version=False, nrows=-1,
+                          delta_softplus=True, to_dtype=True):
+    """Drop-in for the reference's cross_selective_scanC (RealSR/VmambaIR/archs/MambaRealSR11_arch.py:478-534): same signature, shapes
+    and result.  x (B,D,L) fp32 / bf16 / fp16 (SS2D_1 passes the pooled (B, 1, C) descriptor: D = 1, L = C); x_proj_weight
+    (2, R+2N, D); x_proj_bias (2, R+2N) or None; dt_projs_weight (2, D, R); dt_projs_bias (2, D); A_logs (2D, N); Ds (2D); out_norm:
+    the module applied to the merged y (B, L, 1, D) fp32.  -> out_norm(y), cast to x.dtype when to_dtype.  Differentiable w.r.t. x
+    and every parameter; gradients come back in each parameter's dtype, and are bitwise reproducible on the fused path.
+
+    dtype rule: every operand is cast to fp32 and the scan runs in fp32, as the reference's SelectiveScan (custom_fwd with
+    cast_inputs=float32) does.  The one difference: x_proj and dt_proj also run in fp32 here, where an autocast caller of the
+    reference would run those two einsums in bf16.  softmax_version=True raises NotImplementedError; nrows is accepted and ignored."""
+    if softmax_version:
+        raise NotImplementedError("cross_selective_scanC: softmax_version is not supported")
+    _check_cuda(x, x_proj_weight, x_proj_bias, dt_projs_weight, dt_projs_bias, A_logs, Ds)
+    if x.dtype not in _DTYPES:
+        raise RuntimeError(f"cross_selective_scanC: x dtype must be float32/float16/bfloat16, got {x.dtype}")
+    if x.dim() != 3 or dt_projs_weight.dim() != 3 or A_logs.dim() != 2:
+        raise RuntimeError("cross_selective_scanC: expected x (B,D,L), dt_projs_weight (2,D,R), A_logs (2D,N)")
+    B, D, L = x.shape
+    K, D2, R = dt_projs_weight.shape
+    N = A_logs.shape[1]
+    if K != 2 or D2 != D or tuple(x_proj_weight.shape) != (2, R + 2 * N, D) or tuple(A_logs.shape) != (2 * D, N) \
+            or Ds.numel() != 2 * D or dt_projs_bias.numel() != 2 * D or (x_proj_bias is not None and x_proj_bias.numel() != 2 * (R + 2 * N)):
+        raise RuntimeError("cross_selective_scanC: expected x (B,D,L), x_proj_weight (2,R+2N,D), x_proj_bias (2,R+2N), "
+                           "dt_projs_weight (2,D,R), dt_projs_bias (2,D), A_logs (2D,N), Ds (2D)")
+    with torch.autocast("cuda", enabled=False):
+        y = _CrossSelectiveScanC.apply(x, x_proj_weight, x_proj_bias, dt_projs_weight, dt_projs_bias, A_logs, Ds, bool(delta_softplus))
     y = out_norm(y)
     if to_dtype:
         y = y.to(x.dtype)

@@ -8,6 +8,7 @@ library owns nothing), on the input's device and current stream.
 from __future__ import annotations
 
 import ctypes as C
+import math
 
 import torch
 
@@ -389,6 +390,70 @@ def selective_scan_bwd_grouped(us, deltas, Bs, Cs, douts, revs, A, D, delta_bias
     with torch.cuda.device(dev), _timed("scan_bwd", nbytes, dev, 2):
         _lib.check(Lb.vmb_selective_scan_bwd_grouped(C.byref(a), _stream(us[0])), "selective_scan_bwd_grouped")
     return dus, dds, dA, dBs, dCs, dD, dbias
+
+
+_CSC_SMEM_LIMIT = 227 * 1024
+
+
+def cross_scan_c_supported(D, L, R, N) -> bool:
+    """True when vmb_cross_selective_scan_c_fwd / _bwd take (D, L, R, N) on one CTA per image: d_state <= 16, D <= 16 and the
+    backward's shared memory within 227 KB (the library's own check)."""
+    s = _lib.lib().vmb_cross_selective_scan_c_smem_bytes(int(D), int(L), int(R), int(N))
+    return 0 < s <= _CSC_SMEM_LIMIT
+
+
+def _csc_args(x, xw, xb, dtw, dtb, A_logs, Ds, y, delta_softplus):
+    b, D, L = x.shape
+    K, RN, D2 = xw.shape
+    N = A_logs.shape[1]
+    R = RN - 2 * N
+    if x.dtype not in _DT or not x.is_cuda or x.stride(2) != 1:
+        raise RuntimeError("cross_selective_scan_c: x must be a float32/bfloat16/float16 CUDA tensor (B, D, L) with stride(-1) == 1")
+    for n, t, shp in (("x_proj_weight", xw, (2, RN, D)), ("x_proj_bias", xb, (2, RN)), ("dt_projs_weight", dtw, (2, D, R)),
+                      ("dt_projs_bias", dtb, (2 * D,)), ("A_logs", A_logs, (2 * D, N)), ("Ds", Ds, (2 * D,))):
+        if t is None and n == "x_proj_bias":
+            continue
+        if t.dtype != torch.float32 or not t.is_contiguous() or t.device != x.device or tuple(t.shape) != shp:
+            raise RuntimeError(f"cross_selective_scan_c: {n} must be a contiguous float32 tensor of shape {shp} on x's device")
+    return _lib.CrossScanCArgs(_ptr(x), _ptr(xw), _ptr(xb), _ptr(dtw), _ptr(dtb), _ptr(A_logs), _ptr(Ds), _ptr(y),
+                               b, D, L, R, N, x.stride(0), x.stride(1), int(bool(delta_softplus)), _DT[x.dtype])
+
+
+def cross_selective_scan_c_fwd(x, x_proj_weight, x_proj_bias, dt_projs_weight, dt_projs_bias, A_logs, Ds, delta_softplus=True):
+    """Two-direction channel scan, one launch: x (B, D, L) any of the three dtypes; parameters fp32 contiguous, x_proj_weight (2, R+2N, D),
+    x_proj_bias (2, R+2N) or None, dt_projs_weight (2, D, R), dt_projs_bias (2D), A_logs (2D, N), Ds (2D).
+    -> y fp32 (B, L, D) = y_0 + flip(y_1) (include/vmambair_b200.h, vmb_cross_selective_scan_c_fwd)."""
+    b, D, L = x.shape
+    y = torch.empty((b, L, D), dtype=torch.float32, device=x.device)
+    a = _csc_args(x, x_proj_weight, x_proj_bias, dt_projs_weight, dt_projs_bias, A_logs, Ds, y, delta_softplus)
+    _run("vmb_cross_selective_scan_c_fwd", a, x, "cscan_c_fwd")
+    return y
+
+
+def cross_selective_scan_c_bwd(x, x_proj_weight, x_proj_bias, dt_projs_weight, dt_projs_bias, A_logs, Ds, dy, delta_softplus=True):
+    """Backward of cross_selective_scan_c_fwd (two launches: the per-image kernel and the fixed-order batch sum).  dy: fp32 (B, L, D).
+    -> (dx (B, D, L) in x's dtype, {name: fp32 gradient shaped like the parameter}); "x_proj_bias" only when the bias is given."""
+    b, D, L = x.shape
+    K, RN, _ = x_proj_weight.shape
+    N = A_logs.shape[1]
+    R = RN - 2 * N
+    if dy.dtype != torch.float32 or tuple(dy.shape) != (b, L, D) or not dy.is_contiguous() or dy.device != x.device:
+        raise RuntimeError(f"cross_selective_scan_c_bwd: dy must be a contiguous float32 tensor of shape {(b, L, D)}")
+    dx = torch.empty((b, D, L), dtype=x.dtype, device=x.device)
+    sizes = [("x_proj_weight", (2, RN, D)), ("x_proj_bias", (2, RN)), ("dt_projs_weight", (2, D, R)), ("dt_projs_bias", (2 * D,)),
+             ("A_logs", (2 * D, N)), ("Ds", (2 * D,))]
+    flat = torch.empty(sum(math.prod(s) for _, s in sizes), dtype=torch.float32, device=x.device)
+    ws = torch.empty(_lib.lib().vmb_cross_selective_scan_c_workspace_bytes(b, D, R, N) // 4, dtype=torch.float32, device=x.device)
+    a = _lib.CrossScanCBwdArgs(_csc_args(x, x_proj_weight, x_proj_bias, dt_projs_weight, dt_projs_bias, A_logs, Ds, None, delta_softplus),
+                               _ptr(dy), _ptr(dx), _ptr(flat), _ptr(ws))
+    _run("vmb_cross_selective_scan_c_bwd", a, x, "cscan_c_bwd", 0, 2)
+    grads, o = {}, 0
+    for n, s in sizes:
+        k = math.prod(s)
+        if n != "x_proj_bias" or x_proj_bias is not None:
+            grads[n] = flat[o:o + k].view(s)
+        o += k
+    return dx, grads
 
 
 def merge_sum(ys, C_, H, W, in_place_order=False, out=None):
