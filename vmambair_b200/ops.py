@@ -613,7 +613,7 @@ def pixlin_wgrad(dy, x, per_batch=False, out=None, dbias=None):
           and all(s % 8 == 0 for s in (dy.stride(0), dy.stride(1), x.stride(0), x.stride(1)))
           and dy.data_ptr() % 16 == 0 and x.data_ptr() % 16 == 0)
     if not ok:
-        wb = torch.bmm(dy, x.transpose(1, 2)).float()
+        wb = torch.bmm(dy.float(), x.float().transpose(1, 2))  # fp32 operands: a 16-bit bmm would round dW to 16 bits
         if dbias is not None:
             dbias += dy.float().sum((0, 2))
         res = wb if per_batch else wb.sum(0)
@@ -640,9 +640,12 @@ def prep_block_weights(jobs, dtype):
 
 
 def sum4_add(x4, add):
-    """x4 (B,4,C,L) contiguous, add (B,C,L) contiguous -> add + x4.sum(1) (fp32 accumulation, result in the input dtype)"""
+    """x4 (B,4,C,L) contiguous, add (B,C,L) contiguous -> add + x4.sum(1) (fp32 accumulation, result in the input dtype).
+    The kernel moves 16 B vectors; C*L not a multiple of the vector width, or an operand not 16 B aligned, takes the same sum in torch."""
     B = x4.shape[0]
     assert x4.is_contiguous() and add.is_contiguous() and x4.dtype == add.dtype
+    if add[0].numel() % (16 // add.element_size()) or x4.data_ptr() % 16 or add.data_ptr() % 16:
+        return (add.float() + x4.float().sum(1)).to(add.dtype)
     out = torch.empty_like(add)
     global _LAUNCHES
     with torch.cuda.device(x4.device):
