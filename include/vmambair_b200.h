@@ -44,7 +44,11 @@ int vmb_scan_ckpt_interval(void);
  *   D, delta_bias : (dim) fp32 or NULL
  *   ckpt          : fp32 (batch, dim, n_ckpt, dstate) or NULL (inference: no checkpoints)
  * out = D*u + sum_n C_n * h_n,   h_n,l = exp(dt_l*A_n) h_n,l-1 + dt_l*u_l*B_n,l,
- * dt = softplus?(delta + delta_bias).  State and accumulation in fp32. */
+ * dt = softplus?(delta + delta_bias).  State and accumulation in fp32.
+ *   out_f32       : 0 -> `out` has dtype `dt`;  1 (bf16 / fp16 `dt` only) -> `out` is fp32, the fp32 accumulator stored without
+ *                   rounding: selective_scan_cuda_oflex.fwd(..., out_float=True) (cusoflex/selective_scan_oflex.cpp:157-243,
+ *                   out allocated at :219, the <input_t, weight_t, float> kernel at :238).  Last member: a zero-initialised
+ *                   struct keeps the plain operator. */
 typedef struct {
     const void* u; const void* delta; const float* A; const void* Bm; const void* Cm;
     const float* D; const float* delta_bias; void* out; float* ckpt;
@@ -55,7 +59,8 @@ typedef struct {
     int64_t B_bs, B_gs, B_ns;   /* batch / group / state strides  */
     int64_t C_bs, C_gs, C_ns;
     int delta_softplus;
-    int dtype; /* vmb_dtype of u, delta, Bm, Cm, out */
+    int dtype; /* vmb_dtype of u, delta, Bm, Cm, out (out: fp32 when out_f32) */
+    int out_f32;
 } vmb_scan_fwd_args;
 int vmb_selective_scan_fwd(const vmb_scan_fwd_args* a, void* stream);
 
@@ -90,7 +95,11 @@ int vmb_selective_scan_fwd_grouped(const vmb_scan_grouped_args* a, void* stream)
  *       `workspace` and the cast is done by the library)
  *   workspace : device scratch of vmb_scan_bwd_workspace_bytes(...) bytes, 16 B aligned; the library
  *       zero-fills it on `stream`
- *   ckpt  : as written by the forward (required when seqlen > interval). */
+ *   ckpt  : as written by the forward (required when seqlen > interval).
+ *   dout_f32 : 0 -> dout has dtype `dt`;  1 (bf16 / fp16 `dt` only) -> dout is fp32, read without rounding:
+ *       selective_scan_cuda_oflex.bwd (cusoflex/selective_scan_oflex.cpp:245-358; output_type == Float at :260, :353).
+ *       du, ddelta, dB, dC keep dtype `dt`; dA, dD, ddelta_bias stay fp32 (cpp:324-356).  Last member: zero keeps the
+ *       plain operator. */
 typedef struct {
     const void* u; const void* delta; const float* A; const void* Bm; const void* Cm;
     const float* D; const float* delta_bias; const void* dout; const float* ckpt;
@@ -101,6 +110,7 @@ typedef struct {
     int64_t B_bs, B_gs, B_ns, C_bs, C_gs, C_ns;
     int delta_softplus;
     int dtype;
+    int dout_f32;
 } vmb_scan_bwd_args;
 int vmb_selective_scan_bwd(const vmb_scan_bwd_args* a, void* stream);
 int64_t vmb_scan_bwd_workspace_bytes(int batch, int ngroups, int dstate, int seqlen);

@@ -24,7 +24,7 @@ class ScanFwdArgs(C.Structure):
         ("batch", C.c_int), ("dim", C.c_int), ("seqlen", C.c_int), ("dstate", C.c_int), ("ngroups", C.c_int),
         ("u_bs", i64), ("u_ds", i64), ("delta_bs", i64), ("delta_ds", i64), ("out_bs", i64), ("out_ds", i64),
         ("B_bs", i64), ("B_gs", i64), ("B_ns", i64), ("C_bs", i64), ("C_gs", i64), ("C_ns", i64),
-        ("delta_softplus", C.c_int), ("dtype", C.c_int),
+        ("delta_softplus", C.c_int), ("dtype", C.c_int), ("out_f32", C.c_int),
     ]
 
 
@@ -37,7 +37,7 @@ class ScanBwdArgs(C.Structure):
         ("u_bs", i64), ("u_ds", i64), ("delta_bs", i64), ("delta_ds", i64), ("dout_bs", i64), ("dout_ds", i64),
         ("du_bs", i64), ("du_ds", i64), ("ddelta_bs", i64), ("ddelta_ds", i64),
         ("B_bs", i64), ("B_gs", i64), ("B_ns", i64), ("C_bs", i64), ("C_gs", i64), ("C_ns", i64),
-        ("delta_softplus", C.c_int), ("dtype", C.c_int),
+        ("delta_softplus", C.c_int), ("dtype", C.c_int), ("dout_f32", C.c_int),
     ]
 
 

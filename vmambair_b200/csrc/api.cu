@@ -51,6 +51,8 @@ extern "C" int vmb_selective_scan_fwd(const vmb_scan_fwd_args* a, void* stream) 
     VMB_CHECK(a->dim % a->ngroups == 0, "selective_scan_fwd: dims should be dividable by n_groups");
     VMB_CHECK(a->dstate <= 256, "selective_scan only supports state dimension <= 256");
     VMB_CHECK(a->batch <= 65535, "selective_scan_fwd: batch > 65535");
+    VMB_CHECK(a->out_f32 == 0 || a->out_f32 == 1, "selective_scan_fwd: out_f32 must be 0 or 1 (got %d)", a->out_f32);
+    VMB_CHECK(!a->out_f32 || a->dtype == VMB_BF16 || a->dtype == VMB_F16, "selective_scan_fwd: out_f32 needs bf16 / fp16 inputs");
     ScanFwdParams p{};
     p.u = a->u; p.delta = a->delta; p.Bm = a->Bm; p.Cm = a->Cm; p.A = a->A; p.D = a->D; p.bias = a->delta_bias;
     p.out = a->out; p.ckpt = a->ckpt;
@@ -61,13 +63,14 @@ extern "C" int vmb_selective_scan_fwd(const vmb_scan_fwd_args* a, void* stream) 
     p.u_bs = a->u_bs; p.u_ds = a->u_ds; p.dl_bs = a->delta_bs; p.dl_ds = a->delta_ds; p.o_bs = a->out_bs; p.o_ds = a->out_ds;
     p.B_bs = a->B_bs; p.B_gs = a->B_gs; p.B_ns = a->B_ns; p.C_bs = a->C_bs; p.C_gs = a->C_gs; p.C_ns = a->C_ns;
     p.softplus = a->delta_softplus;
-    const int v = 16 / elt_size(a->dtype);
+    const int v = 16 / elt_size(a->dtype), vo = a->out_f32 ? 4 : v;  // 16 B rows of `out` in its own element type
     auto mult = [v](int64_t s) { return s % v == 0; };
+    auto mult_o = [vo](int64_t s) { return s % vo == 0; };
     p.vec_ok = aligned16(a->u) && aligned16(a->delta) && aligned16(a->Bm) && aligned16(a->Cm) && aligned16(a->out) &&
-               mult(a->u_bs) && mult(a->u_ds) && mult(a->delta_bs) && mult(a->delta_ds) && mult(a->out_bs) &&
-               mult(a->out_ds) && mult(a->B_bs) && mult(a->B_gs) && mult(a->B_ns) && mult(a->C_bs) && mult(a->C_gs) &&
+               mult(a->u_bs) && mult(a->u_ds) && mult(a->delta_bs) && mult(a->delta_ds) && mult_o(a->out_bs) &&
+               mult_o(a->out_ds) && mult(a->B_bs) && mult(a->B_gs) && mult(a->B_ns) && mult(a->C_bs) && mult(a->C_gs) &&
                mult(a->C_ns);
-    return scan_fwd_launch(p, a->dtype, static_cast<cudaStream_t>(stream));
+    return scan_fwd_launch(p, a->dtype, static_cast<cudaStream_t>(stream), a->out_f32 != 0);
 }
 
 extern "C" int64_t vmb_scan_bwd_workspace_bytes(int batch, int ngroups, int dstate, int seqlen) {
@@ -92,6 +95,8 @@ extern "C" int vmb_selective_scan_bwd(const vmb_scan_bwd_args* a, void* stream) 
     VMB_CHECK((a->D == nullptr) == (a->dD == nullptr), "selective_scan_bwd: D and dD must both be given or both be NULL");
     VMB_CHECK((a->delta_bias == nullptr) == (a->ddelta_bias == nullptr),
               "selective_scan_bwd: delta_bias and ddelta_bias must both be given or both be NULL");
+    VMB_CHECK(a->dout_f32 == 0 || a->dout_f32 == 1, "selective_scan_bwd: dout_f32 must be 0 or 1 (got %d)", a->dout_f32);
+    VMB_CHECK(!a->dout_f32 || a->dtype == VMB_BF16 || a->dtype == VMB_F16, "selective_scan_bwd: dout_f32 needs bf16 / fp16 inputs");
     ScanBwdParams p{};
     p.u = a->u; p.delta = a->delta; p.Bm = a->Bm; p.Cm = a->Cm; p.dout = a->dout; p.A = a->A; p.D = a->D;
     p.bias = a->delta_bias; p.ckpt = a->ckpt; p.du = a->du; p.ddelta = a->ddelta; p.dA = a->dA; p.dB = a->dB; p.dC = a->dC;
@@ -104,14 +109,15 @@ extern "C" int vmb_selective_scan_bwd(const vmb_scan_bwd_args* a, void* stream) 
     p.du_bs = a->du_bs; p.du_ds = a->du_ds; p.dd_bs = a->ddelta_bs; p.dd_ds = a->ddelta_ds;
     p.B_bs = a->B_bs; p.B_gs = a->B_gs; p.B_ns = a->B_ns; p.C_bs = a->C_bs; p.C_gs = a->C_gs; p.C_ns = a->C_ns;
     p.softplus = a->delta_softplus;
-    const int v = 16 / elt_size(a->dtype);
+    const int v = 16 / elt_size(a->dtype), vg = a->dout_f32 ? 4 : v;  // 16 B rows of dout in its own element type
     auto mult = [v](int64_t s) { return s % v == 0; };
+    auto mult_g = [vg](int64_t s) { return s % vg == 0; };
     p.vec_ok = aligned16(a->u) && aligned16(a->delta) && aligned16(a->Bm) && aligned16(a->Cm) && aligned16(a->dout) &&
                aligned16(a->du) && aligned16(a->ddelta) && aligned16(a->workspace) && mult(a->u_bs) && mult(a->u_ds) && mult(a->delta_bs) &&
-               mult(a->delta_ds) && mult(a->dout_bs) && mult(a->dout_ds) && mult(a->du_bs) && mult(a->du_ds) &&
+               mult(a->delta_ds) && mult_g(a->dout_bs) && mult_g(a->dout_ds) && mult(a->du_bs) && mult(a->du_ds) &&
                mult(a->ddelta_bs) && mult(a->ddelta_ds) && mult(a->B_bs) && mult(a->B_gs) && mult(a->B_ns) &&
                mult(a->C_bs) && mult(a->C_gs) && mult(a->C_ns);
-    return scan_bwd_launch(p, a->dtype, static_cast<cudaStream_t>(stream));
+    return scan_bwd_launch(p, a->dtype, static_cast<cudaStream_t>(stream), a->dout_f32 != 0);
 }
 
 static inline bool dt_ok(int d) { return d == VMB_F32 || d == VMB_BF16 || d == VMB_F16; }

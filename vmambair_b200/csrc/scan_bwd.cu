@@ -18,14 +18,16 @@
 // reference does one scalar atomicAdd per ROW per (n,l) (bwd kernel :209-221) and casts in torch.
 #include <stdlib.h>
 
+#include <type_traits>
+
 #include "scan_common.cuh"
 
 namespace vmb {
 
-template <typename in_t, int RB>
+template <typename in_t, int RB, int NIO = 3>
 struct BwdSmem {
     using Cfg = FwdCfg<RB>;
-    using R = RawCfg<in_t, RB, 3>;
+    using R = RawCfg<in_t, RB, NIO>;
     static constexpr size_t red_bytes = sizeof(float4) * Cfg::SEGW * T * RB;  // [sl][t][r] float4
     static size_t bytes(int npad) {
         return sizeof(float4) * (2 * 8 * Cfg::SLOTS) + R::bytes + red_bytes + sizeof(float) * (4 * RB * npad + RB);
@@ -37,11 +39,15 @@ __device__ __forceinline__ void red_add_f32x4(float4* addr, float4 v) {
                  : "memory");
 }
 
-template <typename in_t, int RB>
+// g_t: element type of dout.  float with 16-bit in_t (selective_scan_cuda_oflex's fp32 dout): dout is read straight from global
+// memory (16 B vectors when aligned) and only u / delta are staged (NIO = 2); every output keeps its type.
+template <typename in_t, int RB, typename g_t>
 __global__ void __launch_bounds__(32, 8) scan_bwd_kernel(const ScanBwdParams p) {
     pdl_wait();
+    constexpr bool G_IN = std::is_same<g_t, in_t>::value;
+    constexpr int NIO = G_IN ? 3 : 2;
     using Cfg = FwdCfg<RB>;
-    using R = RawCfg<in_t, RB, 3>;
+    using R = RawCfg<in_t, RB, NIO>;
     constexpr int SEGW = Cfg::SEGW, CHUNK = Cfg::CHUNK, SEGQ = Cfg::SEGQ, SLOTS = Cfg::SLOTS;
     constexpr int V = Vec<in_t>::N;
 
@@ -80,7 +86,7 @@ __global__ void __launch_bounds__(32, 8) scan_bwd_kernel(const ScanBwdParams p) 
     const float* __restrict__ ckrow = p.ckpt + ((int64_t)b * p.dim + d0) * p.n_ckpt * N;  // + (rr*n_ckpt + k)*N + n
 
     const int nchunks = (L + CHUNK - 1) / CHUNK;
-    if (async_ok) prefetch_chunk<in_t, RB, 3>(raw, io_base, io_ds, Bg, Cg, p.B_ns, p.C_ns, N, (nchunks - 1) * CHUNK, L, lane);
+    if (async_ok) prefetch_chunk<in_t, RB, NIO>(raw, io_base, io_ds, Bg, Cg, p.B_ns, p.C_ns, N, (nchunks - 1) * CHUNK, L, lane);
     for (int i = lane; i < RB * npad; i += 32) {
         const int rr = i / npad, n = i % npad;
         sA[i] = n < N ? p.A[(int64_t)(d0 + rr) * N + n] * kLog2e : 0.f;
@@ -101,23 +107,29 @@ __global__ void __launch_bounds__(32, 8) scan_bwd_kernel(const ScanBwdParams p) 
         if (async_ok) {
             cp_async_wait_all();
             __syncwarp();
-            convert_bc<in_t, RB, 3>(sB, raw + (3 * RB) * R::PITCH, lane);
-            convert_bc<in_t, RB, 3>(sC, raw + (3 * RB + 16) * R::PITCH, lane);
+            convert_bc<in_t, RB, NIO>(sB, raw + (NIO * RB) * R::PITCH, lane);
+            convert_bc<in_t, RB, NIO>(sC, raw + (NIO * RB + 16) * R::PITCH, lane);
 #pragma unroll
             for (int v = 0; v < T / V; ++v) {
                 load_vec_smem<in_t>(raw + r * R::PITCH + sl * T + v * V, uv + v * V);
                 load_vec_smem<in_t>(raw + (RB + r) * R::PITCH + sl * T + v * V, dt + v * V);
-                load_vec_smem<in_t>(raw + (2 * RB + r) * R::PITCH + sl * T + v * V, go + v * V);
+                if constexpr (G_IN) load_vec_smem<in_t>(raw + (2 * RB + r) * R::PITCH + sl * T + v * V, go + v * V);
             }
             __syncwarp();
-            if (ci > 0) prefetch_chunk<in_t, RB, 3>(raw, io_base, io_ds, Bg, Cg, p.B_ns, p.C_ns, N, c0 - CHUNK, L, lane);
+            if (ci > 0) prefetch_chunk<in_t, RB, NIO>(raw, io_base, io_ds, Bg, Cg, p.B_ns, p.C_ns, N, c0 - CHUNK, L, lane);
         } else {
 #pragma unroll
             for (int v = 0; v < T / V; ++v) {
                 load_vec<in_t>(urow + l0 + v * V, uv + v * V, valid - v * V, false);
                 load_vec<in_t>(drow + l0 + v * V, dt + v * V, valid - v * V, false);
-                load_vec<in_t>(gorow + l0 + v * V, go + v * V, valid - v * V, false);
+                if constexpr (G_IN) load_vec<in_t>(gorow + l0 + v * V, go + v * V, valid - v * V, false);
             }
+        }
+        if constexpr (!G_IN) {
+            constexpr int VG = Vec<g_t>::N;
+            const g_t* __restrict__ grow = reinterpret_cast<const g_t*>(p.dout) + (int64_t)b * p.do_bs + (int64_t)d * p.do_ds;
+#pragma unroll
+            for (int v = 0; v < T / VG; ++v) load_vec<g_t>(grow + l0 + v * VG, go + v * VG, valid - v * VG, p.vec_ok);
         }
         // forward state at the chunk start (checkpoint written by the forward; zero for the first chunk)
         for (int i = lane; i < RB * npad; i += 32) {
@@ -339,10 +351,10 @@ __global__ void scan_bwd_finalize_kernel(const float4* __restrict__ scratch, in_
     }
 }
 
-template <typename in_t, int RB>
+template <typename in_t, int RB, typename g_t>
 static int launch_cfg(const ScanBwdParams& p, cudaStream_t stream) {
-    auto kern = scan_bwd_kernel<in_t, RB>;
-    const size_t smem = BwdSmem<in_t, RB>::bytes(p.npad);
+    auto kern = scan_bwd_kernel<in_t, RB, g_t>;
+    const size_t smem = BwdSmem<in_t, RB, std::is_same<g_t, in_t>::value ? 3 : 2>::bytes(p.npad);
     VMB_CHECK(smem <= 227 * 1024, "selective_scan_bwd: dstate=%d needs %zu B of shared memory", p.N, smem);
     if (smem > 48 * 1024) VMB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const long blocks = (long)p.batch * (p.dim / RB);
@@ -370,8 +382,9 @@ template <> struct DtOf<float> { static constexpr int v = VMB_F32; };
 template <> struct DtOf<__nv_bfloat16> { static constexpr int v = VMB_BF16; };
 template <> struct DtOf<__half> { static constexpr int v = VMB_F16; };
 
-template <typename in_t>
+template <typename in_t, typename g_t = in_t>
 static int launch_t(const ScanBwdParams& p_in, cudaStream_t stream) {
+    constexpr bool dout_f32 = !std::is_same<g_t, in_t>::value;
     ScanBwdParams p = p_in;
     if (const char* e = getenv("VMB_BWD_NORED")) p.debug_nored = atoi(e);
     const size_t scratch_bytes = sizeof(float4) * (size_t)p.batch * p.G * (p.npad / 2) * p.L;
@@ -379,13 +392,13 @@ static int launch_t(const ScanBwdParams& p_in, cudaStream_t stream) {
     int rc;
     int trb, tss;
     if (scan_bwd_tma_pick(p, DtOf<in_t>::v, trb, tss)) {  // fast path: TMA-staged 4-warp CTAs (scan_bwd_tma.cu)
-        rc = scan_bwd_tma_launch(p, DtOf<in_t>::v, trb, tss, stream);
+        rc = scan_bwd_tma_launch(p, DtOf<in_t>::v, trb, tss, stream, dout_f32);
     } else
     switch (pick_rb_bwd(p)) {
-        case 8: rc = launch_cfg<in_t, 8>(p, stream); break;
-        case 4: rc = launch_cfg<in_t, 4>(p, stream); break;
-        case 2: rc = launch_cfg<in_t, 2>(p, stream); break;
-        default: rc = launch_cfg<in_t, 1>(p, stream); break;
+        case 8: rc = launch_cfg<in_t, 8, g_t>(p, stream); break;
+        case 4: rc = launch_cfg<in_t, 4, g_t>(p, stream); break;
+        case 2: rc = launch_cfg<in_t, 2, g_t>(p, stream); break;
+        default: rc = launch_cfg<in_t, 1, g_t>(p, stream); break;
     }
     if (rc != VMB_OK) return rc;
     const long total = (long)p.batch * p.G * (p.npad / 2) * p.L;
@@ -396,8 +409,16 @@ static int launch_t(const ScanBwdParams& p_in, cudaStream_t stream) {
     return VMB_OK;
 }
 
-int scan_bwd_launch(const ScanBwdParams& p, int dtype, cudaStream_t stream) {
+int scan_bwd_launch(const ScanBwdParams& p, int dtype, cudaStream_t stream, bool dout_f32) {
     VMB_CHECK((long)p.batch * p.dim < (1L << 31), "selective_scan_bwd: batch*dim too large");
+    if (dout_f32) {  // fp32 dout against 16-bit inputs
+        switch (dtype) {
+            case VMB_BF16: return launch_t<__nv_bfloat16, float>(p, stream);
+            case VMB_F16: return launch_t<__half, float>(p, stream);
+        }
+        set_error("selective_scan_bwd: fp32 dout needs bf16 / fp16 inputs (dtype %d)", dtype);
+        return VMB_ERR_INVALID;
+    }
     switch (dtype) {
         case VMB_F32: return launch_t<float>(p, stream);
         case VMB_BF16: return launch_t<__nv_bfloat16>(p, stream);

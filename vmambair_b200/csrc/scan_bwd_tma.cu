@@ -32,7 +32,8 @@ struct ScanBwdTmaMapsG : ScanBwdTmaMapsN<4> {
 template <bool GRP>
 using BwdMaps = typename std::conditional<GRP, ScanBwdTmaMapsG, ScanBwdTmaMapsN<1>>::type;
 
-template <typename in_t, int RB, int SS>
+// g_t: element type of dout (float with 16-bit in_t: selective_scan_cuda_oflex's fp32 dout); its tile has its own width
+template <typename in_t, int RB, int SS, typename g_t = in_t>
 struct BwdTmaCfg {
     using Cfg = FwdCfg<RB>;
     static constexpr int NW = 4;
@@ -42,15 +43,16 @@ struct BwdTmaCfg {
     static constexpr int CELLS = SEGW * T;                      // positions of a warp-chunk (= CHUNK)
     static constexpr int RED_RS = SEGW * (T + 1) + 4;           // float4 slots of one row of a warp's dB/dC transpose: [segment][T + 1 pad] (+4: rows half a wavefront apart)
     static constexpr int RED_F4 = RED_RS * RB + 8;              // (odd segment pitch: conflict-free writes by (row, segment) lanes, contiguous reads)
-    static constexpr size_t io_bytes = sizeof(in_t) * (size_t)ROWS * CHUNK;  // one of rawU / rawD / rawG
+    static constexpr size_t io_bytes = sizeof(in_t) * (size_t)ROWS * CHUNK;  // one of rawU / rawD
+    static constexpr size_t g_bytes = sizeof(g_t) * (size_t)ROWS * CHUNK;    // rawG
     static constexpr size_t bc_bytes = sizeof(in_t) * (size_t)16 * CHUNK;
     static constexpr size_t tile_bytes = sizeof(float4) * (size_t)16 * SLOTS;
     static constexpr size_t red_bytes = sizeof(float4) * (size_t)RED_F4;
     static constexpr size_t warp_f32 = 4 * RB * 16 + RB;  // sSt, sCarryD, sA, sdA [RB][16] + sDtNext [RB]
     static constexpr size_t warp_bytes = red_bytes + sizeof(float) * ((warp_f32 + 3) / 4 * 4);
     static constexpr size_t part_bytes = SS > 1 ? sizeof(float) * (size_t)(NW / SS) * (SS - 1) * 2 * T * 32 : 0;
-    static constexpr size_t smem_bytes = 3 * io_bytes + 2 * bc_bytes + tile_bytes + NW * warp_bytes + part_bytes + 16;
-    static constexpr uint32_t tx_bytes = (uint32_t)(3 * io_bytes + 2 * bc_bytes);
+    static constexpr size_t smem_bytes = 2 * io_bytes + g_bytes + 2 * bc_bytes + tile_bytes + NW * warp_bytes + part_bytes + 16;
+    static constexpr uint32_t tx_bytes = (uint32_t)(2 * io_bytes + g_bytes + 2 * bc_bytes);
 };
 
 __device__ __forceinline__ void red_add_f32x4_g(float4* addr, float4 v) {
@@ -71,11 +73,12 @@ __device__ __forceinline__ void named_bar_sync(int idx, int count) {
 
 // GRP: per-group sources and destinations (vmb_selective_scan_bwd_grouped); a reversed group loads mirrored boxes (m0 = L - c0 - CHUNK,
 // underflow zero-filled as in the forward), reads them back to front and stores du / ddelta at memory index L-1-l.
-template <typename in_t, int RB, int SS, bool GRP>
+// g_t = float with 16-bit in_t (flat operator only): fp32 dout, converted on read; every output keeps its type.
+template <typename in_t, int RB, int SS, bool GRP, typename g_t>
 __global__ void __launch_bounds__(128, sizeof(in_t) == 4 ? 1 : 2)
     scan_bwd_tma_kernel(const ScanBwdParams p, const __grid_constant__ BwdMaps<GRP> maps) {
     pdl_wait();
-    using K = BwdTmaCfg<in_t, RB, SS>;
+    using K = BwdTmaCfg<in_t, RB, SS, g_t>;
     using Cfg = FwdCfg<RB>;
     constexpr int SEGW = Cfg::SEGW, CHUNK = Cfg::CHUNK, SEGQ = Cfg::SEGQ, SLOTS = Cfg::SLOTS;
     constexpr int V = Vec<in_t>::N, NW = K::NW, NT = 32 * NW, ROWS = K::ROWS, NPW = K::NPW;
@@ -85,10 +88,10 @@ __global__ void __launch_bounds__(128, sizeof(in_t) == 4 ? 1 : 2)
     unsigned char* smem_raw = smem_dyn + ((128u - (smem_addr(smem_dyn) & 127u)) & 127u);
     in_t* rawU = reinterpret_cast<in_t*>(smem_raw);
     in_t* rawD = reinterpret_cast<in_t*>(smem_raw + K::io_bytes);
-    in_t* rawG = reinterpret_cast<in_t*>(smem_raw + 2 * K::io_bytes);
-    in_t* rawB = reinterpret_cast<in_t*>(smem_raw + 3 * K::io_bytes);
-    in_t* rawC = reinterpret_cast<in_t*>(smem_raw + 3 * K::io_bytes + K::bc_bytes);
-    float4* sB = reinterpret_cast<float4*>(smem_raw + 3 * K::io_bytes + 2 * K::bc_bytes);
+    g_t* rawG = reinterpret_cast<g_t*>(smem_raw + 2 * K::io_bytes);
+    in_t* rawB = reinterpret_cast<in_t*>(smem_raw + 2 * K::io_bytes + K::g_bytes);
+    in_t* rawC = reinterpret_cast<in_t*>(smem_raw + 2 * K::io_bytes + K::g_bytes + K::bc_bytes);
+    float4* sB = reinterpret_cast<float4*>(smem_raw + 2 * K::io_bytes + K::g_bytes + 2 * K::bc_bytes);
     float4* sC = sB + 8 * SLOTS;
     unsigned char* after_tile = reinterpret_cast<unsigned char*>(sC + 8 * SLOTS);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -175,7 +178,18 @@ __global__ void __launch_bounds__(128, sizeof(in_t) == 4 ? 1 : 2)
         if (ci < nchunks - 1) __syncthreads();  // every warp is done with the previous fp32 tile
         convert_bc_dense<in_t, RB, NT>(sB, rawB, tid, GRP && rev);
         convert_bc_dense<in_t, RB, NT>(sC, rawC, tid, GRP && rev);
-        {
+        if constexpr (!std::is_same<g_t, in_t>::value) {  // fp32 dout: its own vector width
+            static_assert(!GRP, "scan_bwd_tma: fp32 dout is a flat-operator mode");
+            constexpr int VG = Vec<g_t>::N;
+            const int row = rs * RB + r;
+#pragma unroll
+            for (int v = 0; v < T / V; ++v) {
+                load_vec_smem<in_t>(rawU + row * CHUNK + sl * T + v * V, uv + v * V);
+                load_vec_smem<in_t>(rawD + row * CHUNK + sl * T + v * V, dt + v * V);
+            }
+#pragma unroll
+            for (int v = 0; v < T / VG; ++v) load_vec_smem<g_t>(rawG + row * CHUNK + sl * T + v * VG, go + v * VG);
+        } else {
             const int row = rs * RB + r;
             if (!GRP || !rev) {
 #pragma unroll
@@ -465,10 +479,10 @@ __global__ void __launch_bounds__(128, sizeof(in_t) == 4 ? 1 : 2)
 }
 
 // ---------------------------------------------------------------------------------------------------- host
-template <typename in_t, int RB, int SS, bool GRP>
+template <typename in_t, int RB, int SS, bool GRP, typename g_t>
 static int launch_bt3(const ScanBwdParams& p, const BwdMaps<GRP>& maps, cudaStream_t stream) {
-    using K = BwdTmaCfg<in_t, RB, SS>;
-    auto kern = scan_bwd_tma_kernel<in_t, RB, SS, GRP>;
+    using K = BwdTmaCfg<in_t, RB, SS, g_t>;
+    auto kern = scan_bwd_tma_kernel<in_t, RB, SS, GRP, g_t>;
     constexpr size_t smem = K::smem_bytes + 128;
     static_assert(sizeof(in_t) == 4 ? smem <= 227 * 1024 : smem <= 113 * 1024, "scan_bwd_tma: two CTAs per SM (one for fp32 I/O)");
     VMB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -478,18 +492,18 @@ static int launch_bt3(const ScanBwdParams& p, const BwdMaps<GRP>& maps, cudaStre
     return VMB_OK;
 }
 
-template <typename in_t, int RB, bool GRP>
+template <typename in_t, int RB, bool GRP, typename g_t>
 static int launch_bt2(const ScanBwdParams& p, const BwdMaps<GRP>& maps, int ss, cudaStream_t stream) {
     switch (ss) {
-        case 4: return launch_bt3<in_t, RB, 4, GRP>(p, maps, stream);
-        case 2: return launch_bt3<in_t, RB, 2, GRP>(p, maps, stream);
-        default: return launch_bt3<in_t, RB, 1, GRP>(p, maps, stream);
+        case 4: return launch_bt3<in_t, RB, 4, GRP, g_t>(p, maps, stream);
+        case 2: return launch_bt3<in_t, RB, 2, GRP, g_t>(p, maps, stream);
+        default: return launch_bt3<in_t, RB, 1, GRP, g_t>(p, maps, stream);
     }
 }
 
-template <typename in_t, bool GRP>
+template <typename in_t, bool GRP, typename g_t = in_t>
 static int launch_bt1(const ScanBwdParams& p, const BwdMaps<GRP>& maps, int ss, cudaStream_t stream) {
-    return launch_bt2<in_t, 2, GRP>(p, maps, ss, stream);  // rows per warp: 2 (scan_bwd_tma_pick)
+    return launch_bt2<in_t, 2, GRP, g_t>(p, maps, ss, stream);  // rows per warp: 2 (scan_bwd_tma_pick)
 }
 
 // state split at RB = 2: the 255-register kernel keeps 2 CTAs x 4 warps per SM resident (2 x SMs CTAs per wave)
@@ -516,7 +530,7 @@ bool scan_bwd_tma_pick(const ScanBwdParams& p, int dtype, int& rb, int& ss) {
     return p.rows_per_group % (rb * 4 / ss) == 0;
 }
 
-int scan_bwd_tma_launch(const ScanBwdParams& p, int dtype, int rb, int ss, cudaStream_t stream) {
+int scan_bwd_tma_launch(const ScanBwdParams& p, int dtype, int rb, int ss, cudaStream_t stream, bool dout_f32) {
     ScanBwdTmaMapsN<1> maps;
     const uint32_t chunk = 32 / rb * T, rows = rb * 4 / ss;
     const uint32_t box_io[4] = {chunk, rows, 1, 1}, box_bc[4] = {chunk, 16, 1, 1};
@@ -527,9 +541,18 @@ int scan_bwd_tma_launch(const ScanBwdParams& p, int dtype, int rb, int ss, cudaS
     int rc;
     if ((rc = make_tmap_4d(&maps.u[0], dtype, p.u, dio, su, box_io)) != VMB_OK) return rc;
     if ((rc = make_tmap_4d(&maps.d[0], dtype, p.delta, dio, sd, box_io)) != VMB_OK) return rc;
-    if ((rc = make_tmap_4d(&maps.g[0], dtype, p.dout, dio, sg, box_io)) != VMB_OK) return rc;
+    if ((rc = make_tmap_4d(&maps.g[0], dout_f32 ? VMB_F32 : dtype, p.dout, dio, sg, box_io)) != VMB_OK) return rc;
     if ((rc = make_tmap_4d(&maps.b[0], dtype, p.Bm, dbc, sb, box_bc)) != VMB_OK) return rc;
     if ((rc = make_tmap_4d(&maps.c[0], dtype, p.Cm, dbc, sc, box_bc)) != VMB_OK) return rc;
+    if (dout_f32) {  // fp32 dout against 16-bit inputs: a dout tile twice as wide (+4 / 2 / 1 KB at SS = 1 / 2 / 4), still two CTAs
+                     // per SM (static_assert in launch_bt3)
+        switch (dtype) {
+            case VMB_BF16: return launch_bt1<__nv_bfloat16, false, float>(p, maps, ss, stream);
+            case VMB_F16: return launch_bt1<__half, false, float>(p, maps, ss, stream);
+        }
+        set_error("selective_scan_bwd: fp32 dout needs bf16 / fp16 inputs (dtype %d)", dtype);
+        return VMB_ERR_INVALID;
+    }
     switch (dtype) {
         case VMB_F32: return launch_bt1<float, false>(p, maps, ss, stream);  // 130 KB of tiles: one CTA per SM
         case VMB_BF16: return launch_bt1<__nv_bfloat16, false>(p, maps, ss, stream);

@@ -18,6 +18,8 @@
 //   * checkpoints of h every CKPT positions (fp32) feed the backward kernel.
 #include <stdlib.h>
 
+#include <type_traits>
+
 #include "scan_common.cuh"
 
 namespace vmb {
@@ -118,7 +120,8 @@ __device__ __forceinline__ void stage_bc_cta(float4* __restrict__ dst, const in_
 // MODE 0: plain operator, no checkpoints (inference)   1: plain operator + checkpoints (training forward)
 //      2: direction-aware grouped sources (per-group bases, reversed walk), no checkpoints   3: 2 + checkpoints.
 // Each mode only compiles what it needs: the state loop sits at the 128-register limit.
-template <typename in_t, int RB, int WPC, int MODE>
+// out_t: element type of `out` (float with 16-bit in_t, MODE 0 / 1 only: the fp32 accumulator stored without rounding).
+template <typename in_t, int RB, int WPC, int MODE, typename out_t>
 __global__ void __launch_bounds__(32 * WPC, 12 / WPC) scan_fwd_kernel(const ScanFwdParams p) {
     pdl_trigger();
     pdl_wait();
@@ -126,6 +129,7 @@ __global__ void __launch_bounds__(32 * WPC, 12 / WPC) scan_fwd_kernel(const Scan
     using R = FwdRaw<in_t, RB>;
     constexpr int SEGW = Cfg::SEGW, CHUNK = Cfg::CHUNK, SEGQ = Cfg::SEGQ, SLOTS = Cfg::SLOTS;
     constexpr int V = Vec<in_t>::N, NT = 32 * WPC;
+    constexpr int VO = Vec<out_t>::N;
 
     extern __shared__ float4 smem_f4[];
     float4* sB = smem_f4;                                                  // [8][SLOTS]   CTA-shared
@@ -148,14 +152,14 @@ __global__ void __launch_bounds__(32 * WPC, 12 / WPC) scan_fwd_kernel(const Scan
     constexpr bool HAS_REV = MODE >= 2;
 
     const in_t *Bg, *Cg, *ublk, *dblk;
-    in_t* orow;
+    out_t* orow;
     bool rev = false;
     if (MODE < 2) {
         Bg = reinterpret_cast<const in_t*>(p.Bm) + (int64_t)b * p.B_bs + (int64_t)g * p.B_gs;
         Cg = reinterpret_cast<const in_t*>(p.Cm) + (int64_t)b * p.C_bs + (int64_t)g * p.C_gs;
         ublk = reinterpret_cast<const in_t*>(p.u) + (int64_t)b * p.u_bs + (int64_t)d0 * p.u_ds;
         dblk = reinterpret_cast<const in_t*>(p.delta) + (int64_t)b * p.dl_bs + (int64_t)d0 * p.dl_ds;
-        orow = reinterpret_cast<in_t*>(p.out) + (int64_t)b * p.o_bs + (int64_t)d * p.o_ds;
+        orow = reinterpret_cast<out_t*>(p.out) + (int64_t)b * p.o_bs + (int64_t)d * p.o_ds;
     } else {  // per-group sources; rows are indexed inside the group
         const ScanGroupDesc& gd = p.grp[g];
         const int dg0 = d0 - g * p.rows_per_group;
@@ -163,7 +167,7 @@ __global__ void __launch_bounds__(32 * WPC, 12 / WPC) scan_fwd_kernel(const Scan
         Cg = reinterpret_cast<const in_t*>(gd.Cm) + (int64_t)b * p.C_bs;
         ublk = reinterpret_cast<const in_t*>(gd.u) + (int64_t)b * p.u_bs + (int64_t)dg0 * p.u_ds;
         dblk = reinterpret_cast<const in_t*>(gd.delta) + (int64_t)b * p.dl_bs + (int64_t)dg0 * p.dl_ds;
-        orow = reinterpret_cast<in_t*>(gd.out) + (int64_t)b * p.o_bs + (int64_t)(dg0 + r) * p.o_ds;
+        orow = reinterpret_cast<out_t*>(gd.out) + (int64_t)b * p.o_bs + (int64_t)(dg0 + r) * p.o_ds;
         if constexpr (HAS_REV) rev = gd.rev != 0;
     }
     const in_t* __restrict__ urow = ublk + (int64_t)r * p.u_ds;
@@ -307,28 +311,28 @@ __global__ void __launch_bounds__(32 * WPC, 12 / WPC) scan_fwd_kernel(const Scan
         }
         if (!HAS_REV || !rev) {
 #pragma unroll
-            for (int v = 0; v < T / V; ++v) store_vec<in_t>(orow + l0 + v * V, y + v * V, valid - v * V, p.vec_ok);
+            for (int v = 0; v < T / VO; ++v) store_vec<out_t>(orow + l0 + v * VO, y + v * VO, valid - v * VO, p.vec_ok);
         } else if (valid == T) {  // sequence l0+t -> memory L-1-l0-t: one reversed contiguous block
 #pragma unroll
-            for (int v = 0; v < T / V; ++v) {
-                float yr[V];
+            for (int v = 0; v < T / VO; ++v) {
+                float yr[VO];
 #pragma unroll
-                for (int i = 0; i < V; ++i) yr[i] = y[T - 1 - (v * V + i)];
-                store_vec<in_t>(orow + (L - l0 - T) + v * V, yr, V, p.vec_ok);
+                for (int i = 0; i < VO; ++i) yr[i] = y[T - 1 - (v * VO + i)];
+                store_vec<out_t>(orow + (L - l0 - T) + v * VO, yr, VO, p.vec_ok);
             }
         } else {
 #pragma unroll
             for (int t = 0; t < T; ++t)
-                if (t < valid) orow[L - 1 - l0 - t] = from_f32<in_t>(y[t]);
+                if (t < valid) orow[L - 1 - l0 - t] = from_f32<out_t>(y[t]);
         }
     }
 }
 
-template <typename in_t, int RB, int WPC, int MODE>
+template <typename in_t, int RB, int WPC, int MODE, typename out_t>
 static int launch_cfg2(const ScanFwdParams& p, cudaStream_t stream) {
     using Cfg = FwdCfg<RB>;
     using R = FwdRaw<in_t, RB>;
-    auto kern = scan_fwd_kernel<in_t, RB, WPC, MODE>;
+    auto kern = scan_fwd_kernel<in_t, RB, WPC, MODE, out_t>;
     const size_t smem = sizeof(float4) * 16 * Cfg::SLOTS + R::bc_bytes + WPC * (R::io_bytes + sizeof(float) * 2 * RB * p.npad);
     VMB_CHECK(smem <= 227 * 1024, "selective_scan_fwd: dstate=%d needs %zu B of shared memory", p.N, smem);
     if (smem > 48 * 1024) VMB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -338,16 +342,19 @@ static int launch_cfg2(const ScanFwdParams& p, cudaStream_t stream) {
     return VMB_OK;
 }
 
-template <typename in_t, int RB, int WPC>
+template <typename in_t, int RB, int WPC, typename out_t>
 static int launch_cfg(const ScanFwdParams& p, cudaStream_t stream) {
-    if (p.ndesc) {
-        if constexpr (RB <= 2) {
-            if (p.ckpt) return launch_cfg2<in_t, RB, WPC, 3>(p, stream);
+    if constexpr (std::is_same<in_t, out_t>::value) {  // the grouped modes exist with the input's output type only
+        if (p.ndesc) {
+            if constexpr (RB <= 2) {
+                if (p.ckpt) return launch_cfg2<in_t, RB, WPC, 3, out_t>(p, stream);
+            }
+            VMB_CHECK(p.ckpt == nullptr, "grouped scan: checkpoints need RB <= 2 (pick_cfg)");
+            return launch_cfg2<in_t, RB, WPC, 2, out_t>(p, stream);
         }
-        VMB_CHECK(p.ckpt == nullptr, "grouped scan: checkpoints need RB <= 2 (pick_cfg)");
-        return launch_cfg2<in_t, RB, WPC, 2>(p, stream);
     }
-    return p.ckpt ? launch_cfg2<in_t, RB, WPC, 1>(p, stream) : launch_cfg2<in_t, RB, WPC, 0>(p, stream);
+    VMB_CHECK(p.ndesc == 0, "grouped scan: no fp32 output");
+    return p.ckpt ? launch_cfg2<in_t, RB, WPC, 1, out_t>(p, stream) : launch_cfg2<in_t, RB, WPC, 0, out_t>(p, stream);
 }
 
 // (rows per warp RB, warps per CTA WPC): RB*WPC must divide the rows of a group.  Small RB = more warps and
@@ -370,36 +377,39 @@ static void pick_cfg(const ScanFwdParams& p, int& rb, int& wpc) {
     if (env_wpc > 0 && (env_wpc & (env_wpc - 1)) == 0 && rpg % (rb * env_wpc) == 0 && env_wpc <= 4) wpc = env_wpc;
 }
 
-template <typename in_t, int RB>
+template <typename in_t, int RB, typename out_t>
 static int launch_rb(const ScanFwdParams& p, int wpc, cudaStream_t stream) {
     switch (wpc) {
-        case 4: return launch_cfg<in_t, RB, 4>(p, stream);
-        case 2: return launch_cfg<in_t, RB, 2>(p, stream);
-        default: return launch_cfg<in_t, RB, 1>(p, stream);
+        case 4: return launch_cfg<in_t, RB, 4, out_t>(p, stream);
+        case 2: return launch_cfg<in_t, RB, 2, out_t>(p, stream);
+        default: return launch_cfg<in_t, RB, 1, out_t>(p, stream);
     }
 }
 
-template <typename in_t>
+template <typename in_t, typename out_t = in_t>
 static int launch_t(const ScanFwdParams& p, cudaStream_t stream) {
     int rb, wpc;
     pick_cfg(p, rb, wpc);
     switch (rb) {
-        case 8: return launch_rb<in_t, 8>(p, wpc, stream);
-        case 4: return launch_rb<in_t, 4>(p, wpc, stream);
-        case 2: return launch_rb<in_t, 2>(p, wpc, stream);
-        default: return launch_rb<in_t, 1>(p, wpc, stream);
+        case 8: return launch_rb<in_t, 8, out_t>(p, wpc, stream);
+        case 4: return launch_rb<in_t, 4, out_t>(p, wpc, stream);
+        case 2: return launch_rb<in_t, 2, out_t>(p, wpc, stream);
+        default: return launch_rb<in_t, 1, out_t>(p, wpc, stream);
     }
 }
 
-int scan_fwd_launch(const ScanFwdParams& p, int dtype, cudaStream_t stream) {
+int scan_fwd_launch(const ScanFwdParams& p, int dtype, cudaStream_t stream, bool out_f32) {
     VMB_CHECK((long)p.batch * p.dim < (1L << 31), "selective_scan_fwd: batch*dim too large");
+    VMB_CHECK(!out_f32 || (p.ndesc == 0 && (dtype == VMB_BF16 || dtype == VMB_F16)),
+              "selective_scan_fwd: fp32 output needs bf16 / fp16 inputs and the flat operator");
     {  // fast path: TMA-staged kernel (scan_fwd_tma.cu); this file keeps the generic shapes (unaligned rows, dstate > 16, short L)
         int rb, ss;
-        if (scan_fwd_tma_pick(p, rb, ss)) return scan_fwd_tma_launch(p, dtype, rb, ss, stream);
+        if (scan_fwd_tma_pick(p, rb, ss)) return scan_fwd_tma_launch(p, dtype, rb, ss, stream, out_f32);
     }
     if (p.ndesc) {
         VMB_CHECK(p.vec_ok && p.npad == 16, "grouped scan: needs 16 B-aligned rows (L %% 8 == 0) and dstate <= 16");
     }
+    if (out_f32) return dtype == VMB_BF16 ? launch_t<__nv_bfloat16, float>(p, stream) : launch_t<__half, float>(p, stream);
     switch (dtype) {
         case VMB_F32: return launch_t<float>(p, stream);
         case VMB_BF16: return launch_t<__nv_bfloat16>(p, stream);

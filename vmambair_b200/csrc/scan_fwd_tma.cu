@@ -13,6 +13,8 @@
 //   * packed-pair softplus: max(x,0) + log1p(exp(-|x|)) in f32x2, the lg2 MUFU skipped when every exp(-|x|) of the warp is small.
 #include <stdlib.h>
 
+#include <type_traits>
+
 #include "scan_common.cuh"
 #include "tma.cuh"
 #include "scan_tma_common.cuh"
@@ -36,7 +38,9 @@ struct TmaCfg {
 
 // MODE 0: plain operator   1: plain + checkpoints (training forward)   2: per-group sources, reversed walk (fused OSS block)
 //      3: per-group sources + checkpoints (cross_selective_scan forward; indexed by sequence position, like MODE 1 on gathered copies)
-template <typename in_t, int RB, int NW, int SS, int MODE>
+// out_t: element type of `out`; float with 16-bit in_t (MODE 0 / 1 only) stores the fp32 accumulator without rounding
+// (selective_scan_cuda_oflex, out_float=True)
+template <typename in_t, int RB, int NW, int SS, int MODE, typename out_t>
 __global__ void __launch_bounds__(32 * NW, NW == 8 ? 2 : 3)
     scan_fwd_tma_kernel(const ScanFwdParams p, const __grid_constant__ ScanTmaMaps maps) {
     pdl_trigger();
@@ -45,6 +49,7 @@ __global__ void __launch_bounds__(32 * NW, NW == 8 ? 2 : 3)
     using Cfg = FwdCfg<RB>;
     constexpr int SEGW = Cfg::SEGW, CHUNK = Cfg::CHUNK, SEGQ = Cfg::SEGQ, SLOTS = Cfg::SLOTS;
     constexpr int V = Vec<in_t>::N, NT = 32 * NW, ROWS = K::ROWS, NPW = K::NPW;
+    constexpr int VO = Vec<out_t>::N;
 
     extern __shared__ unsigned char smem_dyn[];
     unsigned char* smem_raw = smem_dyn + ((128u - (smem_addr(smem_dyn) & 127u)) & 127u);  // TMA destinations: 128 B aligned
@@ -70,15 +75,15 @@ __global__ void __launch_bounds__(32 * NW, NW == 8 ? 2 : 3)
     const int d0 = dc0 + rs * RB, d = d0 + r;
     const int N = p.N, L = p.L;
 
-    in_t* orow;
+    out_t* orow;
     bool rev = false;
     int gi = 0, zbc = g, urow0 = dc0;
     if (MODE < 2) {
-        orow = reinterpret_cast<in_t*>(p.out) + (int64_t)b * p.o_bs + (int64_t)d * p.o_ds;
+        orow = reinterpret_cast<out_t*>(p.out) + (int64_t)b * p.o_bs + (int64_t)d * p.o_ds;
     } else {
         const ScanGroupDesc& gd = p.grp[g];
         urow0 = dc0 - g * p.rows_per_group;
-        orow = reinterpret_cast<in_t*>(gd.out) + (int64_t)b * p.o_bs + (int64_t)(urow0 + rs * RB + r) * p.o_ds;
+        orow = reinterpret_cast<out_t*>(gd.out) + (int64_t)b * p.o_bs + (int64_t)(urow0 + rs * RB + r) * p.o_ds;
         rev = gd.rev != 0;
         gi = g;
         zbc = 0;
@@ -298,19 +303,19 @@ __global__ void __launch_bounds__(32 * NW, NW == 8 ? 2 : 3)
         }
         if (MODE < 2 || !rev) {
 #pragma unroll
-            for (int v = 0; v < T / V; ++v) store_vec<in_t>(orow + l0 + v * V, y + v * V, valid - v * V, true);
+            for (int v = 0; v < T / VO; ++v) store_vec<out_t>(orow + l0 + v * VO, y + v * VO, valid - v * VO, true);
         } else if (valid == T) {  // sequence l0+t -> memory L-1-l0-t: one reversed contiguous block
 #pragma unroll
-            for (int v = 0; v < T / V; ++v) {
-                float yr[V];
+            for (int v = 0; v < T / VO; ++v) {
+                float yr[VO];
 #pragma unroll
-                for (int i = 0; i < V; ++i) yr[i] = y[T - 1 - (v * V + i)];
-                store_vec<in_t>(orow + (L - l0 - T) + v * V, yr, V, true);
+                for (int i = 0; i < VO; ++i) yr[i] = y[T - 1 - (v * VO + i)];
+                store_vec<out_t>(orow + (L - l0 - T) + v * VO, yr, VO, true);
             }
         } else {
 #pragma unroll
             for (int t = 0; t < T; ++t)
-                if (t < valid) orow[L - 1 - l0 - t] = from_f32<in_t>(y[t]);
+                if (t < valid) orow[L - 1 - l0 - t] = from_f32<out_t>(y[t]);
         }
     }
 }
@@ -360,10 +365,10 @@ int make_tmap_4d(CUtensorMap* map, int dtype, const void* base, const uint64_t d
     return VMB_OK;
 }
 
-template <typename in_t, int RB, int NW, int SS, int MODE>
+template <typename in_t, int RB, int NW, int SS, int MODE, typename out_t>
 static int launch_tma4(const ScanFwdParams& p, const ScanTmaMaps& maps, cudaStream_t stream) {
     using K = TmaCfg<in_t, RB, NW, SS>;
-    auto kern = scan_fwd_tma_kernel<in_t, RB, NW, SS, MODE>;
+    auto kern = scan_fwd_tma_kernel<in_t, RB, NW, SS, MODE, out_t>;
     constexpr size_t smem = K::smem_bytes + 128;  // + alignment slack
     static_assert(smem <= 227 * 1024, "scan_fwd_tma: shared memory");
     VMB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -373,28 +378,31 @@ static int launch_tma4(const ScanFwdParams& p, const ScanTmaMaps& maps, cudaStre
     return VMB_OK;
 }
 
-template <typename in_t, int RB, int NW, int SS>
+template <typename in_t, int RB, int NW, int SS, typename out_t>
 static int launch_tma3(const ScanFwdParams& p, const ScanTmaMaps& maps, cudaStream_t stream) {
-    if (p.ndesc) return p.ckpt ? launch_tma4<in_t, RB, NW, SS, 3>(p, maps, stream) : launch_tma4<in_t, RB, NW, SS, 2>(p, maps, stream);
-    return p.ckpt ? launch_tma4<in_t, RB, NW, SS, 1>(p, maps, stream) : launch_tma4<in_t, RB, NW, SS, 0>(p, maps, stream);
+    if constexpr (std::is_same<in_t, out_t>::value) {  // the grouped modes exist with the input's output type only
+        if (p.ndesc) return p.ckpt ? launch_tma4<in_t, RB, NW, SS, 3, out_t>(p, maps, stream) : launch_tma4<in_t, RB, NW, SS, 2, out_t>(p, maps, stream);
+    }
+    VMB_CHECK(p.ndesc == 0, "selective_scan_fwd_grouped: no fp32 output");
+    return p.ckpt ? launch_tma4<in_t, RB, NW, SS, 1, out_t>(p, maps, stream) : launch_tma4<in_t, RB, NW, SS, 0, out_t>(p, maps, stream);
 }
 
 // 4-warp CTAs, three resident per SM: 384 CTAs at (8, 384, 4096) spread 2-3 per SM (8-warp CTAs: 192 on 132 SMs, 1-2 per SM)
 constexpr int kTmaWarps = 4;
 
-template <typename in_t, int RB>
+template <typename in_t, int RB, typename out_t>
 static int launch_tma2(const ScanFwdParams& p, const ScanTmaMaps& maps, int ss, cudaStream_t stream) {
     switch (ss) {
-        case 4: return launch_tma3<in_t, RB, kTmaWarps, 4>(p, maps, stream);
-        case 2: return launch_tma3<in_t, RB, kTmaWarps, 2>(p, maps, stream);
-        default: return launch_tma3<in_t, RB, kTmaWarps, 1>(p, maps, stream);
+        case 4: return launch_tma3<in_t, RB, kTmaWarps, 4, out_t>(p, maps, stream);
+        case 2: return launch_tma3<in_t, RB, kTmaWarps, 2, out_t>(p, maps, stream);
+        default: return launch_tma3<in_t, RB, kTmaWarps, 1, out_t>(p, maps, stream);
     }
 }
 
-template <typename in_t>
+template <typename in_t, typename out_t = in_t>
 static int launch_tma1(const ScanFwdParams& p, const ScanTmaMaps& maps, int ss, cudaStream_t stream) {
     // rows per warp: 2 (scan_fwd_tma_pick; tools/scan_sweep.py: RB = 4 / 8 lose at every batch size, not instantiated)
-    return launch_tma2<in_t, 2>(p, maps, ss, stream);
+    return launch_tma2<in_t, 2, out_t>(p, maps, ss, stream);
 }
 
 // (rows per warp, state split) for the TMA kernel; false when the shape is left to the generic kernel.
@@ -418,7 +426,7 @@ bool scan_fwd_tma_pick(const ScanFwdParams& p, int& rb, int& ss) {
     return rpg % (rb * kTmaWarps / ss) == 0;
 }
 
-int scan_fwd_tma_launch(const ScanFwdParams& p_in, int dtype, int rb, int ss, cudaStream_t stream) {
+int scan_fwd_tma_launch(const ScanFwdParams& p_in, int dtype, int rb, int ss, cudaStream_t stream, bool out_f32) {
     ScanFwdParams p = p_in;
     {
         p.num_sms = num_sms();
@@ -446,6 +454,14 @@ int scan_fwd_tma_launch(const ScanFwdParams& p_in, int dtype, int rb, int ss, cu
         if ((rc = make_tmap_4d(&maps.d[0], dtype, p.delta, dio, sd, box_io)) != VMB_OK) return rc;
         if ((rc = make_tmap_4d(&maps.b[0], dtype, p.Bm, dbc, sb, box_bc)) != VMB_OK) return rc;
         if ((rc = make_tmap_4d(&maps.c[0], dtype, p.Cm, dbc, sc, box_bc)) != VMB_OK) return rc;
+    }
+    if (out_f32) {  // fp32 `out` from 16-bit inputs
+        switch (dtype) {
+            case VMB_BF16: return launch_tma1<__nv_bfloat16, float>(p, maps, ss, stream);
+            case VMB_F16: return launch_tma1<__half, float>(p, maps, ss, stream);
+        }
+        set_error("selective_scan_fwd: fp32 output needs bf16 / fp16 inputs (dtype %d)", dtype);
+        return VMB_ERR_INVALID;
     }
     switch (dtype) {
         case VMB_F32: return launch_tma1<float>(p, maps, ss, stream);

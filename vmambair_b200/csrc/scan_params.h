@@ -61,12 +61,14 @@ struct ScanBwdGroups {
     int64_t dB_bs, dB_ns, dC_bs, dC_ns;  // strides of every group's dB / dC (B,N,L) destination
 };
 
-int scan_fwd_launch(const ScanFwdParams& p, int dtype, cudaStream_t stream);
+// out_f32 / dout_f32 (16-bit dtype only): `out` / `dout` are fp32 (selective_scan_cuda_oflex).  They are launcher arguments, not
+// parameter-block members, so that the kernels instantiated without them keep their parameter layout.
+int scan_fwd_launch(const ScanFwdParams& p, int dtype, cudaStream_t stream, bool out_f32 = false);
 bool scan_fwd_tma_pick(const ScanFwdParams& p, int& rb, int& ss);
-int scan_fwd_tma_launch(const ScanFwdParams& p, int dtype, int rb, int ss, cudaStream_t stream);
-int scan_bwd_launch(const ScanBwdParams& p, int dtype, cudaStream_t stream);
+int scan_fwd_tma_launch(const ScanFwdParams& p, int dtype, int rb, int ss, cudaStream_t stream, bool out_f32 = false);
+int scan_bwd_launch(const ScanBwdParams& p, int dtype, cudaStream_t stream, bool dout_f32 = false);
 bool scan_bwd_tma_pick(const ScanBwdParams& p, int dtype, int& rb, int& ss);
-int scan_bwd_tma_launch(const ScanBwdParams& p, int dtype, int rb, int ss, cudaStream_t stream);
+int scan_bwd_tma_launch(const ScanBwdParams& p, int dtype, int rb, int ss, cudaStream_t stream, bool dout_f32 = false);
 int scan_bwd_grouped_launch(const ScanBwdParams& p, const ScanBwdGroups& gr, int dtype, cudaStream_t stream);
 
 }  // namespace vmb

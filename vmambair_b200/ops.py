@@ -93,13 +93,19 @@ def ckpt_interval() -> int:
     return _lib.lib().vmb_scan_ckpt_interval()
 
 
-def selective_scan_fwd(u, delta, A, B, C_, D=None, delta_bias=None, delta_softplus=False, need_ckpt=True):
-    """-> (out, ckpt).  out has delta's dtype/shape; ckpt is the opaque fp32 checkpoint tensor."""
+def selective_scan_fwd(u, delta, A, B, C_, D=None, delta_bias=None, delta_softplus=False, need_ckpt=True, out_float=False):
+    """-> (out, ckpt).  out has delta's dtype/shape; ckpt is the opaque fp32 checkpoint tensor.
+    out_float: out is fp32 whatever the input dtype -- with bf16 / fp16 inputs the fp32 accumulator is stored without rounding
+    (the reference's selective_scan_cuda_oflex, cusoflex/selective_scan_oflex.cpp:219,235-239)."""
     b, d, l, n, g = _check_common(u, delta, A, B, C_, D, delta_bias, "selective_scan_fwd")
     L = _lib.lib()
-    out = torch.empty_like(delta)
-    if out.stride(-1) != 1:
-        out = torch.empty(delta.shape, dtype=delta.dtype, device=delta.device)
+    out_f32 = bool(out_float) and u.dtype != torch.float32
+    if out_f32:
+        out = torch.empty(delta.shape, dtype=torch.float32, device=delta.device)
+    else:
+        out = torch.empty_like(delta)
+        if out.stride(-1) != 1:
+            out = torch.empty(delta.shape, dtype=delta.dtype, device=delta.device)
     ck = ckpt_interval()
     ckpt = torch.empty((b, d, (l + ck - 1) // ck, n), dtype=torch.float32, device=u.device) if need_ckpt else None
     a = _lib.ScanFwdArgs(
@@ -107,20 +113,24 @@ def selective_scan_fwd(u, delta, A, B, C_, D=None, delta_bias=None, delta_softpl
         b, d, l, n, g,
         u.stride(0), u.stride(1), delta.stride(0), delta.stride(1), out.stride(0), out.stride(1),
         B.stride(0), B.stride(1), B.stride(2), C_.stride(0), C_.stride(1), C_.stride(2),
-        int(bool(delta_softplus)), _DT[u.dtype])
+        int(bool(delta_softplus)), _DT[u.dtype], int(out_f32))
     es = u.element_size()
-    nbytes = es * (3 * b * d * l + 2 * b * g * n * l) + 4 * (d * n + 2 * d)  # SURVEY.md 8(d): every operand once
+    nbytes = es * (2 * b * d * l + 2 * b * g * n * l) + out.element_size() * b * d * l + 4 * (d * n + 2 * d)  # SURVEY.md 8(d): every operand once
     with torch.cuda.device(u.device), _timed("scan_fwd", nbytes, u.device, 1):
         _lib.check(L.vmb_selective_scan_fwd(C.byref(a), _stream(u)), "selective_scan_fwd")
     return out, ckpt
 
 
-def selective_scan_bwd(u, delta, A, B, C_, D, delta_bias, dout, ckpt, delta_softplus=False, zeroed=None):
+def selective_scan_bwd(u, delta, A, B, C_, D, delta_bias, dout, ckpt, delta_softplus=False, zeroed=None, dout_float=False):
     """-> (du, ddelta, dA, dB, dC, dD, ddelta_bias); dB/dC returned in B/C dtype (reference cpp:347).
+    dout has u's dtype (cus/selective_scan.cpp:259).  dout_float=True also accepts an fp32 dout against bf16 / fp16 u (the gradient
+    of an out_float forward; the reference's selective_scan_cuda_oflex.bwd, cusoflex/selective_scan_oflex.cpp:257-260,349-355):
+    du, ddelta, dB, dC keep u's dtype.
     zeroed: optional (dA, dD, dbias) pre-zeroed fp32 buffers (the training path hands out slices of one zeroed workspace)."""
     b, d, l, n, g = _check_common(u, delta, A, B, C_, D, delta_bias, "selective_scan_bwd")
-    if dout.dtype != u.dtype or tuple(dout.shape) != (b, d, l) or (dout.stride(-1) != 1 and dout.size(-1) != 1):
-        raise RuntimeError("selective_scan_bwd: dout must match u in dtype/shape with stride(-1)==1")
+    dout_f32 = bool(dout_float) and dout.dtype == torch.float32 and u.dtype != torch.float32
+    if (dout.dtype != u.dtype and not dout_f32) or tuple(dout.shape) != (b, d, l) or (dout.stride(-1) != 1 and dout.size(-1) != 1):
+        raise RuntimeError("selective_scan_bwd: dout must match u in dtype (or be float32) and shape, with stride(-1)==1")
     L = _lib.lib()
     du = torch.empty((b, d, l), dtype=u.dtype, device=u.device)
     ddelta = torch.empty((b, d, l), dtype=u.dtype, device=u.device)
@@ -137,9 +147,9 @@ def selective_scan_bwd(u, delta, A, B, C_, D, delta_bias, dout, ckpt, delta_soft
         u.stride(0), u.stride(1), delta.stride(0), delta.stride(1), dout.stride(0), dout.stride(1),
         du.stride(0), du.stride(1), ddelta.stride(0), ddelta.stride(1),
         B.stride(0), B.stride(1), B.stride(2), C_.stride(0), C_.stride(1), C_.stride(2),
-        int(bool(delta_softplus)), _DT[u.dtype])
+        int(bool(delta_softplus)), _DT[u.dtype], int(dout_f32))
     es = u.element_size()
-    nbytes = es * (5 * b * d * l + 4 * b * g * n * l) + 4 * b * d * ((l + 63) // 64) * n
+    nbytes = es * (4 * b * d * l + 4 * b * g * n * l) + dout.element_size() * b * d * l + 4 * b * d * ((l + 63) // 64) * n
     with torch.cuda.device(u.device), _timed("scan_bwd", nbytes, u.device, 2):
         _lib.check(L.vmb_selective_scan_bwd(C.byref(a), _stream(u)), "selective_scan_bwd")
     return du, ddelta, dA, dB, dC, dD, dbias
