@@ -98,8 +98,12 @@ int vmb_selective_scan_fwd_grouped(const vmb_scan_grouped_args* a, void* stream)
  *   ckpt  : as written by the forward (required when seqlen > interval).
  *   dout_f32 : 0 -> dout has dtype `dt`;  1 (bf16 / fp16 `dt` only) -> dout is fp32, read without rounding:
  *       selective_scan_cuda_oflex.bwd (cusoflex/selective_scan_oflex.cpp:245-358; output_type == Float at :260, :353).
- *       du, ddelta, dB, dC keep dtype `dt`; dA, dD, ddelta_bias stay fp32 (cpp:324-356).  Last member: zero keeps the
- *       plain operator. */
+ *       du, ddelta, dB, dC keep dtype `dt`; dA, dD, ddelta_bias stay fp32 (cpp:324-356).  Zero keeps the plain operator.
+ *   deterministic : 0 -> the fp32 sums over rows and batch are float atomics (run-to-run differences in the last bits), `workspace`
+ *       as above;  1 -> bitwise reproducible: every contributing CTA stores its partial sums into its own slot of `workspace`
+ *       (vmb_scan_bwd_det_workspace_bytes(a) bytes, 16 B aligned, not zero-filled: every slot read is written) and a second
+ *       kernel sums them in a fixed order, writes dB / dC and ADDS one sum to each element of dA, dD, ddelta_bias.  Other
+ *       values return VMB_ERR_INVALID.  Last member. */
 typedef struct {
     const void* u; const void* delta; const float* A; const void* Bm; const void* Cm;
     const float* D; const float* delta_bias; const void* dout; const float* ckpt;
@@ -111,9 +115,14 @@ typedef struct {
     int delta_softplus;
     int dtype;
     int dout_f32;
+    int deterministic;
 } vmb_scan_bwd_args;
 int vmb_selective_scan_bwd(const vmb_scan_bwd_args* a, void* stream);
 int64_t vmb_scan_bwd_workspace_bytes(int batch, int ngroups, int dstate, int seqlen);
+/* workspace of the deterministic mode for exactly these arguments (the launch configuration depends on the sizes, dtype, strides
+ * and alignment; `workspace` and `deterministic` are ignored): 16 nc batch ngroups ceil16(dstate)/2 seqlen + 4 batch dim (dstate + 2)
+ * bytes, nc = the CTAs that share one (batch, group).  -1 for invalid arguments (vmb_last_error()). */
+int64_t vmb_scan_bwd_det_workspace_bytes(const vmb_scan_bwd_args* a);
 
 /* Direction-aware backward, the adjoint of vmb_selective_scan_fwd_grouped: group g (<= 4) reads u, delta, Bm, Cm, dout from its own
  * tensors and writes du, ddelta (batch, rows, seqlen) and dB, dC (batch, dstate, seqlen) to its own destinations, every one in the
@@ -122,7 +131,9 @@ int64_t vmb_scan_bwd_workspace_bytes(int batch, int ngroups, int dstate, int seq
  * SelectiveScan.backward compute (RealSR/VmambaIR/archs/MambaRealSR11_arch.py:295-343) without the four gathered copies.
  *   dA (dim,dstate), dD (dim), ddelta_bias (dim): fp32, indexed by g*rows+r, ACCUMULATED into (caller zero-fills)
  *   workspace : vmb_scan_bwd_workspace_bytes(batch, ngroups, dstate, seqlen) bytes, 16 B aligned, zero-filled by the library
+ *       (deterministic = 1: vmb_scan_grouped_bwd_det_workspace_bytes(a) bytes, not zero-filled)
  *   ckpt : as written by vmb_selective_scan_fwd_grouped (required when seqlen > interval)
+ *   deterministic : 0 or 1, as for vmb_selective_scan_bwd; last member
  * Strides are shared by the groups.  Requires 16 B-aligned rows of u, delta, Bm, Cm, dout, du, ddelta (seqlen % 8 == 0 for
  * 16-bit I/O, % 4 for fp32) and dstate <= 16; dB / dC need no alignment.  Anything else returns VMB_ERR_INVALID. */
 typedef struct {
@@ -135,8 +146,10 @@ typedef struct {
     int64_t B_bs, B_ns, C_bs, C_ns, dB_bs, dB_ns, dC_bs, dC_ns;
     int delta_softplus;
     int dtype;
+    int deterministic;
 } vmb_scan_grouped_bwd_args;
 int vmb_selective_scan_bwd_grouped(const vmb_scan_grouped_bwd_args* a, void* stream);
+int64_t vmb_scan_grouped_bwd_det_workspace_bytes(const vmb_scan_grouped_bwd_args* a);  /* as vmb_scan_bwd_det_workspace_bytes */
 
 
 /* ---- B1 module boundary: fused stages of one OSS block (inference) -------------------------------
@@ -387,7 +400,10 @@ int64_t vmb_cross_selective_scan_c_workspace_bytes(int batch, int D, int R, int 
 /* weight gradient of a 1x1 conv: out[m][k] += sum_{b,p} dy[b][m][p] * x[b][k][p]  (out fp32 (M,K), accumulated: the caller zero-fills;
  * per_batch != 0: out is (B,M,K) and batches are not summed -- the channel gate in front of out_conv scales them per image).
  * dy (B,M,L), x (B,K,L): bf16 / fp16 views with 16 B aligned, pixel-contiguous rows.  mma.sync tensor-core kernel, split over
- * pixels.  (fp32 activations: use the library GEMM.) */
+ * pixels.  (fp32 activations: use the library GEMM.)
+ * deterministic = 0: the pixel splits meet in fp32 atomics (workspace unused, may be NULL);  1: bitwise reproducible -- every CTA stores
+ * its partial into its own slot of `workspace` (vmb_pixlin_wgrad_workspace_bytes(a) bytes, 16 B aligned, not zero-filled) and a
+ * second kernel adds the slots' sum, taken in a fixed order, once to each element of out and dbias.  Other values: VMB_ERR_INVALID. */
 typedef struct {
     const void* dy; const void* x; float* out;
     int batch, M, K, L;
@@ -395,8 +411,12 @@ typedef struct {
     int per_batch;
     int dtype;
     float* dbias; /* optional (M) fp32, accumulated: dbias[m] += sum_{b,p} dy[b][m][p] (the conv's bias gradient) */
+    void* workspace;
+    int deterministic;
 } vmb_wgrad_args;
 int vmb_pixlin_wgrad(const vmb_wgrad_args* a, void* stream);
+/* 4 batch splits (M K + M if dbias) bytes: the deterministic mode's partial slots for exactly these arguments; -1 for bad sizes */
+int64_t vmb_pixlin_wgrad_workspace_bytes(const vmb_wgrad_args* a);
 
 /* Per-step weight preparation of one OSS block in ONE launch: every job converts an fp32 parameter into the layout a kernel of
  * this library consumes.  type 0: (M,K) -> dst (M, ld) in `dtype`, columns >= K zero;  1: (M,K) -> dst (K, ld) = transpose, columns

@@ -37,7 +37,7 @@ class ScanBwdArgs(C.Structure):
         ("u_bs", i64), ("u_ds", i64), ("delta_bs", i64), ("delta_ds", i64), ("dout_bs", i64), ("dout_ds", i64),
         ("du_bs", i64), ("du_ds", i64), ("ddelta_bs", i64), ("ddelta_ds", i64),
         ("B_bs", i64), ("B_gs", i64), ("B_ns", i64), ("C_bs", i64), ("C_gs", i64), ("C_ns", i64),
-        ("delta_softplus", C.c_int), ("dtype", C.c_int), ("dout_f32", C.c_int),
+        ("delta_softplus", C.c_int), ("dtype", C.c_int), ("dout_f32", C.c_int), ("deterministic", C.c_int),
     ]
 
 
@@ -115,7 +115,7 @@ class ScanGroupedBwdArgs(C.Structure):
         ("u_bs", i64), ("u_ds", i64), ("delta_bs", i64), ("delta_ds", i64), ("dout_bs", i64), ("dout_ds", i64),
         ("du_bs", i64), ("du_ds", i64), ("ddelta_bs", i64), ("ddelta_ds", i64),
         ("B_bs", i64), ("B_ns", i64), ("C_bs", i64), ("C_ns", i64), ("dB_bs", i64), ("dB_ns", i64), ("dC_bs", i64), ("dC_ns", i64),
-        ("delta_softplus", C.c_int), ("dtype", C.c_int),
+        ("delta_softplus", C.c_int), ("dtype", C.c_int), ("deterministic", C.c_int),
     ]
 
 
@@ -162,7 +162,7 @@ class GateBwdArgs(C.Structure):
 class WgradArgs(C.Structure):
     _fields_ = [("dy", vp), ("x", vp), ("out", vp), ("batch", C.c_int), ("M", C.c_int), ("K", C.c_int), ("L", C.c_int),
                 ("dy_bs", i64), ("dy_cs", i64), ("x_bs", i64), ("x_cs", i64), ("per_batch", C.c_int), ("dtype", C.c_int),
-                ("dbias", vp)]
+                ("dbias", vp), ("workspace", vp), ("deterministic", C.c_int)]
 
 
 class ChannelBwdArgs(C.Structure):
@@ -206,6 +206,7 @@ SYMBOLS = {
     "vmb_selective_scan_fwd": (C.c_int, [C.POINTER(ScanFwdArgs), vp]),
     "vmb_selective_scan_bwd": (C.c_int, [C.POINTER(ScanBwdArgs), vp]),
     "vmb_scan_bwd_workspace_bytes": (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int]),
+    "vmb_scan_bwd_det_workspace_bytes": (C.c_int64, [C.POINTER(ScanBwdArgs)]),
     "vmb_pixlin": (C.c_int, [C.POINTER(PixlinArgs), vp]),
     "vmb_dwconv3x3": (C.c_int, [C.POINTER(DwconvArgs), vp]),
     "vmb_cross_scan": (C.c_int, [C.POINTER(CrossScanArgs), vp]),
@@ -219,6 +220,7 @@ SYMBOLS = {
     "vmb_dwconv3x3_t": (C.c_int, [C.POINTER(DwconvArgs), vp, vp]),
     "vmb_selective_scan_fwd_grouped": (C.c_int, [C.POINTER(ScanGroupedArgs), vp]),
     "vmb_selective_scan_bwd_grouped": (C.c_int, [C.POINTER(ScanGroupedBwdArgs), vp]),
+    "vmb_scan_grouped_bwd_det_workspace_bytes": (C.c_int64, [C.POINTER(ScanGroupedBwdArgs)]),
     "vmb_merge_sum": (C.c_int, [C.POINTER(MergeArgs), vp, vp]),
     "vmb_channel_branch": (C.c_int, [C.POINTER(ChannelArgs), vp]),
     "vmb_layernorm_fwd": (C.c_int, [C.POINTER(LnFwdArgs), vp]),
@@ -228,6 +230,7 @@ SYMBOLS = {
     "vmb_channel_gate_bwd": (C.c_int, [C.POINTER(GateBwdArgs), vp]),
     "vmb_fused_adam": (C.c_int, [C.POINTER(AdamArgs), vp]),
     "vmb_pixlin_wgrad": (C.c_int, [C.POINTER(WgradArgs), vp]),
+    "vmb_pixlin_wgrad_workspace_bytes": (C.c_int64, [C.POINTER(WgradArgs)]),
     "vmb_channel_branch_bwd": (C.c_int, [C.POINTER(ChannelBwdArgs), vp]),
     "vmb_channel_branch_bwd_smem_bytes": (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int]),
     "vmb_channel_branch_bwd_scratch_bytes": (C.c_int64, [C.c_int, C.c_int, C.c_int]),

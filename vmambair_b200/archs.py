@@ -26,6 +26,7 @@ from __future__ import annotations
 import math
 import numbers
 import os
+import warnings
 
 import torch
 import torch.nn as nn
@@ -291,6 +292,22 @@ class SS2D_1(nn.Module):
         return self.forward_compose(x)
 
 
+_FUSED_DET_WARNED = False
+_FUSED_DET_MSG = (
+    "torch.use_deterministic_algorithms(True) is on, but MamberBlock runs its fused path, which is not bitwise reproducible: "
+    "the fused training step's backward accumulates in fp32 atomics (the train_ops.cu and channel_bwd.cu kernels, the scan and "
+    "the wgrad parameter phases), and inference computes the merge statistics in two kernels with atomics.  For reproducible "
+    "training set VMB_TRAIN_PATH=compose (or archs.set_train_path('compose')): torch ops plus this library's deterministic "
+    "selective-scan backward.")
+
+
+def _warn_fused_nondeterministic():
+    global _FUSED_DET_WARNED
+    if not _FUSED_DET_WARNED and torch.are_deterministic_algorithms_enabled():
+        _FUSED_DET_WARNED = True
+        warnings.warn(_FUSED_DET_MSG, UserWarning, stacklevel=3)
+
+
 class MamberBlock(nn.Module):
     def __init__(self, dim, num_heads, ffn_expansion_factor, bias, LayerNorm_type, variant="sisr"):
         super().__init__()
@@ -310,9 +327,11 @@ class MamberBlock(nn.Module):
             from . import fused
             if not torch.is_grad_enabled():
                 if fused.available(self, x):
+                    _warn_fused_nondeterministic()
                     return fused.block_forward(self, x, out)
             elif _TRAIN_PATH == "fused" and fused.available(self, x):
                 from . import fused_train
+                _warn_fused_nondeterministic()
                 return fused_train.block_forward(self, x)  # forward + backward of every stage on this library's kernels
         y = self.forward_compose(x)
         if out is not None:

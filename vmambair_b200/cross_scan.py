@@ -219,7 +219,10 @@ def cross_selective_scan(x: torch.Tensor = None, x_proj_weight: torch.Tensor = N
     reference within bf16 / fp16 rounding of u, delta, B and C.  x_proj and dt_proj are applied as one folded matrix W_dt W_x[:R]
     (fp32 product, cast to x's dtype), so even fp32 results differ from the reference's two einsums in rounding only.
     softmax_version=True raises NotImplementedError (as SS2D_1 does); nrows is accepted and ignored (the kernels pick their own
-    rows per warp, as selective_scan_cuda_core does)."""
+    rows per warp, as selective_scan_cuda_core does).
+    Under torch.use_deterministic_algorithms(True) the scan backward and the x_proj / dt_proj weight gradients (vmb_pixlin_wgrad) run
+    the library's deterministic kernels, so the gradients are bitwise reproducible; the weight unfold's torch matmuls then need
+    CUBLAS_WORKSPACE_CONFIG=:4096:8 (or :16:8), as torch requires for cuBLAS under that flag."""
     if softmax_version:
         raise NotImplementedError("cross_selective_scan: softmax_version is not supported")
     _check_cuda(x, x_proj_weight, x_proj_bias, dt_projs_weight, dt_projs_bias, A_logs, Ds)

@@ -78,11 +78,13 @@ extern "C" int64_t vmb_scan_bwd_workspace_bytes(int batch, int ngroups, int dsta
     return 16 * (int64_t)batch * ngroups * (npad / 2) * seqlen;
 }
 
-extern "C" int vmb_selective_scan_bwd(const vmb_scan_bwd_args* a, void* stream) {
+// checks + parameter block of vmb_selective_scan_bwd, shared with the workspace query (which needs no workspace: the call requires
+// it 16 B aligned, so it never changes the launch configuration)
+static int scan_bwd_params(const vmb_scan_bwd_args* a, ScanBwdParams& p) {
     VMB_CHECK(a != nullptr, "selective_scan_bwd: null args");
     VMB_CHECK(a->dtype == VMB_F32 || a->dtype == VMB_BF16 || a->dtype == VMB_F16,
               "selective_scan_bwd: dtype must be f32/bf16/f16 (got %d)", a->dtype);
-    VMB_CHECK(a->u && a->delta && a->A && a->Bm && a->Cm && a->dout && a->du && a->ddelta && a->dA && a->dB && a->dC && a->workspace,
+    VMB_CHECK(a->u && a->delta && a->A && a->Bm && a->Cm && a->dout && a->du && a->ddelta && a->dA && a->dB && a->dC,
               "selective_scan_bwd: null tensor pointer");
     VMB_CHECK(a->batch > 0 && a->dim > 0 && a->seqlen > 0 && a->dstate > 0 && a->ngroups > 0,
               "selective_scan_bwd: non-positive size");
@@ -91,16 +93,16 @@ extern "C" int vmb_selective_scan_bwd(const vmb_scan_bwd_args* a, void* stream) 
     VMB_CHECK(a->batch <= 65535, "selective_scan_bwd: batch > 65535");
     VMB_CHECK(a->ckpt != nullptr || a->seqlen <= kScanCkpt,
               "selective_scan_bwd: forward checkpoints required when seqlen > %d", kScanCkpt);
-    VMB_CHECK(aligned16(a->workspace), "selective_scan_bwd: workspace must be 16-byte aligned");
     VMB_CHECK((a->D == nullptr) == (a->dD == nullptr), "selective_scan_bwd: D and dD must both be given or both be NULL");
     VMB_CHECK((a->delta_bias == nullptr) == (a->ddelta_bias == nullptr),
               "selective_scan_bwd: delta_bias and ddelta_bias must both be given or both be NULL");
     VMB_CHECK(a->dout_f32 == 0 || a->dout_f32 == 1, "selective_scan_bwd: dout_f32 must be 0 or 1 (got %d)", a->dout_f32);
     VMB_CHECK(!a->dout_f32 || a->dtype == VMB_BF16 || a->dtype == VMB_F16, "selective_scan_bwd: dout_f32 needs bf16 / fp16 inputs");
-    ScanBwdParams p{};
+    VMB_CHECK(a->deterministic == 0 || a->deterministic == 1, "selective_scan_bwd: deterministic must be 0 or 1 (got %d)", a->deterministic);
+    p = ScanBwdParams{};
     p.u = a->u; p.delta = a->delta; p.Bm = a->Bm; p.Cm = a->Cm; p.dout = a->dout; p.A = a->A; p.D = a->D;
     p.bias = a->delta_bias; p.ckpt = a->ckpt; p.du = a->du; p.ddelta = a->ddelta; p.dA = a->dA; p.dB = a->dB; p.dC = a->dC;
-    p.dD = a->dD; p.dbias = a->ddelta_bias; p.dBC = static_cast<float*>(a->workspace);
+    p.dD = a->dD; p.dbias = a->ddelta_bias;
     p.batch = a->batch; p.dim = a->dim; p.L = a->seqlen; p.N = a->dstate; p.G = a->ngroups;
     p.npad = (a->dstate + 15) / 16 * 16;
     p.rows_per_group = a->dim / a->ngroups;
@@ -113,11 +115,27 @@ extern "C" int vmb_selective_scan_bwd(const vmb_scan_bwd_args* a, void* stream) 
     auto mult = [v](int64_t s) { return s % v == 0; };
     auto mult_g = [vg](int64_t s) { return s % vg == 0; };
     p.vec_ok = aligned16(a->u) && aligned16(a->delta) && aligned16(a->Bm) && aligned16(a->Cm) && aligned16(a->dout) &&
-               aligned16(a->du) && aligned16(a->ddelta) && aligned16(a->workspace) && mult(a->u_bs) && mult(a->u_ds) && mult(a->delta_bs) &&
+               aligned16(a->du) && aligned16(a->ddelta) && mult(a->u_bs) && mult(a->u_ds) && mult(a->delta_bs) &&
                mult(a->delta_ds) && mult_g(a->dout_bs) && mult_g(a->dout_ds) && mult(a->du_bs) && mult(a->du_ds) &&
                mult(a->ddelta_bs) && mult(a->ddelta_ds) && mult(a->B_bs) && mult(a->B_gs) && mult(a->B_ns) &&
                mult(a->C_bs) && mult(a->C_gs) && mult(a->C_ns);
-    return scan_bwd_launch(p, a->dtype, static_cast<cudaStream_t>(stream), a->dout_f32 != 0);
+    return VMB_OK;
+}
+
+extern "C" int vmb_selective_scan_bwd(const vmb_scan_bwd_args* a, void* stream) {
+    ScanBwdParams p;
+    int rc = scan_bwd_params(a, p);
+    if (rc != VMB_OK) return rc;
+    VMB_CHECK(a->workspace != nullptr, "selective_scan_bwd: null tensor pointer");
+    VMB_CHECK(aligned16(a->workspace), "selective_scan_bwd: workspace must be 16-byte aligned");
+    p.dBC = static_cast<float*>(a->workspace);
+    return scan_bwd_launch(p, a->dtype, static_cast<cudaStream_t>(stream), a->dout_f32 != 0, a->deterministic != 0);
+}
+
+extern "C" int64_t vmb_scan_bwd_det_workspace_bytes(const vmb_scan_bwd_args* a) {
+    ScanBwdParams p;
+    if (scan_bwd_params(a, p) != VMB_OK) return -1;
+    return scan_bwd_det_workspace(p, a->dtype);
 }
 
 static inline bool dt_ok(int d) { return d == VMB_F32 || d == VMB_BF16 || d == VMB_F16; }
@@ -304,22 +322,23 @@ extern "C" int vmb_selective_scan_fwd_grouped(const vmb_scan_grouped_args* a, vo
     return scan_fwd_launch(p, a->dtype, static_cast<cudaStream_t>(stream));
 }
 
-extern "C" int vmb_selective_scan_bwd_grouped(const vmb_scan_grouped_bwd_args* a, void* stream) {
+static int scan_bwd_grouped_params(const vmb_scan_grouped_bwd_args* a, ScanBwdParams& p, ScanBwdGroups& gr) {
     VMB_CHECK(a != nullptr, "selective_scan_bwd_grouped: null args");
     VMB_CHECK(dt_ok(a->dtype), "selective_scan_bwd_grouped: dtype must be f32/bf16/f16 (got %d)", a->dtype);
     VMB_CHECK(a->ngroups >= 1 && a->ngroups <= 4 && a->dim % a->ngroups == 0, "selective_scan_bwd_grouped: 1..4 groups dividing dim");
     VMB_CHECK(a->batch > 0 && a->batch <= 65535 && a->dim > 0 && a->seqlen > 0 && a->dstate > 0 && a->dstate <= 16,
               "selective_scan_bwd_grouped: bad sizes (dstate <= 16)");
-    VMB_CHECK(a->A && a->dA && a->workspace, "selective_scan_bwd_grouped: A, dA or workspace missing");
+    VMB_CHECK(a->A && a->dA, "selective_scan_bwd_grouped: A, dA or workspace missing");
     VMB_CHECK(a->ckpt != nullptr || a->seqlen <= kScanCkpt,
               "selective_scan_bwd_grouped: forward checkpoints required when seqlen > %d", kScanCkpt);
-    VMB_CHECK(aligned16(a->workspace), "selective_scan_bwd_grouped: workspace must be 16-byte aligned");
     VMB_CHECK((a->D == nullptr) == (a->dD == nullptr), "selective_scan_bwd_grouped: D and dD must both be given or both be NULL");
     VMB_CHECK((a->delta_bias == nullptr) == (a->ddelta_bias == nullptr),
               "selective_scan_bwd_grouped: delta_bias and ddelta_bias must both be given or both be NULL");
-    ScanBwdParams p{};
+    VMB_CHECK(a->deterministic == 0 || a->deterministic == 1, "selective_scan_bwd_grouped: deterministic must be 0 or 1 (got %d)",
+              a->deterministic);
+    p = ScanBwdParams{};
     p.A = a->A; p.D = a->D; p.bias = a->delta_bias; p.ckpt = a->ckpt;
-    p.dA = a->dA; p.dD = a->dD; p.dbias = a->ddelta_bias; p.dBC = static_cast<float*>(a->workspace);
+    p.dA = a->dA; p.dD = a->dD; p.dbias = a->ddelta_bias;
     p.batch = a->batch; p.dim = a->dim; p.L = a->seqlen; p.N = a->dstate; p.G = a->ngroups;
     p.npad = 16;
     p.rows_per_group = a->dim / a->ngroups;
@@ -333,7 +352,7 @@ extern "C" int vmb_selective_scan_bwd_grouped(const vmb_scan_grouped_bwd_args* a
     bool ok = mult(a->u_bs) && mult(a->u_ds) && mult(a->delta_bs) && mult(a->delta_ds) && mult(a->dout_bs) && mult(a->dout_ds) &&
               mult(a->du_bs) && mult(a->du_ds) && mult(a->ddelta_bs) && mult(a->ddelta_ds) && mult(a->B_bs) && mult(a->B_ns) &&
               mult(a->C_bs) && mult(a->C_ns) && a->seqlen % v == 0;
-    ScanBwdGroups gr{};
+    gr = ScanBwdGroups{};
     gr.ndesc = a->ngroups;
     gr.dB_bs = a->dB_bs; gr.dB_ns = a->dB_ns; gr.dC_bs = a->dC_bs; gr.dC_ns = a->dC_ns;
     for (int g = 0; g < a->ngroups; ++g) {
@@ -346,5 +365,25 @@ extern "C" int vmb_selective_scan_bwd_grouped(const vmb_scan_grouped_bwd_args* a
     VMB_CHECK(ok, "selective_scan_bwd_grouped: needs 16 B-aligned rows (base pointers, batch / row strides, seqlen %% %d == 0)", v);
     p.vec_ok = true;
     VMB_CHECK((long)p.batch * p.dim < (1L << 31), "selective_scan_bwd_grouped: batch*dim too large");
-    return scan_bwd_grouped_launch(p, gr, a->dtype, static_cast<cudaStream_t>(stream));
+    return VMB_OK;
+}
+
+extern "C" int vmb_selective_scan_bwd_grouped(const vmb_scan_grouped_bwd_args* a, void* stream) {
+    ScanBwdParams p;
+    ScanBwdGroups gr;
+    int rc = scan_bwd_grouped_params(a, p, gr);
+    if (rc != VMB_OK) return rc;
+    VMB_CHECK(a->workspace, "selective_scan_bwd_grouped: A, dA or workspace missing");
+    VMB_CHECK(aligned16(a->workspace), "selective_scan_bwd_grouped: workspace must be 16-byte aligned");
+    p.dBC = static_cast<float*>(a->workspace);
+    return scan_bwd_grouped_launch(p, gr, a->dtype, static_cast<cudaStream_t>(stream), a->deterministic != 0);
+}
+
+extern "C" int64_t vmb_scan_grouped_bwd_det_workspace_bytes(const vmb_scan_grouped_bwd_args* a) {
+    ScanBwdParams p;
+    ScanBwdGroups gr;
+    if (scan_bwd_grouped_params(a, p, gr) != VMB_OK) return -1;
+    const int64_t n = scan_bwd_grouped_det_workspace(p);
+    if (n < 0) set_error("selective_scan_bwd_grouped: rows per group (%d) must be even", p.rows_per_group);
+    return n;
 }

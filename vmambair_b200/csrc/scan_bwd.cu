@@ -41,7 +41,9 @@ __device__ __forceinline__ void red_add_f32x4(float4* addr, float4 v) {
 
 // g_t: element type of dout.  float with 16-bit in_t (selective_scan_cuda_oflex's fp32 dout): dout is read straight from global
 // memory (16 B vectors when aligned) and only u / delta are staged (NIO = 2); every output keeps its type.
-template <typename in_t, int RB, typename g_t>
+// DET (deterministic mode, scan_params.h): plain stores into the warp's own partial slots instead of float atomics; the contributor
+// of a (batch, group) is the warp's index inside the group.
+template <typename in_t, int RB, typename g_t, bool DET = false>
 __global__ void __launch_bounds__(32, 8) scan_bwd_kernel(const ScanBwdParams p) {
     pdl_wait();
     constexpr bool G_IN = std::is_same<g_t, in_t>::value;
@@ -82,7 +84,9 @@ __global__ void __launch_bounds__(32, 8) scan_bwd_kernel(const ScanBwdParams p) 
     const in_t* __restrict__ gorow = io_base[2] + (int64_t)r * p.do_ds;
     in_t* __restrict__ durow = reinterpret_cast<in_t*>(p.du) + (int64_t)b * p.du_bs + (int64_t)d * p.du_ds;
     in_t* __restrict__ ddrow = reinterpret_cast<in_t*>(p.ddelta) + (int64_t)b * p.dd_bs + (int64_t)d * p.dd_ds;
-    float4* __restrict__ scratch = reinterpret_cast<float4*>(p.dBC) + ((int64_t)b * p.G + g) * (npad / 2) * (int64_t)L;
+    int64_t slot = (int64_t)b * p.G + g;
+    if constexpr (DET) slot += (int64_t)((d0 % p.rows_per_group) / RB) * p.batch * p.G;
+    float4* __restrict__ scratch = reinterpret_cast<float4*>(p.dBC) + slot * (npad / 2) * (int64_t)L;
     const float* __restrict__ ckrow = p.ckpt + ((int64_t)b * p.dim + d0) * p.n_ckpt * N;  // + (rr*n_ckpt + k)*N + n
 
     const int nchunks = (L + CHUNK - 1) / CHUNK;
@@ -289,7 +293,11 @@ __global__ void __launch_bounds__(32, 8) scan_bwd_kernel(const ScanBwdParams p) 
                         acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
                     }
                     const int l = c0 + cell;
-                    if (l < L && n0 < N && !p.debug_nored) red_add_f32x4(scratch + (int64_t)(n0 / 2) * L + l, acc);
+                    if constexpr (DET) {
+                        if (l < L && n0 < N) scratch[(int64_t)(n0 / 2) * L + l] = acc;
+                    } else {
+                        if (l < L && n0 < N && !p.debug_nored) red_add_f32x4(scratch + (int64_t)(n0 / 2) * L + l, acc);
+                    }
                 }
                 __syncwarp();
             }
@@ -319,13 +327,22 @@ __global__ void __launch_bounds__(32, 8) scan_bwd_kernel(const ScanBwdParams p) 
         dbias_acc += __shfl_xor_sync(0xffffffffu, dbias_acc, o);
     }
     if (sl == 0) {
-        if (p.dD) atomicAdd(p.dD + d, dD_acc);
-        if (p.dbias) atomicAdd(p.dbias + d, dbias_acc);
+        if constexpr (DET) {
+            if (p.dD) p.dD[(int64_t)b * p.dim + d] = dD_acc;
+            if (p.dbias) p.dbias[(int64_t)b * p.dim + d] = dbias_acc;
+        } else {
+            if (p.dD) atomicAdd(p.dD + d, dD_acc);
+            if (p.dbias) atomicAdd(p.dbias + d, dbias_acc);
+        }
     }
     __syncwarp();
     for (int i = lane; i < RB * npad; i += 32) {
         const int rr = i / npad, n = i % npad;
-        if (n < N) atomicAdd(p.dA + (int64_t)(d0 + rr) * N + n, sdA[i]);
+        if constexpr (DET) {
+            if (n < N) p.dA[((int64_t)b * p.dim + d0 + rr) * N + n] = sdA[i];
+        } else {
+            if (n < N) atomicAdd(p.dA + (int64_t)(d0 + rr) * N + n, sdA[i]);
+        }
     }
 }
 
@@ -351,14 +368,101 @@ __global__ void scan_bwd_finalize_kernel(const float4* __restrict__ scratch, in_
     }
 }
 
-template <typename in_t, int RB, typename g_t>
+// deterministic mode: the sums over contributors (in index order), then over the batch (in index order) -- dB / dC are written in the
+// I/O dtype, dA / dD / ddelta_bias receive ONE addition each.  Threads [0, n_bc) own a (b, g, n/2, l) cell, the rest a (row, n) of
+// the parameter gradients (n = N: dD, n = N+1: ddelta_bias).
+template <typename in_t, bool GRP>
+__global__ void scan_bwd_det_finalize_kernel(const ScanBwdDetFin f, const ScanBwdGroups gr, long n_bc, long n_prm) {
+    pdl_wait();
+    const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n_bc) {
+        const int L = f.L, N = f.N;
+        const int l = (int)(i % L);
+        const long t = i / L;
+        const int np = (int)(t % (f.npad / 2));
+        const long bg = t / (f.npad / 2);
+        const int n0 = 2 * np;
+        if (n0 >= N) return;  // padding states: never written
+        float4 v = f.bc[i];
+        for (int c = 1; c < f.nc; ++c) {
+            const float4 w = f.bc[(long)c * n_bc + i];
+            v.x += w.x; v.y += w.y; v.z += w.z; v.w += w.w;
+        }
+        in_t *dB, *dC;
+        int64_t sB, sC;
+        if constexpr (GRP) {
+            const int g = (int)(bg % gr.ndesc);
+            const int64_t b = bg / gr.ndesc;
+            const ScanBwdGroupDesc& gd = gr.grp[g];
+            const int m = gd.rev ? L - 1 - l : l;
+            dB = reinterpret_cast<in_t*>(gd.dB) + b * gr.dB_bs + m + n0 * gr.dB_ns;
+            dC = reinterpret_cast<in_t*>(gd.dC) + b * gr.dC_bs + m + n0 * gr.dC_ns;
+            sB = gr.dB_ns;
+            sC = gr.dC_ns;
+        } else {
+            dB = reinterpret_cast<in_t*>(f.dB) + (bg * N + n0) * L + l;
+            dC = reinterpret_cast<in_t*>(f.dC) + (bg * N + n0) * L + l;
+            sB = sC = L;
+        }
+        dB[0] = from_f32<in_t>(v.x);
+        dC[0] = from_f32<in_t>(v.z);
+        if (n0 + 1 < N) {
+            dB[sB] = from_f32<in_t>(v.y);
+            dC[sC] = from_f32<in_t>(v.w);
+        }
+        return;
+    }
+    const long j = i - n_bc;
+    if (j >= n_prm) return;
+    const int N2 = f.N + 2;
+    const long d = j / N2;
+    const int n = (int)(j % N2);
+    const float* src;
+    float* dst;
+    long stride, off;
+    if (n < f.N) {
+        src = f.pA; dst = f.dA + d * f.N + n; stride = (long)f.dim * f.N; off = d * f.N + n;
+    } else {
+        src = n == f.N ? f.pD : f.pbias;
+        dst = n == f.N ? f.dD + d : f.dbias + d;
+        stride = f.dim;
+        off = d;
+        if (!src) return;
+    }
+    float s = 0.f;
+    for (int b = 0; b < f.batch; ++b) s += src[b * stride + off];
+    *dst += s;
+}
+
+template <typename in_t>
+static int det_finalize_t(const ScanBwdDetFin& f, const ScanBwdGroups* gr, cudaStream_t stream) {
+    const long n_bc = (long)f.batch * f.G * (f.npad / 2) * f.L, n_prm = (long)f.dim * (f.N + 2);
+    const unsigned blocks = (unsigned)((n_bc + n_prm + 255) / 256);
+    if (gr) VMB_CUDA(launch_pdl(scan_bwd_det_finalize_kernel<in_t, true>, dim3(blocks), dim3(256), 0, stream, f, *gr, n_bc, n_prm));
+    else VMB_CUDA(launch_pdl(scan_bwd_det_finalize_kernel<in_t, false>, dim3(blocks), dim3(256), 0, stream, f, ScanBwdGroups{}, n_bc, n_prm));
+    VMB_CUDA(cudaGetLastError());
+    return VMB_OK;
+}
+
+int scan_bwd_det_finalize(const ScanBwdDetFin& f, const ScanBwdGroups* gr, int dtype, cudaStream_t stream) {
+    switch (dtype) {
+        case VMB_F32: return det_finalize_t<float>(f, gr, stream);
+        case VMB_BF16: return det_finalize_t<__nv_bfloat16>(f, gr, stream);
+        case VMB_F16: return det_finalize_t<__half>(f, gr, stream);
+    }
+    set_error("selective_scan_bwd: unsupported dtype %d", dtype);
+    return VMB_ERR_INVALID;
+}
+
+template <typename in_t, int RB, typename g_t, bool DET = false>
 static int launch_cfg(const ScanBwdParams& p, cudaStream_t stream) {
-    auto kern = scan_bwd_kernel<in_t, RB, g_t>;
+    auto kern = scan_bwd_kernel<in_t, RB, g_t, DET>;
     const size_t smem = BwdSmem<in_t, RB, std::is_same<g_t, in_t>::value ? 3 : 2>::bytes(p.npad);
     VMB_CHECK(smem <= 227 * 1024, "selective_scan_bwd: dstate=%d needs %zu B of shared memory", p.N, smem);
     if (smem > 48 * 1024) VMB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const long blocks = (long)p.batch * (p.dim / RB);
-    kern<<<(unsigned)blocks, 32, smem, stream>>>(p);
+    if constexpr (DET) VMB_CUDA(launch_pdl(kern, dim3((unsigned)blocks), dim3(32), smem, stream, p));
+    else kern<<<(unsigned)blocks, 32, smem, stream>>>(p);
     VMB_CUDA(cudaGetLastError());
     return VMB_OK;
 }
@@ -409,20 +513,53 @@ static int launch_t(const ScanBwdParams& p_in, cudaStream_t stream) {
     return VMB_OK;
 }
 
-int scan_bwd_launch(const ScanBwdParams& p, int dtype, cudaStream_t stream, bool dout_f32) {
+// deterministic mode: contributors of one (batch, group) -- the CTAs (TMA path) or warps (generic path) that share it
+static int det_contributors(const ScanBwdParams& p, int dtype, int& trb, int& tss, int& rb) {
+    if (scan_bwd_tma_pick(p, dtype, trb, tss)) return p.rows_per_group / (trb * 4 / tss);
+    trb = 0;
+    rb = pick_rb_bwd(p);
+    return p.rows_per_group / rb;
+}
+
+int64_t scan_bwd_det_workspace(const ScanBwdParams& p, int dtype) {
+    int trb, tss, rb;
+    return scan_bwd_det_bytes(p, det_contributors(p, dtype, trb, tss, rb));
+}
+
+template <typename in_t, typename g_t = in_t>
+static int launch_det_t(const ScanBwdParams& p_in, cudaStream_t stream) {
+    constexpr bool dout_f32 = !std::is_same<g_t, in_t>::value;
+    ScanBwdParams p = p_in;
+    int trb, tss, rb = 1;
+    const ScanBwdDetFin f = scan_bwd_det_carve(p, det_contributors(p, DtOf<in_t>::v, trb, tss, rb));
+    int rc;
+    if (trb) {
+        rc = scan_bwd_tma_launch(p, DtOf<in_t>::v, trb, tss, stream, dout_f32, true);
+    } else
+    switch (rb) {
+        case 8: rc = launch_cfg<in_t, 8, g_t, true>(p, stream); break;
+        case 4: rc = launch_cfg<in_t, 4, g_t, true>(p, stream); break;
+        case 2: rc = launch_cfg<in_t, 2, g_t, true>(p, stream); break;
+        default: rc = launch_cfg<in_t, 1, g_t, true>(p, stream); break;
+    }
+    if (rc != VMB_OK) return rc;
+    return det_finalize_t<in_t>(f, nullptr, stream);
+}
+
+int scan_bwd_launch(const ScanBwdParams& p, int dtype, cudaStream_t stream, bool dout_f32, bool det) {
     VMB_CHECK((long)p.batch * p.dim < (1L << 31), "selective_scan_bwd: batch*dim too large");
     if (dout_f32) {  // fp32 dout against 16-bit inputs
         switch (dtype) {
-            case VMB_BF16: return launch_t<__nv_bfloat16, float>(p, stream);
-            case VMB_F16: return launch_t<__half, float>(p, stream);
+            case VMB_BF16: return det ? launch_det_t<__nv_bfloat16, float>(p, stream) : launch_t<__nv_bfloat16, float>(p, stream);
+            case VMB_F16: return det ? launch_det_t<__half, float>(p, stream) : launch_t<__half, float>(p, stream);
         }
         set_error("selective_scan_bwd: fp32 dout needs bf16 / fp16 inputs (dtype %d)", dtype);
         return VMB_ERR_INVALID;
     }
     switch (dtype) {
-        case VMB_F32: return launch_t<float>(p, stream);
-        case VMB_BF16: return launch_t<__nv_bfloat16>(p, stream);
-        case VMB_F16: return launch_t<__half>(p, stream);
+        case VMB_F32: return det ? launch_det_t<float>(p, stream) : launch_t<float>(p, stream);
+        case VMB_BF16: return det ? launch_det_t<__nv_bfloat16>(p, stream) : launch_t<__nv_bfloat16>(p, stream);
+        case VMB_F16: return det ? launch_det_t<__half>(p, stream) : launch_t<__half>(p, stream);
     }
     set_error("selective_scan_bwd: unsupported dtype %d", dtype);
     return VMB_ERR_INVALID;

@@ -58,6 +58,12 @@ struct BwdTmaCfg {
 __device__ __forceinline__ void red_add_f32x4_g(float4* addr, float4 v) {
     asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
 }
+// DET: a plain store into this CTA's own partial slot (summed in a fixed order by scan_bwd_det_finalize_kernel)
+template <bool DET>
+__device__ __forceinline__ void put_bc(float4* addr, float4 v) {
+    if constexpr (DET) *addr = v;
+    else red_add_f32x4_g(addr, v);
+}
 
 
 // named barrier BASE + idx (idx < 4) with an immediate id, so that ptxas counts the barriers really used
@@ -74,7 +80,10 @@ __device__ __forceinline__ void named_bar_sync(int idx, int count) {
 // GRP: per-group sources and destinations (vmb_selective_scan_bwd_grouped); a reversed group loads mirrored boxes (m0 = L - c0 - CHUNK,
 // underflow zero-filled as in the forward), reads them back to front and stores du / ddelta at memory index L-1-l.
 // g_t = float with 16-bit in_t (flat operator only): fp32 dout, converted on read; every output keeps its type.
-template <typename in_t, int RB, int SS, bool GRP, typename g_t>
+// DET (deterministic mode): no float atomics.  The launcher points p.dBC / p.dA / p.dD / p.dbias at partial slots of the workspace;
+// the CTA stores its dB/dC row sums into slot [contributor][b][g][n/2][l] (contributor = the CTA's index inside its group) and its
+// dA / dD / ddelta_bias into [b][row](..), each slot written by exactly one CTA.
+template <typename in_t, int RB, int SS, bool GRP, typename g_t, bool DET = false>
 __global__ void __launch_bounds__(128, sizeof(in_t) == 4 ? 1 : 2)
     scan_bwd_tma_kernel(const ScanBwdParams p, const __grid_constant__ BwdMaps<GRP> maps) {
     pdl_wait();
@@ -130,6 +139,7 @@ __global__ void __launch_bounds__(128, sizeof(in_t) == 4 ? 1 : 2)
     in_t* __restrict__ durow = reinterpret_cast<in_t*>(const_cast<void*>(du_base)) + (int64_t)b * p.du_bs + (int64_t)dg * p.du_ds;
     in_t* __restrict__ ddrow = reinterpret_cast<in_t*>(const_cast<void*>(dd_base)) + (int64_t)b * p.dd_bs + (int64_t)dg * p.dd_ds;
     float4* __restrict__ scratch = reinterpret_cast<float4*>(p.dBC) + ((int64_t)b * p.G + g) * 8 * (int64_t)L;
+    if constexpr (DET) scratch += (int64_t)((dc0 % p.rows_per_group) / ROWS) * p.batch * p.G * 8 * L;  // this CTA's own slot
     const float* __restrict__ ckrow = p.ckpt + ((int64_t)b * p.dim + d0) * p.n_ckpt * N;
 
     const int nchunks = (L + CHUNK - 1) / CHUNK;
@@ -383,7 +393,7 @@ __global__ void __launch_bounds__(128, sizeof(in_t) == 4 ? 1 : 2)
                     }
                     acc = make_float4(acc_b.x, acc_b.y, acc_c.x, acc_c.y);
                     const int l = c0 + cell;
-                    if (l < L && n0 < N && !p.debug_nored) red_add_f32x4_g(scratch + (int64_t)np * L + l, acc);
+                    if (l < L && n0 < N && (DET || !p.debug_nored)) put_bc<DET>(scratch + (int64_t)np * L + l, acc);
                 }
             } else {
                 // dB/dC: sum the RB rows of each (segment, position) cell, one vector reduction per cell
@@ -397,7 +407,7 @@ __global__ void __launch_bounds__(128, sizeof(in_t) == 4 ? 1 : 2)
                         acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
                     }
                     const int l = c0 + cell;
-                    if (l < L && n0 < N && !p.debug_nored) red_add_f32x4_g(scratch + (int64_t)np * L + l, acc);
+                    if (l < L && n0 < N && (DET || !p.debug_nored)) put_bc<DET>(scratch + (int64_t)np * L + l, acc);
                 }
                 __syncwarp();
             }
@@ -468,21 +478,30 @@ __global__ void __launch_bounds__(128, sizeof(in_t) == 4 ? 1 : 2)
         dbias_acc += __shfl_xor_sync(0xffffffffu, dbias_acc, o);
     }
     if (sl == 0 && sp == 0) {
-        if (p.dD) atomicAdd(p.dD + d, dD_acc);
-        if (p.dbias) atomicAdd(p.dbias + d, dbias_acc);
+        if constexpr (DET) {
+            if (p.dD) p.dD[(int64_t)b * p.dim + d] = dD_acc;
+            if (p.dbias) p.dbias[(int64_t)b * p.dim + d] = dbias_acc;
+        } else {
+            if (p.dD) atomicAdd(p.dD + d, dD_acc);
+            if (p.dbias) atomicAdd(p.dbias + d, dbias_acc);
+        }
     }
     __syncwarp();
     for (int i = lane; i < RB * 2 * NPW; i += 32) {
         const int rr = i / (2 * NPW), n = sp * 2 * NPW + i % (2 * NPW);
-        if (n < N) atomicAdd(p.dA + (int64_t)(d0 + rr) * N + n, sdA[rr * 16 + n]);
+        if constexpr (DET) {
+            if (n < N) p.dA[((int64_t)b * p.dim + d0 + rr) * N + n] = sdA[rr * 16 + n];
+        } else {
+            if (n < N) atomicAdd(p.dA + (int64_t)(d0 + rr) * N + n, sdA[rr * 16 + n]);
+        }
     }
 }
 
 // ---------------------------------------------------------------------------------------------------- host
-template <typename in_t, int RB, int SS, bool GRP, typename g_t>
+template <typename in_t, int RB, int SS, bool GRP, typename g_t, bool DET>
 static int launch_bt3(const ScanBwdParams& p, const BwdMaps<GRP>& maps, cudaStream_t stream) {
     using K = BwdTmaCfg<in_t, RB, SS, g_t>;
-    auto kern = scan_bwd_tma_kernel<in_t, RB, SS, GRP, g_t>;
+    auto kern = scan_bwd_tma_kernel<in_t, RB, SS, GRP, g_t, DET>;
     constexpr size_t smem = K::smem_bytes + 128;
     static_assert(sizeof(in_t) == 4 ? smem <= 227 * 1024 : smem <= 113 * 1024, "scan_bwd_tma: two CTAs per SM (one for fp32 I/O)");
     VMB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -492,18 +511,19 @@ static int launch_bt3(const ScanBwdParams& p, const BwdMaps<GRP>& maps, cudaStre
     return VMB_OK;
 }
 
-template <typename in_t, int RB, bool GRP, typename g_t>
+template <typename in_t, int RB, bool GRP, typename g_t, bool DET>
 static int launch_bt2(const ScanBwdParams& p, const BwdMaps<GRP>& maps, int ss, cudaStream_t stream) {
     switch (ss) {
-        case 4: return launch_bt3<in_t, RB, 4, GRP, g_t>(p, maps, stream);
-        case 2: return launch_bt3<in_t, RB, 2, GRP, g_t>(p, maps, stream);
-        default: return launch_bt3<in_t, RB, 1, GRP, g_t>(p, maps, stream);
+        case 4: return launch_bt3<in_t, RB, 4, GRP, g_t, DET>(p, maps, stream);
+        case 2: return launch_bt3<in_t, RB, 2, GRP, g_t, DET>(p, maps, stream);
+        default: return launch_bt3<in_t, RB, 1, GRP, g_t, DET>(p, maps, stream);
     }
 }
 
 template <typename in_t, bool GRP, typename g_t = in_t>
-static int launch_bt1(const ScanBwdParams& p, const BwdMaps<GRP>& maps, int ss, cudaStream_t stream) {
-    return launch_bt2<in_t, 2, GRP, g_t>(p, maps, ss, stream);  // rows per warp: 2 (scan_bwd_tma_pick)
+static int launch_bt1(const ScanBwdParams& p, const BwdMaps<GRP>& maps, int ss, cudaStream_t stream, bool det = false) {
+    // rows per warp: 2 (scan_bwd_tma_pick)
+    return det ? launch_bt2<in_t, 2, GRP, g_t, true>(p, maps, ss, stream) : launch_bt2<in_t, 2, GRP, g_t, false>(p, maps, ss, stream);
 }
 
 // state split at RB = 2: the 255-register kernel keeps 2 CTAs x 4 warps per SM resident (2 x SMs CTAs per wave)
@@ -530,7 +550,7 @@ bool scan_bwd_tma_pick(const ScanBwdParams& p, int dtype, int& rb, int& ss) {
     return p.rows_per_group % (rb * 4 / ss) == 0;
 }
 
-int scan_bwd_tma_launch(const ScanBwdParams& p, int dtype, int rb, int ss, cudaStream_t stream, bool dout_f32) {
+int scan_bwd_tma_launch(const ScanBwdParams& p, int dtype, int rb, int ss, cudaStream_t stream, bool dout_f32, bool det) {
     ScanBwdTmaMapsN<1> maps;
     const uint32_t chunk = 32 / rb * T, rows = rb * 4 / ss;
     const uint32_t box_io[4] = {chunk, rows, 1, 1}, box_bc[4] = {chunk, 16, 1, 1};
@@ -547,16 +567,16 @@ int scan_bwd_tma_launch(const ScanBwdParams& p, int dtype, int rb, int ss, cudaS
     if (dout_f32) {  // fp32 dout against 16-bit inputs: a dout tile twice as wide (+4 / 2 / 1 KB at SS = 1 / 2 / 4), still two CTAs
                      // per SM (static_assert in launch_bt3)
         switch (dtype) {
-            case VMB_BF16: return launch_bt1<__nv_bfloat16, false, float>(p, maps, ss, stream);
-            case VMB_F16: return launch_bt1<__half, false, float>(p, maps, ss, stream);
+            case VMB_BF16: return launch_bt1<__nv_bfloat16, false, float>(p, maps, ss, stream, det);
+            case VMB_F16: return launch_bt1<__half, false, float>(p, maps, ss, stream, det);
         }
         set_error("selective_scan_bwd: fp32 dout needs bf16 / fp16 inputs (dtype %d)", dtype);
         return VMB_ERR_INVALID;
     }
     switch (dtype) {
-        case VMB_F32: return launch_bt1<float, false>(p, maps, ss, stream);  // 130 KB of tiles: one CTA per SM
-        case VMB_BF16: return launch_bt1<__nv_bfloat16, false>(p, maps, ss, stream);
-        case VMB_F16: return launch_bt1<__half, false>(p, maps, ss, stream);
+        case VMB_F32: return launch_bt1<float, false>(p, maps, ss, stream, det);  // 130 KB of tiles: one CTA per SM
+        case VMB_BF16: return launch_bt1<__nv_bfloat16, false>(p, maps, ss, stream, det);
+        case VMB_F16: return launch_bt1<__half, false>(p, maps, ss, stream, det);
     }
     set_error("selective_scan_bwd: unsupported dtype %d", dtype);
     return VMB_ERR_INVALID;
@@ -590,6 +610,15 @@ __global__ void scan_bwd_finalize_grouped_kernel(const float4* __restrict__ scra
 }
 
 template <typename in_t>
+static int launch_grouped_det_t(const ScanBwdParams& p, const ScanBwdTmaMapsG& maps, int ss, int dtype, cudaStream_t stream) {
+    ScanBwdParams q = p;
+    const ScanBwdDetFin f = scan_bwd_det_carve(q, p.rows_per_group / (2 * 4 / ss));
+    int rc = launch_bt1<in_t, true>(q, maps, ss, stream, true);
+    if (rc != VMB_OK) return rc;
+    return scan_bwd_det_finalize(f, &maps.gr, dtype, stream);
+}
+
+template <typename in_t>
 static int launch_grouped_t(const ScanBwdParams& p, const ScanBwdTmaMapsG& maps, int ss, cudaStream_t stream) {
     int rc = launch_bt1<in_t, true>(p, maps, ss, stream);
     if (rc != VMB_OK) return rc;
@@ -602,11 +631,22 @@ static int launch_grouped_t(const ScanBwdParams& p, const ScanBwdTmaMapsG& maps,
 
 // the grouped mode always runs the TMA kernel (any seqlen: tails and the reversed walk's underflow are zero-filled boxes); the state
 // split grows until the CTA's rows divide the group
-int scan_bwd_grouped_launch(const ScanBwdParams& p, const ScanBwdGroups& gr, int dtype, cudaStream_t stream) {
+static int grouped_ss(const ScanBwdParams& p) {
+    int ss = bwd_tma_ss(p, 2);
+    while (ss < 4 && p.rows_per_group % (2 * 4 / ss)) ss <<= 1;
+    return ss;
+}
+
+int64_t scan_bwd_grouped_det_workspace(const ScanBwdParams& p) {
+    const int ss = grouped_ss(p);
+    if (p.rows_per_group % (2 * 4 / ss)) return -1;
+    return scan_bwd_det_bytes(p, p.rows_per_group / (2 * 4 / ss));
+}
+
+int scan_bwd_grouped_launch(const ScanBwdParams& p, const ScanBwdGroups& gr, int dtype, cudaStream_t stream, bool det) {
     VMB_CHECK(gr.ndesc == p.G && p.G >= 1 && p.G <= 4 && p.vec_ok && p.npad == 16, "selective_scan_bwd_grouped: needs 16 B-aligned rows and dstate <= 16");
     const int rb = 2;
-    int ss = bwd_tma_ss(p, rb);
-    while (ss < 4 && p.rows_per_group % (rb * 4 / ss)) ss <<= 1;
+    const int ss = grouped_ss(p);
     VMB_CHECK(p.rows_per_group % (rb * 4 / ss) == 0, "selective_scan_bwd_grouped: rows per group (%d) must be even", p.rows_per_group);
     ScanBwdTmaMapsG maps;
     maps.gr = gr;
@@ -624,6 +664,15 @@ int scan_bwd_grouped_launch(const ScanBwdParams& p, const ScanBwdGroups& gr, int
         if ((rc = make_tmap_4d(&maps.g[g], dtype, gd.dout, dio, sg, box_io)) != VMB_OK) return rc;
         if ((rc = make_tmap_4d(&maps.b[g], dtype, gd.Bm, dbc, sb, box_bc)) != VMB_OK) return rc;
         if ((rc = make_tmap_4d(&maps.c[g], dtype, gd.Cm, dbc, sc, box_bc)) != VMB_OK) return rc;
+    }
+    if (det) {  // no memset: every partial slot is written
+        switch (dtype) {
+            case VMB_F32: return launch_grouped_det_t<float>(p, maps, ss, dtype, stream);
+            case VMB_BF16: return launch_grouped_det_t<__nv_bfloat16>(p, maps, ss, dtype, stream);
+            case VMB_F16: return launch_grouped_det_t<__half>(p, maps, ss, dtype, stream);
+        }
+        set_error("selective_scan_bwd_grouped: unsupported dtype %d", dtype);
+        return VMB_ERR_INVALID;
     }
     VMB_CUDA(cudaMemsetAsync(p.dBC, 0, sizeof(float4) * (size_t)p.batch * p.G * (p.npad / 2) * p.L, stream));
     switch (dtype) {

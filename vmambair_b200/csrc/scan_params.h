@@ -61,14 +61,51 @@ struct ScanBwdGroups {
     int64_t dB_bs, dB_ns, dC_bs, dC_ns;  // strides of every group's dB / dC (B,N,L) destination
 };
 
+// Deterministic backward (det = true below): the workspace holds per-contributor partials instead of one atomically accumulated
+// scratch, and scan_bwd_det_finalize sums them in a fixed order.  Layout, in fp32:
+//   [nc][batch][G][npad/2][L][4]  dB/dC row sums of each contributor (nc = the CTAs / warps that share a (batch, group))
+//   [batch][dim][N]  dA,  [batch][dim]  dD,  [batch][dim]  ddelta_bias  (one slot per (batch, row): written by one CTA)
+// Every slot the finalize reads is written by the backward kernel, so nothing is zero-filled.
+struct ScanBwdDetFin {
+    const float4* bc;                 // dB/dC partials
+    const float *pA, *pD, *pbias;     // parameter partials
+    float *dA, *dD, *dbias;           // destinations: the sums over the batch are ADDED (accumulate-into contract)
+    void *dB, *dC;                    // flat operator: (batch, G, N, L) contiguous
+    int batch, dim, N, npad, G, L, nc;
+};
+inline int64_t scan_bwd_det_bytes(const ScanBwdParams& p, int nc) {
+    return 16 * (int64_t)nc * p.batch * p.G * (p.npad / 2) * p.L + 4 * (int64_t)p.batch * p.dim * (p.N + 2);
+}
+// points p's accumulators at the partial slots of the workspace p.dBC; returns the finalize's view (the real destinations)
+inline ScanBwdDetFin scan_bwd_det_carve(ScanBwdParams& p, int nc) {
+    ScanBwdDetFin f{};
+    float* ws = p.dBC;
+    float* prm = ws + 4 * (int64_t)nc * p.batch * p.G * (p.npad / 2) * p.L;
+    const int64_t rows = (int64_t)p.batch * p.dim;
+    f.bc = reinterpret_cast<const float4*>(ws);
+    f.pA = prm;
+    f.pD = p.dD ? prm + rows * p.N : nullptr;
+    f.pbias = p.dbias ? prm + rows * (p.N + 1) : nullptr;
+    f.dA = p.dA; f.dD = p.dD; f.dbias = p.dbias; f.dB = p.dB; f.dC = p.dC;
+    f.batch = p.batch; f.dim = p.dim; f.N = p.N; f.npad = p.npad; f.G = p.G; f.L = p.L; f.nc = nc;
+    p.dA = prm;
+    p.dD = const_cast<float*>(f.pD);
+    p.dbias = const_cast<float*>(f.pbias);
+    return f;
+}
+// gr: NULL for the flat operator, else the grouped destinations (each group's dB / dC in its memory order)
+int scan_bwd_det_finalize(const ScanBwdDetFin& f, const ScanBwdGroups* gr, int dtype, cudaStream_t stream);
+int64_t scan_bwd_det_workspace(const ScanBwdParams& p, int dtype);
+int64_t scan_bwd_grouped_det_workspace(const ScanBwdParams& p);
+
 // out_f32 / dout_f32 (16-bit dtype only): `out` / `dout` are fp32 (selective_scan_cuda_oflex).  They are launcher arguments, not
 // parameter-block members, so that the kernels instantiated without them keep their parameter layout.
 int scan_fwd_launch(const ScanFwdParams& p, int dtype, cudaStream_t stream, bool out_f32 = false);
 bool scan_fwd_tma_pick(const ScanFwdParams& p, int& rb, int& ss);
 int scan_fwd_tma_launch(const ScanFwdParams& p, int dtype, int rb, int ss, cudaStream_t stream, bool out_f32 = false);
-int scan_bwd_launch(const ScanBwdParams& p, int dtype, cudaStream_t stream, bool dout_f32 = false);
+int scan_bwd_launch(const ScanBwdParams& p, int dtype, cudaStream_t stream, bool dout_f32 = false, bool det = false);
 bool scan_bwd_tma_pick(const ScanBwdParams& p, int dtype, int& rb, int& ss);
-int scan_bwd_tma_launch(const ScanBwdParams& p, int dtype, int rb, int ss, cudaStream_t stream, bool dout_f32 = false);
-int scan_bwd_grouped_launch(const ScanBwdParams& p, const ScanBwdGroups& gr, int dtype, cudaStream_t stream);
+int scan_bwd_tma_launch(const ScanBwdParams& p, int dtype, int rb, int ss, cudaStream_t stream, bool dout_f32 = false, bool det = false);
+int scan_bwd_grouped_launch(const ScanBwdParams& p, const ScanBwdGroups& gr, int dtype, cudaStream_t stream, bool det = false);
 
 }  // namespace vmb

@@ -210,7 +210,7 @@ class _Front(torch.autograd.Function):
             (g_dD, k_dD), (g_dbias, k_dbias) = _acc(Ds, Z["dD"]), _acc(dt_b, Z["dbias"])
             du, ddelta, dA, dB, dC, dD, dbias = ops.selective_scan_bwd(
                 xs.view(B, 4 * C, L), dts.view(B, 4 * C, L), A, bc[:, :, :N], bc[:, :, N:], _f32(Ds), _f32(dt_b.reshape(-1)),
-                dys.view(B, 4 * C, L), ckpt, True, zeroed=(Z["dA"], g_dD, g_dbias))
+                dys.view(B, 4 * C, L), ckpt, True, zeroed=(Z["dA"], g_dD, g_dbias), deterministic=False)
             # back to pixel order: pi_k^-1 is pi_k with H and W swapped
             ddbl = torch.empty((B, 4, C + 2 * N, L), dtype=dt_, device=dev)
             dxc4 = ops.cross_scan_multi([([du.view(B, 4, C, L)[:, k] for k in range(4)], C, None),
@@ -223,7 +223,7 @@ class _Front(torch.autograd.Function):
             gx, gd = getattr(x_proj_w, "grad", None), getattr(dt_w, "grad", None)
             k_big = _DIRECT_GRADS and gx is not None and gd is not None and gx.dtype == gd.dtype == torch.float32 and not torch.is_grad_enabled()
             with _side(k_big, dev, ddbl, xc, Z["dbig"], bit=1):
-                dbig = ops.pixlin_wgrad(ddbl, xc, out=Z["dbig"]).view(4, C + 2 * N, C)
+                dbig = ops.pixlin_wgrad(ddbl, xc, out=Z["dbig"], deterministic=False).view(4, C + 2 * N, C)
                 d_xproj = torch.cat([torch.bmm(dtw.transpose(1, 2), dbig[:, :C]), dbig[:, C:]], 1)  # [W_dt^T dW ; dW[C:]]
                 d_dtw = torch.bmm(dbig[:, :C], xw[:, :R].transpose(1, 2))                            # dW W_x[:R]^T
                 if k_big:
@@ -242,7 +242,7 @@ class _Front(torch.autograd.Function):
             (g_win, k_win), (g_bin, k_bin) = _acc(w_in, Z["dwin"]), _acc(b_in, Z["dbin"])
             with _side(k_win and (b_in is None or k_bin), dev, x3, dxz, bit=2):
                 xn = ops.layernorm_fwd(x3, ln_mode, _f32(n1w), _f32(n1b))
-                d_win = ops.pixlin_wgrad(dxz, xn, out=g_win, dbias=g_bin).view_as(w_in)
+                d_win = ops.pixlin_wgrad(dxz, xn, out=g_win, dbias=g_bin, deterministic=False).view_as(w_in)
             (g_n1w, k_n1w), (g_n1b, k_n1b) = _acc(n1w, Z["n1w"]), _acc(n1b, Z["n1b"])
             dx, st1 = ops.layernorm_bwd(x3, dxn, ln_mode, _f32(n1w), phase="data")
             with _side(k_n1w and (n1b is None or k_n1b), dev, x3, dxn, st1, bit=128):
@@ -291,7 +291,7 @@ class _Tail(torch.autograd.Function):
             dgg = ops.pixlin(dout3, WpoutT)
             (g_wpout, k_wpout), (g_bpout, k_bpout) = _acc(w_pout, Z["wpout"]), _acc(b_pout, Z["bpout"])
             with _side(k_wpout and (b_pout is None or k_bpout), dev, dout3, gg, bit=4):
-                d_wpout = ops.pixlin_wgrad(dout3, gg, out=g_wpout, dbias=g_bpout if b_pout is not None else None).view_as(w_pout)
+                d_wpout = ops.pixlin_wgrad(dout3, gg, out=g_wpout, dbias=g_bpout if b_pout is not None else None, deterministic=False).view_as(w_pout)
             # depthwise conv + GELU gate
             (g_fdw, k_fdw), (g_fdwb, k_fdwb) = _acc(fdw, Z["fdw"]), _acc(fdwb, Z["fdwb"])
             dv = ops.dwconv3x3_bwd(t, _f32(fdw.view(2 * h, 9)), _f32(fdwb), dgg, h, H, W, 1, phase="data")
@@ -304,7 +304,7 @@ class _Tail(torch.autograd.Function):
             (g_wpin, k_wpin), (g_bpin, k_bpin) = _acc(w_pin, Z["wpin"]), _acc(b_pin, Z["bpin"])
             with _side(k_wpin and (b_pin is None or k_bpin), dev, x1, dt, bit=8):
                 x1n = ops.layernorm_fwd(x1, ln_mode, _f32(n2w), _f32(n2b))
-                d_wpin = ops.pixlin_wgrad(dt, x1n, out=g_wpin, dbias=g_bpin if b_pin is not None else None).view_as(w_pin)
+                d_wpin = ops.pixlin_wgrad(dt, x1n, out=g_wpin, dbias=g_bpin if b_pin is not None else None, deterministic=False).view_as(w_pin)
             (g_n2w, k_n2w), (g_n2b, k_n2b) = _acc(n2w, Z["n2w"]), _acc(n2b, Z["n2b"])
             dx1, st2 = ops.layernorm_bwd(x1, dx1n, ln_mode, _f32(n2w), add=dout3, phase="data")
             with _side(k_n2w and (n2b is None or k_n2b), dev, x1, dx1n, st2, bit=128):
@@ -316,7 +316,7 @@ class _Tail(torch.autograd.Function):
             g_wout = getattr(w_out, "grad", None)
             k_wout = _DIRECT_GRADS and g_wout is not None and g_wout.dtype == torch.float32 and not torch.is_grad_enabled()
             with _side(k_wout and (b_out is None or k_bout), dev, dx1, y23, cg, Z["wb"], bit=16):
-                wb = ops.pixlin_wgrad(dx1, y23, per_batch=True, out=Z["wb"], dbias=g_bout)  # (B, C_out, C_in): scaled per image by the gate
+                wb = ops.pixlin_wgrad(dx1, y23, per_batch=True, out=Z["wb"], dbias=g_bout, deterministic=False)  # (B, C_out, C_in): scaled per image by the gate
                 if gate_mode == 1:
                     d_wout = (wb * (1.0 + cg)[:, None, :]).sum(0)
                 else:  # y + c: the gate adds c[b,k] * sum_p dx1[b,m,p]  (per-image row sums: B*C values)

@@ -89,6 +89,22 @@ def _check_common(u, delta, A, B, C_, D, delta_bias, who):
     return b, d, l, n, g
 
 
+def _deterministic(flag) -> bool:
+    """None: follow torch.use_deterministic_algorithms(); True / False: override it."""
+    return torch.are_deterministic_algorithms_enabled() if flag is None else bool(flag)
+
+
+def _workspace(nbytes, given, dev, who):
+    """uint8 device buffer of at least nbytes: the caller's (16 B aligned, contiguous), else a fresh one.  Its contents never matter."""
+    if nbytes < 0:
+        raise RuntimeError(f"{who}: {_lib.lib().vmb_last_error().decode()}")
+    if given is None:
+        return torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+    if not given.is_cuda or not given.is_contiguous() or given.numel() * given.element_size() < nbytes or given.data_ptr() % 16:
+        raise RuntimeError(f"{who}: workspace must be a contiguous, 16 B aligned CUDA tensor of at least {nbytes} bytes")
+    return given
+
+
 def ckpt_interval() -> int:
     return _lib.lib().vmb_scan_ckpt_interval()
 
@@ -121,13 +137,19 @@ def selective_scan_fwd(u, delta, A, B, C_, D=None, delta_bias=None, delta_softpl
     return out, ckpt
 
 
-def selective_scan_bwd(u, delta, A, B, C_, D, delta_bias, dout, ckpt, delta_softplus=False, zeroed=None, dout_float=False):
+def selective_scan_bwd(u, delta, A, B, C_, D, delta_bias, dout, ckpt, delta_softplus=False, zeroed=None, dout_float=False,
+                       deterministic=None, workspace=None):
     """-> (du, ddelta, dA, dB, dC, dD, ddelta_bias); dB/dC returned in B/C dtype (reference cpp:347).
     dout has u's dtype (cus/selective_scan.cpp:259).  dout_float=True also accepts an fp32 dout against bf16 / fp16 u (the gradient
     of an out_float forward; the reference's selective_scan_cuda_oflex.bwd, cusoflex/selective_scan_oflex.cpp:257-260,349-355):
     du, ddelta, dB, dC keep u's dtype.
-    zeroed: optional (dA, dD, dbias) pre-zeroed fp32 buffers (the training path hands out slices of one zeroed workspace)."""
+    zeroed: optional (dA, dD, dbias) pre-zeroed fp32 buffers (the training path hands out slices of one zeroed workspace).
+    deterministic: None follows torch.are_deterministic_algorithms_enabled().  True runs the bitwise-reproducible kernels: every CTA
+    stores its partial sums in its own workspace slot and a second kernel sums them in a fixed order, then ADDS one sum to each
+    element of dA / dD / dbias (timing tag "scan_bwd_det").  False: fp32 atomics (tag "scan_bwd").
+    workspace: optional uint8 CUDA tensor used as the library's scratch (its contents are irrelevant); else one is allocated."""
     b, d, l, n, g = _check_common(u, delta, A, B, C_, D, delta_bias, "selective_scan_bwd")
+    det = _deterministic(deterministic)
     dout_f32 = bool(dout_float) and dout.dtype == torch.float32 and u.dtype != torch.float32
     if (dout.dtype != u.dtype and not dout_f32) or tuple(dout.shape) != (b, d, l) or (dout.stride(-1) != 1 and dout.size(-1) != 1):
         raise RuntimeError("selective_scan_bwd: dout must match u in dtype (or be float32) and shape, with stride(-1)==1")
@@ -137,20 +159,23 @@ def selective_scan_bwd(u, delta, A, B, C_, D, delta_bias, dout, ckpt, delta_soft
     dA = torch.zeros_like(A) if zeroed is None else zeroed[0]
     dB = torch.empty((b, g, n, l), dtype=u.dtype, device=u.device)
     dC = torch.empty((b, g, n, l), dtype=u.dtype, device=u.device)
-    ws = torch.empty(L.vmb_scan_bwd_workspace_bytes(b, g, n, l), dtype=torch.uint8, device=u.device)
     dD = (torch.zeros_like(D) if zeroed is None else zeroed[1]) if D is not None else None
     dbias = (torch.zeros_like(delta_bias) if zeroed is None else zeroed[2]) if delta_bias is not None else None
     a = _lib.ScanBwdArgs(
         _ptr(u), _ptr(delta), _ptr(A), _ptr(B), _ptr(C_), _ptr(D), _ptr(delta_bias), _ptr(dout), _ptr(ckpt),
-        _ptr(du), _ptr(ddelta), _ptr(dA), _ptr(dB), _ptr(dC), _ptr(dD), _ptr(dbias), _ptr(ws),
+        _ptr(du), _ptr(ddelta), _ptr(dA), _ptr(dB), _ptr(dC), _ptr(dD), _ptr(dbias), None,
         b, d, l, n, g,
         u.stride(0), u.stride(1), delta.stride(0), delta.stride(1), dout.stride(0), dout.stride(1),
         du.stride(0), du.stride(1), ddelta.stride(0), ddelta.stride(1),
         B.stride(0), B.stride(1), B.stride(2), C_.stride(0), C_.stride(1), C_.stride(2),
-        int(bool(delta_softplus)), _DT[u.dtype], int(dout_f32))
+        int(bool(delta_softplus)), _DT[u.dtype], int(dout_f32), int(det))
+    with torch.cuda.device(u.device):
+        nws = L.vmb_scan_bwd_det_workspace_bytes(C.byref(a)) if det else L.vmb_scan_bwd_workspace_bytes(b, g, n, l)
+    ws = _workspace(nws, workspace, u.device, "selective_scan_bwd")
+    a.workspace = ws.data_ptr()
     es = u.element_size()
     nbytes = es * (4 * b * d * l + 4 * b * g * n * l) + dout.element_size() * b * d * l + 4 * b * d * ((l + 63) // 64) * n
-    with torch.cuda.device(u.device), _timed("scan_bwd", nbytes, u.device, 2):
+    with torch.cuda.device(u.device), _timed("scan_bwd_det" if det else "scan_bwd", nbytes, u.device, 2):
         _lib.check(L.vmb_selective_scan_bwd(C.byref(a), _stream(u)), "selective_scan_bwd")
     return du, ddelta, dA, dB, dC, dD, dbias
 
@@ -356,12 +381,15 @@ def selective_scan_fwd_grouped(us, deltas, Bs, Cs, revs, A, D, delta_bias, delta
     return (out, ckpt) if need_ckpt else out
 
 
-def selective_scan_bwd_grouped(us, deltas, Bs, Cs, douts, revs, A, D, delta_bias, ckpt, delta_softplus=True, zeroed=None, out=None):
+def selective_scan_bwd_grouped(us, deltas, Bs, Cs, douts, revs, A, D, delta_bias, ckpt, delta_softplus=True, zeroed=None, out=None,
+                               deterministic=None, workspace=None):
     """Backward of selective_scan_fwd_grouped (checkpoints from its need_ckpt=True call): douts[g] (B,R,L) is the gradient of group
     g's output in that group's memory order.  -> (dus, ddeltas, dA, dBs, dCs, dD, ddelta_bias): dus / ddeltas lists of (B,R,L), dBs / dCs
     lists of (B,N,L), every one in the memory order of group g's sources; dA (G*R,N), dD, ddelta_bias (G*R) fp32.
     zeroed: optional (dA, dD, dbias) pre-zeroed fp32 accumulators.  out: optional (dus, ddeltas, dBs, dCs) destination views (each list
-    sharing strides, rows contiguous), e.g. slices of the buffers the next kernels read."""
+    sharing strides, rows contiguous), e.g. slices of the buffers the next kernels read.
+    deterministic / workspace: as in selective_scan_bwd."""
+    det = _deterministic(deterministic)
     G = len(us)
     b, R, L = us[0].shape
     N = A.shape[1]
@@ -383,21 +411,24 @@ def selective_scan_bwd_grouped(us, deltas, Bs, Cs, douts, revs, A, D, delta_bias
     dA = torch.zeros_like(A) if zeroed is None else zeroed[0]
     dD = (torch.zeros_like(D) if zeroed is None else zeroed[1]) if D is not None else None
     dbias = (torch.zeros_like(delta_bias) if zeroed is None else zeroed[2]) if delta_bias is not None else None
-    ws = torch.empty(Lb.vmb_scan_bwd_workspace_bytes(b, G, N, L), dtype=torch.uint8, device=dev)
     arr = lambda lst: (C.c_void_p * 4)(*([t.data_ptr() for t in lst] + [0] * (4 - G)))
     a = _lib.ScanGroupedBwdArgs(
         arr(us), arr(deltas), arr(Bs), arr(Cs), arr(douts), arr(dus), arr(dds), arr(dBs), arr(dCs),
         (C.c_int * 4)(*(list(map(int, revs)) + [0] * (4 - G))),
-        _ptr(A), _ptr(D), _ptr(delta_bias), _ptr(ckpt), _ptr(dA), _ptr(dD), _ptr(dbias), _ptr(ws),
+        _ptr(A), _ptr(D), _ptr(delta_bias), _ptr(ckpt), _ptr(dA), _ptr(dD), _ptr(dbias), None,
         b, G * R, L, N, G,
         us[0].stride(0), us[0].stride(1), deltas[0].stride(0), deltas[0].stride(1), douts[0].stride(0), douts[0].stride(1),
         dus[0].stride(0), dus[0].stride(1), dds[0].stride(0), dds[0].stride(1),
         Bs[0].stride(0), Bs[0].stride(1), Cs[0].stride(0), Cs[0].stride(1),
-        dBs[0].stride(0), dBs[0].stride(1), dCs[0].stride(0), dCs[0].stride(1), int(bool(delta_softplus)), _DT[dt])
+        dBs[0].stride(0), dBs[0].stride(1), dCs[0].stride(0), dCs[0].stride(1), int(bool(delta_softplus)), _DT[dt], int(det))
+    with torch.cuda.device(dev):
+        nws = Lb.vmb_scan_grouped_bwd_det_workspace_bytes(C.byref(a)) if det else Lb.vmb_scan_bwd_workspace_bytes(b, G, N, L)
+    ws = _workspace(nws, workspace, dev, "selective_scan_bwd_grouped")
+    a.workspace = ws.data_ptr()
     es = us[0].element_size()
     uniq = lambda lst: len({t.data_ptr() for t in lst})  # directions that share a source tensor read it once
     nbytes = es * b * L * (R * (uniq(us) + G + uniq(douts) + 2 * G) + 4 * G * N) + (4 * ckpt.numel() if ckpt is not None else 0)
-    with torch.cuda.device(dev), _timed("scan_bwd", nbytes, dev, 2):
+    with torch.cuda.device(dev), _timed("scan_bwd_det" if det else "scan_bwd", nbytes, dev, 2):
         _lib.check(Lb.vmb_selective_scan_bwd_grouped(C.byref(a), _stream(us[0])), "selective_scan_bwd_grouped")
     return dus, dds, dA, dBs, dCs, dD, dbias
 
@@ -612,11 +643,14 @@ def channel_gate_bwd(dyg, y2, gate, mode):
     return dy2, dg
 
 
-def pixlin_wgrad(dy, x, per_batch=False, out=None, dbias=None):
+def pixlin_wgrad(dy, x, per_batch=False, out=None, dbias=None, deterministic=None, workspace=None):
     """dW[m,k] = sum_{b,p} dy[b,m,p] x[b,k,p] -> fp32 (M,K)  (or (B,M,K) without the batch sum).  16-bit activations with 16 B aligned
     rows run this library's mma.sync split-pixel kernel; fp32 (parity mode) or unaligned rows go to the library GEMM.
     out: optional fp32 accumulator (the result is ADDED: pre-zero it for a plain result); dbias: optional (M) fp32 accumulator receiving
-    sum_{b,p} dy (the bias gradient)."""
+    sum_{b,p} dy (the bias gradient).
+    deterministic: None follows torch.are_deterministic_algorithms_enabled().  True: every CTA stores its partial in its own workspace
+    slot and a second kernel adds their fixed-order sum once to out / dbias (bitwise reproducible; timing tag "wgrad_det").  False:
+    fp32 atomics (tag "wgrad").  The fp32 / unaligned fallback is a torch GEMM either way.  workspace: as in selective_scan_bwd."""
     B, M, L = dy.shape
     K = x.shape[1]
     ok = (dy.dtype in (torch.bfloat16, torch.float16) and x.dtype == dy.dtype and dy.stride(2) == 1 and x.stride(2) == 1
@@ -633,9 +667,16 @@ def pixlin_wgrad(dy, x, per_batch=False, out=None, dbias=None):
         return res
     if out is None:
         out = torch.zeros((B, M, K) if per_batch else (M, K), dtype=torch.float32, device=dy.device)
+    det = _deterministic(deterministic)
     a = _lib.WgradArgs(_ptr(dy), _ptr(x), _ptr(out), B, M, K, L, dy.stride(0), dy.stride(1), x.stride(0), x.stride(1),
-                       int(per_batch), _DT[dy.dtype], _ptr(dbias))
-    _run("vmb_pixlin_wgrad", a, dy, "wgrad")
+                       int(per_batch), _DT[dy.dtype], _ptr(dbias), None, int(det))
+    if not det:
+        _run("vmb_pixlin_wgrad", a, dy, "wgrad")
+        return out
+    with torch.cuda.device(dy.device):
+        ws = _workspace(_lib.lib().vmb_pixlin_wgrad_workspace_bytes(C.byref(a)), workspace, dy.device, "pixlin_wgrad")
+    a.workspace = ws.data_ptr()
+    _run("vmb_pixlin_wgrad", a, dy, "wgrad_det", kernels=2)
     return out
 
 

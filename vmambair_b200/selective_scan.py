@@ -65,7 +65,9 @@ class SelectiveScanFn(torch.autograd.Function):
 def selective_scan_fn(u, delta, A, B, C, D=None, delta_bias=None, delta_softplus=False, nrows=1):
     """out = selective_scan(u, delta, A, B, C, D, delta_bias, delta_softplus) with autograd.
     Mixed input dtypes (autocast regions) are promoted to fp32, like the RealSR reference's
-    custom_fwd(cast_inputs=torch.float32) (RealSR/VmambaIR/archs/MambaRealSR11_arch.py:269-270)."""
+    custom_fwd(cast_inputs=torch.float32) (RealSR/VmambaIR/archs/MambaRealSR11_arch.py:269-270).
+    Under torch.use_deterministic_algorithms(True) the backward runs the library's deterministic kernels (fixed-order sums of
+    per-CTA partials instead of fp32 atomics), so its gradients are bitwise reproducible."""
     if not (u.dtype == delta.dtype == B.dtype == C.dtype):
         u, delta, B, C = u.float(), delta.float(), B.float(), C.float()
     if A.dtype != torch.float32:

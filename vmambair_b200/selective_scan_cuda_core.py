@@ -9,6 +9,8 @@ with the same arity / return order, so the UNMODIFIED reference archs run on the
 
 `x` is opaque to the callers (they only hand it back to bwd): here it is the fp32 checkpoint tensor
 (batch, dim, ceil(L/64), dstate).  `nrows` is accepted and ignored, as in the reference (cpp:235,345).
+Under torch.use_deterministic_algorithms(True) the backward runs the library's deterministic kernels (fixed-order sums
+of per-CTA partials instead of fp32 atomics): gradients are bitwise reproducible.
 """
 from . import ops
 

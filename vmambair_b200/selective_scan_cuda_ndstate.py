@@ -11,6 +11,8 @@ layout: A is (dim,), B and C are (batch, ngroups, seqlen).  Exposes
 It runs the dstate = 1 case of the flat operator through views (A -> (dim, 1), B / C -> (batch, ngroups, 1, seqlen)): no copies
 and no kernel of its own.  Gradients come back in the ndstate shapes: dA (dim,), dB / dC (batch, ngroups, seqlen).  `out` has the
 input dtype (cpp:207).  `x` is opaque (the fp32 checkpoint tensor (batch, dim, ceil(L/64), 1)); `nrows` is ignored.
+Under torch.use_deterministic_algorithms(True) the backward runs the library's deterministic kernels (fixed-order sums
+of per-CTA partials instead of fp32 atomics): gradients are bitwise reproducible.
 """
 from . import ops
 

@@ -12,6 +12,8 @@ bwd accepts that fp32 `dout` against 16-bit inputs (cpp:257-260,349-355); du, dd
 dA, dD, ddelta_bias in fp32, as in the reference (cpp:324-356).  With fp32 inputs out_float changes nothing.
 `x` is opaque to the callers (they only hand it back to bwd): here it is the fp32 checkpoint tensor
 (batch, dim, ceil(L/64), dstate), as in selective_scan_cuda_core.  `nrows` is accepted and ignored.
+Under torch.use_deterministic_algorithms(True) the backward runs the library's deterministic kernels (fixed-order sums
+of per-CTA partials instead of fp32 atomics): gradients are bitwise reproducible.
 """
 from . import ops
 
