@@ -13,7 +13,7 @@ Reference classes mirrored (file:line in the reference project):
                                                          mamber32_arch.py:554-649, mamber33_arch.py
   Upsampler / default_conv (SR tail)                     SRGAN/VmambaIR/archs/common.py:7-8,45-60
 
-Two execution paths share the parameters:
+Three execution paths share the parameters, for MamberBlock and for a standalone SS2D_1 alike:
   * `fused`  (CUDA, no-grad calls): the hand-written kernels (vmambair_b200.fused) -- if the CUDA library is missing a
     RuntimeError is raised; shapes outside the kernels' limits (fused.unsupported_reason) take `compose` with a warning;
   * `fused_train` (CUDA, grad enabled; default): the fused stages with their hand-written backward kernels
@@ -289,6 +289,18 @@ class SS2D_1(nn.Module):
                                      self.channel_norm, self.softmax_version, nrows=nrows, delta_softplus=True)
 
     def forward(self, x: torch.Tensor, **kwargs):
+        """on CUDA, as MamberBlock.forward: no-grad calls run fused.ss2d_forward, grad-enabled calls fused_train.ss2d_forward unless
+        the training path is "compose"; configurations outside the kernels' limits (fused.unsupported_reason) take forward_compose with
+        a one-time warning.  Under torch.use_deterministic_algorithms(True) forward_compose runs, which is bitwise reproducible there."""
+        if x.is_cuda and not torch.are_deterministic_algorithms_enabled() and (not torch.is_grad_enabled() or _TRAIN_PATH == "fused"):
+            from . import fused
+            if torch.is_autocast_enabled("cuda"):
+                x = x.to(torch.get_autocast_dtype("cuda"))  # the dtype forward_compose's in_conv would compute in
+            if fused.available(self, x):
+                if not torch.is_grad_enabled():
+                    return fused.ss2d_forward(self, x)
+                from . import fused_train
+                return fused_train.ss2d_forward(self, x)
         return self.forward_compose(x)
 
 

@@ -14,6 +14,8 @@ Structure (three autograd Functions):
     _Channel: pooled sums -> channel-direction OSS -> c         (vmb_channel_branch / vmb_channel_branch_bwd, one CTA per image;
              levels whose (2 dc, 16, C) state history exceeds one CTA's shared memory (C = 384) keep torch autograd)
     _Tail:   (y2, c, x) -> channel gate + out_conv + residual -> norm2 + project_in -> dwconv + GELU gate -> project_out + residual
+A standalone SS2D_1 (ss2d_forward) runs _Front without norm1, _Channel, and _OutConv (channel gate + out_conv, no residual; its backward
+is _Tail's out_conv section, _out_conv_bwd); prepare_block then prepares the attn weights only.
 
 Backward kernels: vmb_pixlin with the transposed weight (data gradients of the five 1x1 convs), vmb_pixlin_wgrad (their weight and bias
 gradients: mma.sync, split over pixels), vmb_selective_scan_bwd, vmb_cross_scan (the gathers pi_k and their inverses = pi_k with H
@@ -123,37 +125,48 @@ class _Arena:
         return {name: buf[o:o + k].view(*shape) for name, o, shape, k in self.specs}
 
 
-def prepare_block(block, dtype, device):
-    """kernel-layout weights of one OSS block for this step, ONE launch (vmb_prep_block_weights)"""
-    a, f = block.attn, block.ffn
-    C, R, N = a.d_inner, a.dt_rank, a.d_state
-    h = f.project_out.weight.shape[1]
+def prepare_block(mod, dtype, device):
+    """kernel-layout weights of one OSS block (or of a standalone SS2D_1: the attn weights only) for this step, ONE launch
+    (vmb_prep_block_weights).  D = d_model, C = d_inner (the scanned width E)."""
+    a = getattr(mod, "attn", mod)
+    f = getattr(mod, "ffn", None)
+    D, C, R, N = a.d_model, a.d_inner, a.dt_rank, a.d_state
     Mb = 4 * (C + 2 * N)
     w = _Arena(dtype, device)
-    for name, rows, cols in (("Win", 2 * C, C), ("WinT", C, 2 * C), ("Wbig", Mb, C), ("WbigT", C, Mb), ("Wout", C, C), ("WoutT", C, C),
-                             ("Wpin", 2 * h, C), ("WpinT", C, 2 * h), ("Wpout", C, h), ("WpoutT", h, C)):
+    mats = [("Win", 2 * C, D), ("WinT", D, 2 * C), ("Wbig", Mb, C), ("WbigT", C, Mb), ("Wout", D, C), ("WoutT", C, D)]
+    if f is not None:
+        h = f.project_out.weight.shape[1]
+        mats += [("Wpin", 2 * h, C), ("WpinT", C, 2 * h), ("Wpout", C, h), ("WpoutT", h, C)]
+    for name, rows, cols in mats:
         w.add(name, rows, _p16(cols))
     W = w.build()
     g = _Arena(torch.float32, device)
     g.add("A", 4 * C, N)
     g.add("cwf", C, 9)
-    g.add("fdwf", 2 * h, 9)
+    if f is not None:
+        g.add("fdwf", 2 * h, 9)
     G = g.build()
     d = lambda p: p.detach()
     jobs = [
-        (0, d(a.in_conv.weight), None, W["Win"], None, 2 * C, C, 0, _p16(C), 0),
-        (1, d(a.in_conv.weight), None, W["WinT"], None, 2 * C, C, 0, _p16(2 * C), 0),
+        (0, d(a.in_conv.weight), None, W["Win"], None, 2 * C, D, 0, _p16(D), 0),
+        (1, d(a.in_conv.weight), None, W["WinT"], None, 2 * C, D, 0, _p16(2 * C), 0),
         (2, d(a.x_proj_weight), d(a.dt_projs_weight), W["Wbig"], W["WbigT"], C, R, 2 * N, _p16(C), _p16(Mb)),
-        (0, d(a.out_conv.weight), None, W["Wout"], None, C, C, 0, _p16(C), 0),
-        (1, d(a.out_conv.weight), None, W["WoutT"], None, C, C, 0, _p16(C), 0),
-        (0, d(f.project_in.weight), None, W["Wpin"], None, 2 * h, C, 0, _p16(C), 0),
-        (1, d(f.project_in.weight), None, W["WpinT"], None, 2 * h, C, 0, _p16(2 * h), 0),
-        (0, d(f.project_out.weight), None, W["Wpout"], None, C, h, 0, _p16(h), 0),
-        (1, d(f.project_out.weight), None, W["WpoutT"], None, C, h, 0, _p16(C), 0),
+        (0, d(a.out_conv.weight), None, W["Wout"], None, D, C, 0, _p16(C), 0),
+        (1, d(a.out_conv.weight), None, W["WoutT"], None, D, C, 0, _p16(D), 0),
+    ]
+    if f is not None:
+        jobs += [
+            (0, d(f.project_in.weight), None, W["Wpin"], None, 2 * h, C, 0, _p16(C), 0),
+            (1, d(f.project_in.weight), None, W["WpinT"], None, 2 * h, C, 0, _p16(2 * h), 0),
+            (0, d(f.project_out.weight), None, W["Wpout"], None, C, h, 0, _p16(h), 0),
+            (1, d(f.project_out.weight), None, W["WpoutT"], None, C, h, 0, _p16(C), 0),
+        ]
+    jobs += [
         (3, d(a.A_logs), None, G["A"], None, 4 * C, N, 0, 0, 0),
         (4, d(a.conv2d.weight), None, G["cwf"], None, C, 9, 0, 0, 0),
-        (4, d(f.dwconv.weight), None, G["fdwf"], None, 2 * h, 9, 0, 0, 0),
     ]
+    if f is not None:
+        jobs.append((4, d(f.dwconv.weight), None, G["fdwf"], None, 2 * h, 9, 0, 0, 0))
     for j in jobs:
         assert j[1].dtype == torch.float32 and j[1].is_contiguous(), "fp32 contiguous parameters"
     ops.prep_block_weights(jobs, dtype)
@@ -165,12 +178,12 @@ class _Front(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, n1w, n1b, w_in, b_in, cw, cb, x_proj_w, dt_w, dt_b, A_logs, Ds, on_w, on_b, Win, WinT, Wbig, WbigT, A, cwf):
         with torch.autocast("cuda", enabled=False):
-            B, C, H, W = x.shape
+            B, D, H, W = x.shape
             L = H * W
-            N, R = A_logs.shape[1], dt_w.shape[2]
-            ln_mode = 1 if n1b is not None else 2
-            x3 = x.contiguous().view(B, C, L)
-            xz = ops.pixlin(x3, Win, _f32(b_in), ln=(ln_mode, _f32(n1w), _f32(n1b)))  # (B,2C,L): [x_pre | z_pre], no activation
+            C, N, R = cw.shape[0], A_logs.shape[1], dt_w.shape[2]
+            ln_mode = 0 if n1w is None else 1 if n1b is not None else 2  # 0: standalone SS2D_1, no norm1 in front of in_conv
+            x3 = x.contiguous().view(B, D, L)
+            xz = ops.pixlin(x3, Win, _f32(b_in), ln=(ln_mode, _f32(n1w), _f32(n1b)) if ln_mode else None)  # (B,2C,L): [x_pre | z_pre]
             cw9 = _f32(cw.view(C, 9))
             xc = ops.dwconv3x3(xz[:, :C], cw9, _f32(cb), C, H, W, 0)
             dbl4 = ops.pixlin(xc, Wbig).view(B, 4, C + 2 * N, L)   # delta, B, C of the four directions, pixel order
@@ -182,7 +195,7 @@ class _Front(torch.autograd.Function):
                                                  z_preact=True, return_ws=True)
             ctx.save_for_backward(x3, xz, xc, xs, dts, bc, ckpt, ws, A, n1w, n1b, w_in, cw, cb, x_proj_w, dt_w, dt_b, Ds, on_w, on_b,
                                   WinT, WbigT, cwf, b_in)
-            ctx.geom = (B, C, H, W, N, R, ln_mode)
+            ctx.geom = (B, D, C, H, W, N, R, ln_mode)
         return y2.view(B, C, H, W), pooled
 
     @staticmethod
@@ -190,12 +203,12 @@ class _Front(torch.autograd.Function):
         with torch.autocast("cuda", enabled=False):
             (x3, xz, xc, xs, dts, bc, ckpt, ws, A, n1w, n1b, w_in, cw, cb, x_proj_w, dt_w, dt_b, Ds, on_w, on_b,
              WinT, WbigT, cwf, b_in) = ctx.saved_tensors
-            B, C, H, W, N, R, ln_mode = ctx.geom
+            B, D, C, H, W, N, R, ln_mode = ctx.geom
             L, dt_, dev = H * W, x3.dtype, x3.device
             Mb = 4 * (C + 2 * N)
             z = _Arena(torch.float32, dev)  # every fp32 accumulator of this backward: one zero fill
             for name, shape in (("onw", (C,)), ("onb", (C,)), ("dA", (4 * C, N)), ("dD", (4 * C,)), ("dbias", (4 * C,)), ("dbig", (Mb, C)),
-                                ("dcw", (C, 9)), ("dcb", (C,)), ("dwin", (2 * C, C)), ("dbin", (2 * C,)), ("n1w", (C,)), ("n1b", (C,))):
+                                ("dcw", (C, 9)), ("dcb", (C,)), ("dwin", (2 * C, D)), ("dbin", (2 * C,)), ("n1w", (D,)), ("n1b", (D,))):
                 z.add(name, *shape)
             Z = z.build(zero=True)
             dy2 = dy2.to(dt_).contiguous().view(B, C, L)
@@ -241,15 +254,18 @@ class _Front(torch.autograd.Function):
             dxn = ops.pixlin(dxz, WinT)
             (g_win, k_win), (g_bin, k_bin) = _acc(w_in, Z["dwin"]), _acc(b_in, Z["dbin"])
             with _side(k_win and (b_in is None or k_bin), dev, x3, dxz, bit=2):
-                xn = ops.layernorm_fwd(x3, ln_mode, _f32(n1w), _f32(n1b))
+                xn = ops.layernorm_fwd(x3, ln_mode, _f32(n1w), _f32(n1b)) if ln_mode else x3
                 d_win = ops.pixlin_wgrad(dxz, xn, out=g_win, dbias=g_bin, deterministic=False).view_as(w_in)
             (g_n1w, k_n1w), (g_n1b, k_n1b) = _acc(n1w, Z["n1w"]), _acc(n1b, Z["n1b"])
-            dx, st1 = ops.layernorm_bwd(x3, dxn, ln_mode, _f32(n1w), phase="data")
-            with _side(k_n1w and (n1b is None or k_n1b), dev, x3, dxn, st1, bit=128):
-                d_n1w, d_n1b = ops.layernorm_bwd(x3, dxn, ln_mode, _f32(n1w), zeroed=(g_n1w, g_n1b), phase="params", stats=st1)
+            if ln_mode:
+                dx, st1 = ops.layernorm_bwd(x3, dxn, ln_mode, _f32(n1w), phase="data")
+                with _side(k_n1w and (n1b is None or k_n1b), dev, x3, dxn, st1, bit=128):
+                    d_n1w, d_n1b = ops.layernorm_bwd(x3, dxn, ln_mode, _f32(n1w), zeroed=(g_n1w, g_n1b), phase="params", stats=st1)
+            else:
+                dx, d_n1w, d_n1b = dxn, None, None
             dA_logs = dA * A  # A = -exp(A_logs)
         drop = lambda t, direct: None if direct else t  # accumulated straight into .grad: nothing for autograd to add
-        return (dx.view(B, C, H, W), drop(d_n1w, k_n1w), drop(d_n1b, k_n1b), drop(d_win, k_win), drop(g_bin, k_bin),
+        return (dx.view(B, D, H, W), drop(d_n1w, k_n1w), drop(d_n1b, k_n1b), drop(d_win, k_win), drop(g_bin, k_bin),
                 drop(d_cw.view_as(cw), k_cw), drop(d_cb, k_cb), d_xproj, d_dtw, drop(dbias.view_as(dt_b), k_dbias),
                 dA_logs, drop(dD, k_dD), drop(d_onw, k_onw), drop(d_onb, k_onb), None, None, None, None, None, None)
 
@@ -310,25 +326,63 @@ class _Tail(torch.autograd.Function):
             with _side(k_n2w and (n2b is None or k_n2b), dev, x1, dx1n, st2, bit=128):
                 d_n2w, d_n2b = ops.layernorm_bwd(x1, dx1n, ln_mode, _f32(n2w), zeroed=(g_n2w, g_n2b), phase="params", stats=st2)
             # out_conv with the channel gate in front, residual behind
-            dyg = ops.pixlin(dx1, WoutT)
-            dy2, dc = ops.channel_gate_bwd(dyg, y23, cg, gate_mode)
-            g_bout, k_bout = _acc(b_out, Z["bout"])
-            g_wout = getattr(w_out, "grad", None)
-            k_wout = _DIRECT_GRADS and g_wout is not None and g_wout.dtype == torch.float32 and not torch.is_grad_enabled()
-            with _side(k_wout and (b_out is None or k_bout), dev, dx1, y23, cg, Z["wb"], bit=16):
-                wb = ops.pixlin_wgrad(dx1, y23, per_batch=True, out=Z["wb"], dbias=g_bout, deterministic=False)  # (B, C_out, C_in): scaled per image by the gate
-                if gate_mode == 1:
-                    d_wout = (wb * (1.0 + cg)[:, None, :]).sum(0)
-                else:  # y + c: the gate adds c[b,k] * sum_p dx1[b,m,p]  (per-image row sums: B*C values)
-                    d_wout = wb.sum(0) + torch.einsum("bm,bk->mk", dx1.float().sum(2), cg)
-                if k_wout:
-                    g_wout.add_(d_wout.view_as(g_wout))
-                    d_wout = None
+            dy2, dc, d_wout, d_bout = _out_conv_bwd(dx1, y23, cg, w_out, b_out, WoutT, gate_mode, Z["wb"], Z["bout"])
         drop = lambda t, direct: None if direct else t
-        return (dy2.view(B, C, H, W), dc, dx1.view(B, C, H, W), None if d_wout is None else d_wout.view_as(w_out), drop(g_bout, k_bout) if b_out is not None else None,
+        return (dy2.view(B, C, H, W), dc, dx1.view(B, C, H, W), d_wout, d_bout,
                 drop(d_n2w, k_n2w), drop(d_n2b, k_n2b), drop(d_wpin, k_wpin), drop(g_bpin, k_bpin) if b_pin is not None else None,
                 drop(d_fdw.view_as(fdw), k_fdw), drop(d_fdwb, k_fdwb), drop(d_wpout, k_wpout),
                 drop(g_bpout, k_bpout) if b_pout is not None else None, None, None, None, None, None, None, None, None)
+
+
+def _out_conv_bwd(dx1, y23, cg, w_out, b_out, WoutT, gate_mode, wb_acc, bout_acc):
+    """backward of the channel gate + out_conv: dx1 (B,D,L) contiguous, the gradient of out_conv's output; y23 (B,E,L) its gated input
+    before the gate; cg (B,E) fp32 the gate; wb_acc (B,D,E) / bout_acc (D) zero-filled fp32 accumulators.
+    -> (dy2 (B,E,L), dgate (B,E) fp32, d out_conv.weight, d out_conv.bias), the last two None when added straight into .grad"""
+    dev = dx1.device
+    dyg = ops.pixlin(dx1, WoutT)
+    dy2, dc = ops.channel_gate_bwd(dyg, y23, cg, gate_mode)
+    g_bout, k_bout = _acc(b_out, bout_acc)
+    g_wout = getattr(w_out, "grad", None)
+    k_wout = _DIRECT_GRADS and g_wout is not None and g_wout.dtype == torch.float32 and not torch.is_grad_enabled()
+    with _side(k_wout and (b_out is None or k_bout), dev, dx1, y23, cg, wb_acc, bit=16):
+        wb = ops.pixlin_wgrad(dx1, y23, per_batch=True, out=wb_acc, dbias=g_bout, deterministic=False)  # (B, C_out, C_in): scaled per image by the gate
+        if gate_mode == 1:
+            d_wout = (wb * (1.0 + cg)[:, None, :]).sum(0)
+        else:  # y + c: the gate adds c[b,k] * sum_p dx1[b,m,p]  (per-image row sums: B*C values)
+            d_wout = wb.sum(0) + torch.einsum("bm,bk->mk", dx1.float().sum(2), cg)
+        if k_wout:
+            g_wout.add_(d_wout.view_as(g_wout))
+            d_wout = None
+    return dy2, dc, None if d_wout is None else d_wout.view_as(w_out), None if b_out is None or k_bout else g_bout
+
+
+class _OutConv(torch.autograd.Function):
+    """channel gate + out_conv of a standalone SS2D_1 (no residual behind): (y2 (B,E,H,W), c (B,E) fp32) -> (B,D,H,W)"""
+
+    @staticmethod
+    def forward(ctx, y2, c, w_out, b_out, gate_mode, Wout, WoutT):
+        with torch.autocast("cuda", enabled=False):
+            B, C, H, W = y2.shape
+            D = w_out.shape[0]
+            y23 = y2.contiguous().view(B, C, H * W)
+            cg = c.detach().float().contiguous()
+            out = ops.pixlin(y23, Wout, _f32(b_out), gate=cg, gate_mode=gate_mode)
+            ctx.save_for_backward(y23, cg, w_out, b_out, WoutT)
+            ctx.geom = (B, C, D, H, W, gate_mode)
+        return out.view(B, D, H, W)
+
+    @staticmethod
+    def backward(ctx, dout):
+        with torch.autocast("cuda", enabled=False):
+            y23, cg, w_out, b_out, WoutT = ctx.saved_tensors
+            B, C, D, H, W, gate_mode = ctx.geom
+            z = _Arena(torch.float32, y23.device)
+            z.add("wb", B, D, C)
+            z.add("bout", D)
+            Z = z.build(zero=True)
+            dout3 = dout.to(y23.dtype).contiguous().view(B, D, H * W)
+            dy2, dc, d_wout, d_bout = _out_conv_bwd(dout3, y23, cg, w_out, b_out, WoutT, gate_mode, Z["wb"], Z["bout"])
+        return dy2.view(B, C, H, W), dc, d_wout, d_bout, None, None, None
 
 
 class _Channel(torch.autograd.Function):
@@ -376,17 +430,34 @@ def channel_gate(a, pooled, L):
         return a.cforward_pooled(pooled * (1.0 / L))
 
 
+def _front(a, x, P, norm=None):
+    """_Front of attn module `a` (norm: the block's norm1 LayerNorm, fused into in_conv) -> (y2, pooled sums)"""
+    on = a.out_norm.body
+    return _Front.apply(x, None if norm is None else norm.weight, getattr(norm, "bias", None), a.in_conv.weight, a.in_conv.bias,
+                        a.conv2d.weight, a.conv2d.bias, a.x_proj_weight, a.dt_projs_weight, a.dt_projs_bias, a.A_logs, a.Ds, on.weight,
+                        on.bias, P["Win"], P["WinT"], P["Wbig"], P["WbigT"], P["A"], P["cwf"])
+
+
 def block_forward(block, x: torch.Tensor) -> torch.Tensor:
     """MamberBlock.forward with autograd on the fused kernels (x: (B,C,H,W) CUDA tensor in the compute dtype)."""
     a, f = block.attn, block.ffn
     L = x.shape[2] * x.shape[3]
-    n1, n2, on = block.norm1.body, block.norm2.body, a.out_norm.body
+    n2 = block.norm2.body
     with torch.no_grad():
         P = prepare_block(block, x.dtype, x.device)
-    y2, pooled = _Front.apply(x, n1.weight, getattr(n1, "bias", None), a.in_conv.weight, a.in_conv.bias, a.conv2d.weight,
-                              a.conv2d.bias, a.x_proj_weight, a.dt_projs_weight, a.dt_projs_bias, a.A_logs, a.Ds, on.weight, on.bias,
-                              P["Win"], P["WinT"], P["Wbig"], P["WbigT"], P["A"], P["cwf"])
+    y2, pooled = _front(a, x, P, block.norm1.body)
     c = channel_gate(a, pooled, L)  # (B, C) fp32: channel-direction OSS on the pooled descriptor
     return _Tail.apply(y2, c, x, a.out_conv.weight, a.out_conv.bias, n2.weight, getattr(n2, "bias", None), f.project_in.weight,
                        f.project_in.bias, f.dwconv.weight, f.dwconv.bias, f.project_out.weight, f.project_out.bias,
                        1 if a.gate == "mul" else 2, P["Wout"], P["WoutT"], P["Wpin"], P["WpinT"], P["Wpout"], P["WpoutT"], P["fdwf"])
+
+
+def ss2d_forward(a, x: torch.Tensor) -> torch.Tensor:
+    """SS2D_1.forward of a standalone module with autograd on the fused kernels (x: (B,D,H,W) CUDA tensor in the compute dtype):
+    _Front without norm1, the channel gate, then _OutConv (gate + out_conv, no residual)."""
+    L = x.shape[2] * x.shape[3]
+    with torch.no_grad():
+        P = prepare_block(a, x.dtype, x.device)
+    y2, pooled = _front(a, x, P)
+    c = channel_gate(a, pooled, L)  # (B, E) fp32
+    return _OutConv.apply(y2, c, a.out_conv.weight, a.out_conv.bias, 1 if a.gate == "mul" else 2, P["Wout"], P["WoutT"])
