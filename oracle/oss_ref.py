@@ -81,8 +81,16 @@ def ss2d(sd, pre, x, gate):
     y = y + ycol.view(B_, C, W, H).transpose(2, 3).reshape(B_, C, L)
     y1 = _ln(y.view(B_, C, H, W), g("out_norm.body.weight"), g("out_norm.body.bias"))
     y2 = _q(y1 * z)
-    # channel direction (forward + backward over the pooled channel descriptor, :438-483)
-    pooled = y2.mean((2, 3))  # (B, C)
+    c = channel(sd, pre, y2.mean((2, 3)))[:, :, None, None]  # (B,C,1,1)
+    y2 = y2 * c + y2 if gate == "mul" else y2 + c
+    return F.conv2d(y2, _qw(g("out_conv.weight")), g("out_conv.bias"))
+
+
+def channel(sd, pre, pooled):
+    """channel direction (forward + backward scan over the pooled channel descriptor, :438-483): pooled (B, C) channel means ->
+    channel_norm output (B, C)"""
+    g = lambda k: sd[pre + k]
+    B_, C = pooled.shape
     if pre + "conv_cin.weight" in sd:
         seq = pooled[:, None, :] * g("conv_cin.weight").view(1, -1, 1) + g("conv_cin.bias").view(1, -1, 1)
     else:
@@ -98,9 +106,7 @@ def ss2d(sd, pre, x, gate):
     yc = oc[:, 0] + oc[:, 1].flip(-1)  # (B, dc, C)
     if pre + "conv_cout.weight" in sd:
         yc = (yc * g("conv_cout.weight").view(1, -1, 1)).sum(1, keepdim=True) + g("conv_cout.bias").view(1, 1, 1)
-    c = _ln(yc.transpose(1, 2).unsqueeze(-1), g("channel_norm.body.weight"), g("channel_norm.body.bias"))  # (B,C,1,1)
-    y2 = y2 * c + y2 if gate == "mul" else y2 + c
-    return F.conv2d(y2, _qw(g("out_conv.weight")), g("out_conv.bias"))
+    return _ln(yc.transpose(1, 2).unsqueeze(-1), g("channel_norm.body.weight"), g("channel_norm.body.bias")).view(B_, C)
 
 
 def ffn(sd, pre, x):
