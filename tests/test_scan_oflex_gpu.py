@@ -78,11 +78,12 @@ def fwd_into(out, u, delta, A, Bm, Cm, Dv, bias, softplus, out_f32):
     from vmambair_b200 import _lib, ops
     b, d, l = u.shape
     n, g = A.shape[1], Bm.shape[1]
+    P = ops._ptr
     a = _lib.ScanFwdArgs(
-        ops._ptr(u), ops._ptr(delta), ops._ptr(A), ops._ptr(Bm), ops._ptr(Cm), ops._ptr(Dv), ops._ptr(bias), ops._ptr(out), None,
-        b, d, l, n, g, u.stride(0), u.stride(1), delta.stride(0), delta.stride(1), out.stride(0), out.stride(1),
-        Bm.stride(0), Bm.stride(1), Bm.stride(2), Cm.stride(0), Cm.stride(1), Cm.stride(2),
-        int(softplus), ops._DT[u.dtype], out_f32)
+        u=P(u), delta=P(delta), A=P(A), Bm=P(Bm), Cm=P(Cm), D=P(Dv), delta_bias=P(bias), out=P(out), ckpt=None,
+        batch=b, dim=d, seqlen=l, dstate=n, ngroups=g, u_bs=u.stride(0), u_ds=u.stride(1), delta_bs=delta.stride(0),
+        delta_ds=delta.stride(1), out_bs=out.stride(0), out_ds=out.stride(1), B_bs=Bm.stride(0), B_gs=Bm.stride(1), B_ns=Bm.stride(2),
+        C_bs=Cm.stride(0), C_gs=Cm.stride(1), C_ns=Cm.stride(2), delta_softplus=int(softplus), dtype=ops._DT[u.dtype], out_f32=out_f32)
     return _lib.lib().vmb_selective_scan_fwd(C.byref(a), ops._stream(u))
 
 
@@ -417,9 +418,13 @@ def test_errors_raise():
     L = _lib.lib()
     ws = torch.empty(L.vmb_scan_bwd_workspace_bytes(1, 2, 16, 512), dtype=torch.uint8, device="cuda")
     P = ops._ptr
-    a = _lib.ScanBwdArgs(P(u), P(delta), P(A), P(Bm), P(Cm), P(Dv), P(bias), P(u), P(ck32), P(du), P(dd), P(dA), P(dB), P(dC),
-                         P(dD), P(db), P(ws), 1, 16, 512, 16, 2, *u.stride()[:2], *delta.stride()[:2], *u.stride()[:2],
-                         *du.stride()[:2], *dd.stride()[:2], *Bm.stride()[:3], *Cm.stride()[:3], 1, _lib.DT_F32, 1)
+    a = _lib.ScanBwdArgs(u=P(u), delta=P(delta), A=P(A), Bm=P(Bm), Cm=P(Cm), D=P(Dv), delta_bias=P(bias), dout=P(u), ckpt=P(ck32),
+                         du=P(du), ddelta=P(dd), dA=P(dA), dB=P(dB), dC=P(dC), dD=P(dD), ddelta_bias=P(db), workspace=P(ws),
+                         batch=1, dim=16, seqlen=512, dstate=16, ngroups=2, u_bs=u.stride(0), u_ds=u.stride(1),
+                         delta_bs=delta.stride(0), delta_ds=delta.stride(1), dout_bs=u.stride(0), dout_ds=u.stride(1),
+                         du_bs=du.stride(0), du_ds=du.stride(1), ddelta_bs=dd.stride(0), ddelta_ds=dd.stride(1),
+                         B_bs=Bm.stride(0), B_gs=Bm.stride(1), B_ns=Bm.stride(2), C_bs=Cm.stride(0), C_gs=Cm.stride(1),
+                         C_ns=Cm.stride(2), delta_softplus=1, dtype=_lib.DT_F32, dout_f32=1)
     assert L.vmb_selective_scan_bwd(C.byref(a), ops._stream(u)) != 0
     assert "dout_f32" in L.vmb_last_error().decode()
     # ndstate: the (D,) / (B, G, L) layout only

@@ -1,6 +1,10 @@
 """ctypes loader of the C-ABI library (include/vmambair_b200.h).
 
 There is NO fallback: if the CUDA library is missing or a call fails, a RuntimeError is raised.
+
+Each Structure mirrors the header typedef its `_c_name_` names, field for field; tests/test_abi_cpu.py compiles the header and checks
+sizes, offsets and names against these mirrors.  Build them with keyword arguments only (that test rejects positional ones), so a
+value can never land in the wrong field.
 """
 from __future__ import annotations
 
@@ -18,6 +22,7 @@ vp = C.c_void_p
 
 
 class ScanFwdArgs(C.Structure):
+    _c_name_ = "vmb_scan_fwd_args"
     _fields_ = [
         ("u", vp), ("delta", vp), ("A", vp), ("Bm", vp), ("Cm", vp), ("D", vp), ("delta_bias", vp),
         ("out", vp), ("ckpt", vp),
@@ -29,6 +34,7 @@ class ScanFwdArgs(C.Structure):
 
 
 class ScanBwdArgs(C.Structure):
+    _c_name_ = "vmb_scan_bwd_args"
     _fields_ = [
         ("u", vp), ("delta", vp), ("A", vp), ("Bm", vp), ("Cm", vp), ("D", vp), ("delta_bias", vp),
         ("dout", vp), ("ckpt", vp),
@@ -42,6 +48,7 @@ class ScanBwdArgs(C.Structure):
 
 
 class PixlinArgs(C.Structure):
+    _c_name_ = "vmb_pixlin_args"
     _fields_ = [
         ("x", vp), ("w", vp), ("bias", vp), ("residual", vp), ("out", vp), ("ln_w", vp), ("ln_b", vp), ("gate", vp),
         ("ln_mode", C.c_int), ("gate_mode", C.c_int), ("act_from", C.c_int), ("act_to", C.c_int),
@@ -52,6 +59,7 @@ class PixlinArgs(C.Structure):
 
 
 class DwconvArgs(C.Structure):
+    _c_name_ = "vmb_dwconv_args"
     _fields_ = [
         ("x", vp), ("w", vp), ("bias", vp), ("out", vp),
         ("batch", C.c_int), ("c_out", C.c_int), ("H", C.c_int), ("W", C.c_int), ("mode", C.c_int),
@@ -60,6 +68,7 @@ class DwconvArgs(C.Structure):
 
 
 class CrossScanArgs(C.Structure):
+    _c_name_ = "vmb_cross_scan_args"
     _fields_ = [
         ("src", vp * 4), ("out", vp),
         ("batch", C.c_int), ("rows", C.c_int), ("H", C.c_int), ("W", C.c_int),
@@ -68,6 +77,7 @@ class CrossScanArgs(C.Structure):
 
 
 class MergeArgs(C.Structure):
+    _c_name_ = "vmb_merge_args"
     _fields_ = [
         ("ys", vp), ("z", vp), ("ln_w", vp), ("ln_b", vp), ("y2", vp), ("pooled", vp),
         ("batch", C.c_int), ("C", C.c_int), ("H", C.c_int), ("W", C.c_int),
@@ -77,14 +87,17 @@ class MergeArgs(C.Structure):
 
 
 class TransposeArgs(C.Structure):
+    _c_name_ = "vmb_transpose_args"
     _fields_ = [("x", vp), ("out", vp), ("planes", C.c_int), ("H", C.c_int), ("W", C.c_int), ("dtype", C.c_int)]
 
 
 class PixelShuffleArgs(C.Structure):
+    _c_name_ = "vmb_pixel_shuffle_args"
     _fields_ = [("x", vp), ("out", vp), ("batch", C.c_int), ("H", C.c_int), ("W", C.c_int), ("C", C.c_int), ("dtype", C.c_int)]
 
 
 class Conv3x3Args(C.Structure):
+    _c_name_ = "vmb_conv3x3_args"
     _fields_ = [
         ("x", vp), ("w", vp), ("bias", vp), ("out", vp), ("add", vp),
         ("batch", C.c_int), ("Cin", C.c_int), ("Cout", C.c_int), ("H", C.c_int), ("W", C.c_int),
@@ -95,6 +108,7 @@ class Conv3x3Args(C.Structure):
 
 
 class ScanGroupedArgs(C.Structure):
+    _c_name_ = "vmb_scan_grouped_args"
     _fields_ = [
         ("u", vp * 4), ("delta", vp * 4), ("Bm", vp * 4), ("Cm", vp * 4), ("out", vp * 4), ("rev", C.c_int * 4),
         ("A", vp), ("D", vp), ("delta_bias", vp),
@@ -106,6 +120,7 @@ class ScanGroupedArgs(C.Structure):
 
 
 class ScanGroupedBwdArgs(C.Structure):
+    _c_name_ = "vmb_scan_grouped_bwd_args"
     _fields_ = [
         ("u", vp * 4), ("delta", vp * 4), ("Bm", vp * 4), ("Cm", vp * 4), ("dout", vp * 4),
         ("du", vp * 4), ("ddelta", vp * 4), ("dB", vp * 4), ("dC", vp * 4), ("rev", C.c_int * 4),
@@ -120,6 +135,7 @@ class ScanGroupedBwdArgs(C.Structure):
 
 
 class ChannelArgs(C.Structure):
+    _c_name_ = "vmb_channel_args"
     _fields_ = [
         ("pooled", vp), ("inv_count", C.c_float),
         ("cin_w", vp), ("cin_b", vp), ("xc_proj", vp), ("dtc_w", vp), ("dtc_b", vp), ("Ac_logs", vp), ("Dsc", vp),
@@ -129,12 +145,14 @@ class ChannelArgs(C.Structure):
 
 
 class LnFwdArgs(C.Structure):
+    _c_name_ = "vmb_ln_fwd_args"
     _fields_ = [("x", vp), ("w", vp), ("b", vp), ("y", vp), ("stats", vp),
                 ("batch", C.c_int), ("C", C.c_int), ("L", C.c_int), ("mode", C.c_int),
                 ("x_bs", i64), ("x_cs", i64), ("y_bs", i64), ("y_cs", i64), ("dtype", C.c_int)]
 
 
 class LnBwdArgs(C.Structure):
+    _c_name_ = "vmb_ln_bwd_args"
     _fields_ = [("x", vp), ("g", vp), ("add", vp), ("w", vp), ("dx", vp), ("dw", vp), ("db", vp), ("stats", vp),
                 ("batch", C.c_int), ("C", C.c_int), ("L", C.c_int), ("mode", C.c_int),
                 ("x_bs", i64), ("x_cs", i64), ("g_bs", i64), ("g_cs", i64), ("a_bs", i64), ("a_cs", i64),
@@ -142,6 +160,7 @@ class LnBwdArgs(C.Structure):
 
 
 class MergeBwdArgs(C.Structure):
+    _c_name_ = "vmb_merge_bwd_args"
     _fields_ = [("merged", vp), ("stats", vp), ("z", vp), ("dy2", vp), ("dpooled", vp), ("w", vp), ("b", vp),
                 ("dm", vp), ("dz", vp), ("dw", vp), ("db", vp),
                 ("batch", C.c_int), ("C", C.c_int), ("L", C.c_int),
@@ -149,29 +168,34 @@ class MergeBwdArgs(C.Structure):
 
 
 class DwconvBwdArgs(C.Structure):
+    _c_name_ = "vmb_dwconv_bwd_args"
     _fields_ = [("x", vp), ("w", vp), ("bias", vp), ("g", vp), ("dv", vp), ("dw", vp), ("dbias", vp),
                 ("batch", C.c_int), ("c_out", C.c_int), ("H", C.c_int), ("W", C.c_int), ("mode", C.c_int),
                 ("x_bs", i64), ("x_cs", i64), ("g_bs", i64), ("g_cs", i64), ("dv_bs", i64), ("dv_cs", i64), ("dtype", C.c_int)]
 
 
 class GateBwdArgs(C.Structure):
+    _c_name_ = "vmb_gate_bwd_args"
     _fields_ = [("dyg", vp), ("y2", vp), ("gate", vp), ("dy2", vp), ("dgate", vp),
                 ("batch", C.c_int), ("C", C.c_int), ("L", C.c_int), ("mode", C.c_int), ("dtype", C.c_int)]
 
 
 class WgradArgs(C.Structure):
+    _c_name_ = "vmb_wgrad_args"
     _fields_ = [("dy", vp), ("x", vp), ("out", vp), ("batch", C.c_int), ("M", C.c_int), ("K", C.c_int), ("L", C.c_int),
                 ("dy_bs", i64), ("dy_cs", i64), ("x_bs", i64), ("x_cs", i64), ("per_batch", C.c_int), ("dtype", C.c_int),
                 ("dbias", vp), ("workspace", vp), ("deterministic", C.c_int)]
 
 
 class ChannelBwdArgs(C.Structure):
+    _c_name_ = "vmb_channel_bwd_args"
     _fields_ = [("fwd", ChannelArgs), ("dc_out", vp), ("d_pooled", vp),
                 ("d_cin_w", vp), ("d_cin_b", vp), ("d_xc_proj", vp), ("d_dtc_w", vp), ("d_dtc_b", vp), ("d_Ac_logs", vp), ("d_Dsc", vp),
                 ("d_cout_w", vp), ("d_cout_b", vp), ("d_cn_w", vp), ("d_cn_b", vp), ("scratch", vp)]
 
 
 class CrossScanCArgs(C.Structure):
+    _c_name_ = "vmb_cross_scan_c_args"
     _fields_ = [("x", vp), ("x_proj_weight", vp), ("x_proj_bias", vp), ("dt_projs_weight", vp), ("dt_projs_bias", vp),
                 ("A_logs", vp), ("Ds", vp), ("y", vp),
                 ("batch", C.c_int), ("D", C.c_int), ("L", C.c_int), ("R", C.c_int), ("N", C.c_int),
@@ -179,19 +203,23 @@ class CrossScanCArgs(C.Structure):
 
 
 class CrossScanCBwdArgs(C.Structure):
+    _c_name_ = "vmb_cross_scan_c_bwd_args"
     _fields_ = [("fwd", CrossScanCArgs), ("dy", vp), ("dx", vp), ("d_params", vp), ("workspace", vp)]
 
 
 class PrepJob(C.Structure):
+    _c_name_ = "vmb_prep_job"
     _fields_ = [("src", vp), ("src2", vp), ("dst", vp), ("dst2", vp), ("type", C.c_int), ("M", C.c_int), ("K", C.c_int),
                 ("N2", C.c_int), ("ld", C.c_int), ("ld2", C.c_int)]
 
 
 class PrepArgs(C.Structure):
+    _c_name_ = "vmb_prep_args"
     _fields_ = [("jobs", PrepJob * 16), ("njobs", C.c_int), ("dtype", C.c_int)]
 
 
 class AdamArgs(C.Structure):
+    _c_name_ = "vmb_adam_args"
     _fields_ = [("param", vp), ("grad", vp), ("exp_avg", vp), ("exp_avg_sq", vp), ("ema", vp), ("state", vp),
                 ("n", C.c_long), ("lr", C.c_float), ("beta1", C.c_float), ("beta2", C.c_float), ("eps", C.c_float),
                 ("weight_decay", C.c_float), ("decoupled_weight_decay", C.c_int),

@@ -147,28 +147,30 @@ def prepare_block(mod, dtype, device):
         g.add("fdwf", 2 * h, 9)
     G = g.build()
     d = lambda p: p.detach()
+    Job = ops.PrepJob
     jobs = [
-        (0, d(a.in_conv.weight), None, W["Win"], None, 2 * C, D, 0, _p16(D), 0),
-        (1, d(a.in_conv.weight), None, W["WinT"], None, 2 * C, D, 0, _p16(2 * C), 0),
-        (2, d(a.x_proj_weight), d(a.dt_projs_weight), W["Wbig"], W["WbigT"], C, R, 2 * N, _p16(C), _p16(Mb)),
-        (0, d(a.out_conv.weight), None, W["Wout"], None, D, C, 0, _p16(C), 0),
-        (1, d(a.out_conv.weight), None, W["WoutT"], None, D, C, 0, _p16(D), 0),
+        Job(type=ops.PREP_PAD_COPY, src=d(a.in_conv.weight), dst=W["Win"], M=2 * C, K=D, ld=_p16(D)),
+        Job(type=ops.PREP_TRANSPOSE, src=d(a.in_conv.weight), dst=W["WinT"], M=2 * C, K=D, ld=_p16(2 * C)),
+        Job(type=ops.PREP_FOLD, src=d(a.x_proj_weight), src2=d(a.dt_projs_weight), dst=W["Wbig"], dst2=W["WbigT"], M=C, K=R, N2=2 * N,
+            ld=_p16(C), ld2=_p16(Mb)),
+        Job(type=ops.PREP_PAD_COPY, src=d(a.out_conv.weight), dst=W["Wout"], M=D, K=C, ld=_p16(C)),
+        Job(type=ops.PREP_TRANSPOSE, src=d(a.out_conv.weight), dst=W["WoutT"], M=D, K=C, ld=_p16(D)),
     ]
     if f is not None:
         jobs += [
-            (0, d(f.project_in.weight), None, W["Wpin"], None, 2 * h, C, 0, _p16(C), 0),
-            (1, d(f.project_in.weight), None, W["WpinT"], None, 2 * h, C, 0, _p16(2 * h), 0),
-            (0, d(f.project_out.weight), None, W["Wpout"], None, C, h, 0, _p16(h), 0),
-            (1, d(f.project_out.weight), None, W["WpoutT"], None, C, h, 0, _p16(C), 0),
+            Job(type=ops.PREP_PAD_COPY, src=d(f.project_in.weight), dst=W["Wpin"], M=2 * h, K=C, ld=_p16(C)),
+            Job(type=ops.PREP_TRANSPOSE, src=d(f.project_in.weight), dst=W["WpinT"], M=2 * h, K=C, ld=_p16(2 * h)),
+            Job(type=ops.PREP_PAD_COPY, src=d(f.project_out.weight), dst=W["Wpout"], M=C, K=h, ld=_p16(h)),
+            Job(type=ops.PREP_TRANSPOSE, src=d(f.project_out.weight), dst=W["WpoutT"], M=C, K=h, ld=_p16(C)),
         ]
     jobs += [
-        (3, d(a.A_logs), None, G["A"], None, 4 * C, N, 0, 0, 0),
-        (4, d(a.conv2d.weight), None, G["cwf"], None, C, 9, 0, 0, 0),
+        Job(type=ops.PREP_NEG_EXP, src=d(a.A_logs), dst=G["A"], M=4 * C, K=N),
+        Job(type=ops.PREP_FLIP_TAPS, src=d(a.conv2d.weight), dst=G["cwf"], M=C, K=9),
     ]
     if f is not None:
-        jobs.append((4, d(f.dwconv.weight), None, G["fdwf"], None, 2 * h, 9, 0, 0, 0))
+        jobs.append(Job(type=ops.PREP_FLIP_TAPS, src=d(f.dwconv.weight), dst=G["fdwf"], M=2 * h, K=9))
     for j in jobs:
-        assert j[1].dtype == torch.float32 and j[1].is_contiguous(), "fp32 contiguous parameters"
+        assert j.src.dtype == torch.float32 and j.src.is_contiguous(), "fp32 contiguous parameters"
     ops.prep_block_weights(jobs, dtype)
     W.update(G)
     return W

@@ -7,6 +7,7 @@ library owns nothing), on the input's device and current stream.
 """
 from __future__ import annotations
 
+import collections
 import ctypes as C
 import math
 
@@ -36,7 +37,7 @@ class _timed:
         self.tag, self.nbytes, self.dev, self.kernels = tag, nbytes, dev, kernels
 
     def __enter__(self):
-        if _TIMING is not None:
+        if _TIMING is not None and self.tag is not None:
             self.s = torch.cuda.Event(enable_timing=True)
             self.e = torch.cuda.Event(enable_timing=True)
             self.s.record(torch.cuda.current_stream(self.dev))
@@ -44,9 +45,18 @@ class _timed:
     def __exit__(self, *a):
         global _LAUNCHES
         _LAUNCHES += self.kernels
-        if _TIMING is not None:
+        if _TIMING is not None and self.tag is not None:
             self.e.record(torch.cuda.current_stream(self.dev))
             _TIMING.append((self.tag, self.nbytes, self.s, self.e))
+
+
+def _run(name, t, tag, *args, nbytes=0, kernels=1):
+    """The one way this module calls the library: `name`(*args, stream) on t's device and current stream, its status checked and
+    its `kernels` launches counted.  Under set_timing the call is recorded as (tag, nbytes, events); tag None: counted, not timed.
+    A struct argument is passed by reference (the argtypes in _lib.SYMBOLS declare a pointer)."""
+    fn = getattr(_lib.lib(), name)
+    with torch.cuda.device(t.device), _timed(tag, nbytes, t.device, kernels):
+        _lib.check(fn(*args, _stream(t)), name)
 
 
 def _stream(t: torch.Tensor):
@@ -55,6 +65,16 @@ def _stream(t: torch.Tensor):
 
 def _ptr(t):
     return None if t is None else C.c_void_p(t.data_ptr())
+
+
+def _ptr4(ts):
+    """up to four tensors -> a `void* [4]` member, zero-padded"""
+    return (C.c_void_p * 4)(*[t.data_ptr() for t in ts])
+
+
+def _rev4(revs):
+    """up to four direction flags -> an `int rev[4]` member, zero-padded"""
+    return (C.c_int * 4)(*map(int, revs))
 
 
 def _check_common(u, delta, A, B, C_, D, delta_bias, who):
@@ -114,7 +134,6 @@ def selective_scan_fwd(u, delta, A, B, C_, D=None, delta_bias=None, delta_softpl
     out_float: out is fp32 whatever the input dtype -- with bf16 / fp16 inputs the fp32 accumulator is stored without rounding
     (the reference's selective_scan_cuda_oflex, cusoflex/selective_scan_oflex.cpp:219,235-239)."""
     b, d, l, n, g = _check_common(u, delta, A, B, C_, D, delta_bias, "selective_scan_fwd")
-    L = _lib.lib()
     out_f32 = bool(out_float) and u.dtype != torch.float32
     if out_f32:
         out = torch.empty(delta.shape, dtype=torch.float32, device=delta.device)
@@ -125,15 +144,14 @@ def selective_scan_fwd(u, delta, A, B, C_, D=None, delta_bias=None, delta_softpl
     ck = ckpt_interval()
     ckpt = torch.empty((b, d, (l + ck - 1) // ck, n), dtype=torch.float32, device=u.device) if need_ckpt else None
     a = _lib.ScanFwdArgs(
-        _ptr(u), _ptr(delta), _ptr(A), _ptr(B), _ptr(C_), _ptr(D), _ptr(delta_bias), _ptr(out), _ptr(ckpt),
-        b, d, l, n, g,
-        u.stride(0), u.stride(1), delta.stride(0), delta.stride(1), out.stride(0), out.stride(1),
-        B.stride(0), B.stride(1), B.stride(2), C_.stride(0), C_.stride(1), C_.stride(2),
-        int(bool(delta_softplus)), _DT[u.dtype], int(out_f32))
+        u=_ptr(u), delta=_ptr(delta), A=_ptr(A), Bm=_ptr(B), Cm=_ptr(C_), D=_ptr(D), delta_bias=_ptr(delta_bias), out=_ptr(out),
+        ckpt=_ptr(ckpt), batch=b, dim=d, seqlen=l, dstate=n, ngroups=g,
+        u_bs=u.stride(0), u_ds=u.stride(1), delta_bs=delta.stride(0), delta_ds=delta.stride(1), out_bs=out.stride(0), out_ds=out.stride(1),
+        B_bs=B.stride(0), B_gs=B.stride(1), B_ns=B.stride(2), C_bs=C_.stride(0), C_gs=C_.stride(1), C_ns=C_.stride(2),
+        delta_softplus=int(bool(delta_softplus)), dtype=_DT[u.dtype], out_f32=int(out_f32))
     es = u.element_size()
     nbytes = es * (2 * b * d * l + 2 * b * g * n * l) + out.element_size() * b * d * l + 4 * (d * n + 2 * d)  # SURVEY.md 8(d): every operand once
-    with torch.cuda.device(u.device), _timed("scan_fwd", nbytes, u.device, 1):
-        _lib.check(L.vmb_selective_scan_fwd(C.byref(a), _stream(u)), "selective_scan_fwd")
+    _run("vmb_selective_scan_fwd", u, "scan_fwd", a, nbytes=nbytes)
     return out, ckpt
 
 
@@ -162,31 +180,24 @@ def selective_scan_bwd(u, delta, A, B, C_, D, delta_bias, dout, ckpt, delta_soft
     dD = (torch.zeros_like(D) if zeroed is None else zeroed[1]) if D is not None else None
     dbias = (torch.zeros_like(delta_bias) if zeroed is None else zeroed[2]) if delta_bias is not None else None
     a = _lib.ScanBwdArgs(
-        _ptr(u), _ptr(delta), _ptr(A), _ptr(B), _ptr(C_), _ptr(D), _ptr(delta_bias), _ptr(dout), _ptr(ckpt),
-        _ptr(du), _ptr(ddelta), _ptr(dA), _ptr(dB), _ptr(dC), _ptr(dD), _ptr(dbias), None,
-        b, d, l, n, g,
-        u.stride(0), u.stride(1), delta.stride(0), delta.stride(1), dout.stride(0), dout.stride(1),
-        du.stride(0), du.stride(1), ddelta.stride(0), ddelta.stride(1),
-        B.stride(0), B.stride(1), B.stride(2), C_.stride(0), C_.stride(1), C_.stride(2),
-        int(bool(delta_softplus)), _DT[u.dtype], int(dout_f32), int(det))
+        u=_ptr(u), delta=_ptr(delta), A=_ptr(A), Bm=_ptr(B), Cm=_ptr(C_), D=_ptr(D), delta_bias=_ptr(delta_bias), dout=_ptr(dout),
+        ckpt=_ptr(ckpt), du=_ptr(du), ddelta=_ptr(ddelta), dA=_ptr(dA), dB=_ptr(dB), dC=_ptr(dC), dD=_ptr(dD), ddelta_bias=_ptr(dbias),
+        batch=b, dim=d, seqlen=l, dstate=n, ngroups=g,
+        u_bs=u.stride(0), u_ds=u.stride(1), delta_bs=delta.stride(0), delta_ds=delta.stride(1), dout_bs=dout.stride(0),
+        dout_ds=dout.stride(1), du_bs=du.stride(0), du_ds=du.stride(1), ddelta_bs=ddelta.stride(0), ddelta_ds=ddelta.stride(1),
+        B_bs=B.stride(0), B_gs=B.stride(1), B_ns=B.stride(2), C_bs=C_.stride(0), C_gs=C_.stride(1), C_ns=C_.stride(2),
+        delta_softplus=int(bool(delta_softplus)), dtype=_DT[u.dtype], dout_f32=int(dout_f32), deterministic=int(det))
     with torch.cuda.device(u.device):
         nws = L.vmb_scan_bwd_det_workspace_bytes(C.byref(a)) if det else L.vmb_scan_bwd_workspace_bytes(b, g, n, l)
     ws = _workspace(nws, workspace, u.device, "selective_scan_bwd")
     a.workspace = ws.data_ptr()
     es = u.element_size()
     nbytes = es * (4 * b * d * l + 4 * b * g * n * l) + dout.element_size() * b * d * l + 4 * b * d * ((l + 63) // 64) * n
-    with torch.cuda.device(u.device), _timed("scan_bwd_det" if det else "scan_bwd", nbytes, u.device, 2):
-        _lib.check(L.vmb_selective_scan_bwd(C.byref(a), _stream(u)), "selective_scan_bwd")
+    _run("vmb_selective_scan_bwd", u, "scan_bwd_det" if det else "scan_bwd", a, nbytes=nbytes, kernels=2)
     return du, ddelta, dA, dB, dC, dD, dbias
 
 
 # ----------------------------------------------------------------------------- fused OSS-block stages
-def _run(name, args, t, tag, nbytes=0, kernels=1):
-    fn = getattr(_lib.lib(), name)
-    with torch.cuda.device(t.device), _timed(tag, nbytes, t.device, kernels):
-        _lib.check(fn(C.byref(args), _stream(t)), name)
-
-
 def pixlin(x, w, bias=None, residual=None, ln=None, gate=None, gate_mode=0, act=(0, 0), out_dtype=None, out=None):
     """out[b,m,p] = epi(sum_k w[m,k] pro(x)[b,k,p]).  x: (B,K,P) view with stride(-1)==1; w: (M,>=K) x.dtype, rows may be
     zero-padded to a multiple of 16 (pad_weight) for vector loads.
@@ -199,12 +210,12 @@ def pixlin(x, w, bias=None, residual=None, ln=None, gate=None, gate_mode=0, act=
         out = torch.empty((B, M, P), dtype=out_dtype, device=x.device)
     ln_mode, ln_w, ln_b = ln if ln is not None else (0, None, None)
     a = _lib.PixlinArgs(
-        _ptr(x), _ptr(w), _ptr(bias), _ptr(residual), _ptr(out), _ptr(ln_w), _ptr(ln_b), _ptr(gate),
-        ln_mode, gate_mode if gate is not None else 0, act[0], act[1], B, K, M, P,
-        x.stride(0), x.stride(1), residual.stride(0) if residual is not None else 0,
-        residual.stride(1) if residual is not None else 0, out.stride(0), out.stride(1),
-        gate.stride(0) if gate is not None else 0, w.stride(0), _DT[x.dtype], _DT[out_dtype])
-    _run("vmb_pixlin", a, x, "pixlin", 0)
+        x=_ptr(x), w=_ptr(w), bias=_ptr(bias), residual=_ptr(residual), out=_ptr(out), ln_w=_ptr(ln_w), ln_b=_ptr(ln_b),
+        gate=_ptr(gate), ln_mode=ln_mode, gate_mode=gate_mode if gate is not None else 0, act_from=act[0], act_to=act[1],
+        batch=B, K=K, M=M, P=P, x_bs=x.stride(0), x_cs=x.stride(1), r_bs=residual.stride(0) if residual is not None else 0,
+        r_cs=residual.stride(1) if residual is not None else 0, o_bs=out.stride(0), o_cs=out.stride(1),
+        g_bs=gate.stride(0) if gate is not None else 0, w_ld=w.stride(0), dtype=_DT[x.dtype], out_dtype=_DT[out_dtype])
+    _run("vmb_pixlin", x, "pixlin", a)
     return out
 
 
@@ -225,10 +236,13 @@ def dwconv3x3(x, w9, bias, c_out, H, W, mode, out=None):
     B = x.shape[0]
     if out is None:
         out = torch.empty((B, c_out, H * W), dtype=x.dtype, device=x.device)
-    a = _lib.DwconvArgs(_ptr(x), _ptr(w9), _ptr(bias), _ptr(out), B, c_out, H, W, mode,
-                        x.stride(0), x.stride(1), out.stride(0), out.stride(1), _DT[x.dtype])
-    _run("vmb_dwconv3x3", a, x, "dwconv")
+    _run("vmb_dwconv3x3", x, "dwconv", _dwconv_args(x, w9, bias, out, c_out, H, W, mode))
     return out
+
+
+def _dwconv_args(x, w9, bias, out, c_out, H, W, mode):
+    return _lib.DwconvArgs(x=_ptr(x), w=_ptr(w9), bias=_ptr(bias), out=_ptr(out), batch=x.shape[0], c_out=c_out, H=H, W=W, mode=mode,
+                           x_bs=x.stride(0), x_cs=x.stride(1), o_bs=out.stride(0), o_cs=out.stride(1), dtype=_DT[x.dtype])
 
 
 def dwconv3x3_t(x, w9, bias, c_out, H, W):
@@ -236,11 +250,7 @@ def dwconv3x3_t(x, w9, bias, c_out, H, W):
     B = x.shape[0]
     out = torch.empty((B, c_out, H * W), dtype=x.dtype, device=x.device)
     out_t = torch.empty_like(out)
-    a = _lib.DwconvArgs(_ptr(x), _ptr(w9), _ptr(bias), _ptr(out), B, c_out, H, W, 0,
-                        x.stride(0), x.stride(1), out.stride(0), out.stride(1), _DT[x.dtype])
-    fn = _lib.lib().vmb_dwconv3x3_t
-    with torch.cuda.device(x.device), _timed("dwconv", 0, x.device, 1):
-        _lib.check(fn(C.byref(a), _ptr(out_t), _stream(x)), "vmb_dwconv3x3_t")
+    _run("vmb_dwconv3x3_t", x, "dwconv", _dwconv_args(x, w9, bias, out, c_out, H, W, 0), _ptr(out_t))
     return out, out_t
 
 
@@ -252,12 +262,16 @@ def cross_scan(srcs, rows, H, W, out=None):
     if out is None:
         out = torch.empty((B, 4, rows, H * W), dtype=s0.dtype, device=s0.device)
     assert out.shape == (B, 4, rows, H * W) and out.stride(3) == 1 and out.stride(2) == H * W and out.dtype == s0.dtype
-    arr = (C.c_void_p * 4)(*[t.data_ptr() for t in srcs])
     for t in srcs:
         assert t.stride() == s0.stride() and t.stride(2) == 1
-    a = _lib.CrossScanArgs(arr, _ptr(out), B, rows, H, W, s0.stride(0), s0.stride(1), out.stride(0), _DT[s0.dtype], out.stride(1))
-    _run("vmb_cross_scan", a, s0, "cross_scan")
+    _run("vmb_cross_scan", s0, "cross_scan", _cross_scan_args(srcs, out, rows, H, W))
     return out
+
+
+def _cross_scan_args(srcs, out, rows, H, W):
+    s0 = srcs[0]
+    return _lib.CrossScanArgs(src=_ptr4(srcs), out=_ptr(out), batch=s0.shape[0], rows=rows, H=H, W=W, src_bs=s0.stride(0),
+                              src_rs=s0.stride(1), out_bs=out.stride(0), dtype=_DT[s0.dtype], out_ks=out.stride(1))
 
 
 def pixel_shuffle2_nhwc(x, bias=None):
@@ -266,14 +280,12 @@ def pixel_shuffle2_nhwc(x, bias=None):
     B, C4, H, W = x.shape
     assert C4 % 4 == 0 and x.is_contiguous(memory_format=torch.channels_last)
     out = torch.empty((B, C4 // 4, 2 * H, 2 * W), dtype=x.dtype, device=x.device, memory_format=torch.channels_last)
-    a = _lib.PixelShuffleArgs(_ptr(x), _ptr(out), B, H, W, C4 // 4, _DT[x.dtype])
+    a = _lib.PixelShuffleArgs(x=_ptr(x), out=_ptr(out), batch=B, H=H, W=W, C=C4 // 4, dtype=_DT[x.dtype])
     if bias is None:
-        _run("vmb_pixel_shuffle2_nhwc", a, x, "pixel_shuffle")
+        _run("vmb_pixel_shuffle2_nhwc", x, "pixel_shuffle", a)
     else:
         assert bias.dtype == torch.float32 and bias.numel() == C4 and bias.is_contiguous() and bias.device == x.device
-        fn = _lib.lib().vmb_pixel_shuffle2_nhwc_bias
-        with torch.cuda.device(x.device), _timed("pixel_shuffle", 0, x.device, 1):
-            _lib.check(fn(C.byref(a), _ptr(bias), _stream(x)), "vmb_pixel_shuffle2_nhwc_bias")
+        _run("vmb_pixel_shuffle2_nhwc_bias", x, "pixel_shuffle", a, _ptr(bias))
     return out
 
 
@@ -291,12 +303,9 @@ def cross_scan_multi(segs, H, W):
         assert out.shape == (B, 4, rows, H * W) and out.stride(3) == 1 and out.stride(2) == H * W and out.dtype == s00.dtype
         for t in srcs:
             assert t.stride() == s0.stride() and t.stride(2) == 1 and t.dtype == s00.dtype and t.shape[0] == B
-        arr[i] = _lib.CrossScanArgs((C.c_void_p * 4)(*[t.data_ptr() for t in srcs]), _ptr(out), B, rows, H, W, s0.stride(0),
-                                    s0.stride(1), out.stride(0), _DT[s0.dtype], out.stride(1))
+        arr[i] = _cross_scan_args(srcs, out, rows, H, W)
         outs.append(out)
-    fn = _lib.lib().vmb_cross_scan_multi
-    with torch.cuda.device(s00.device), _timed("cross_scan", 0, s00.device, 1):
-        _lib.check(fn(arr, len(segs), _stream(s00)), "vmb_cross_scan_multi")
+    _run("vmb_cross_scan_multi", s00, "cross_scan", arr, len(segs))
     return outs
 
 
@@ -336,10 +345,10 @@ def conv3x3(x, wp, bias, c_out, mode=CONV_PLAIN, out=None, add=None, add_scale=1
         assert add is not None and add.dtype == x.dtype and add.shape == (B, c_out, H // add_scale, W // add_scale)
         add = add.contiguous()
         add_bs, add_cs = add.stride(0), add.stride(1)
-    a = _lib.Conv3x3Args(_ptr(x), _ptr(wp), _ptr(bias), _ptr(out), _ptr(add) if mode == CONV_ADD_NEAREST else None,
-                         B, Cin, c_out, H, W, int(nhwc), mode, add_scale, x_bs, x_cs, out.stride(0), out.stride(1), add_bs, add_cs,
-                         _DT[x.dtype])
-    _run("vmb_conv3x3", a, x, "conv3x3")
+    a = _lib.Conv3x3Args(x=_ptr(x), w=_ptr(wp), bias=_ptr(bias), out=_ptr(out), add=_ptr(add) if mode == CONV_ADD_NEAREST else None,
+                         batch=B, Cin=Cin, Cout=c_out, H=H, W=W, in_nhwc=int(nhwc), mode=mode, add_scale=add_scale, x_bs=x_bs, x_cs=x_cs,
+                         o_bs=out.stride(0), o_cs=out.stride(1), add_bs=add_bs, add_cs=add_cs, dtype=_DT[x.dtype])
+    _run("vmb_conv3x3", x, "conv3x3", a)
     return out
 
 
@@ -347,8 +356,8 @@ def transpose_hw(x, H, W):
     """x: (B, C, H*W) contiguous -> (B, C, W*H) with every plane transposed."""
     assert x.is_contiguous()
     out = torch.empty_like(x)
-    a = _lib.TransposeArgs(_ptr(x), _ptr(out), x.shape[0] * x.shape[1], H, W, _DT[x.dtype])
-    _run("vmb_transpose_hw", a, x, "transpose")
+    a = _lib.TransposeArgs(x=_ptr(x), out=_ptr(out), planes=x.shape[0] * x.shape[1], H=H, W=W, dtype=_DT[x.dtype])
+    _run("vmb_transpose_hw", x, "transpose", a)
     return out
 
 
@@ -365,19 +374,18 @@ def selective_scan_fwd_grouped(us, deltas, Bs, Cs, revs, A, D, delta_bias, delta
     out = torch.empty((b, G, R, L), dtype=us[0].dtype, device=us[0].device)
     ck = ckpt_interval()
     ckpt = torch.empty((b, G * R, (L + ck - 1) // ck, N), dtype=torch.float32, device=us[0].device) if need_ckpt else None
-    arr = lambda lst: (C.c_void_p * 4)(*([t.data_ptr() for t in lst] + [0] * (4 - G)))
-    outs = [out[:, g] for g in range(G)]
     a = _lib.ScanGroupedArgs(
-        arr(us), arr(deltas), arr(Bs), arr(Cs), arr(outs), (C.c_int * 4)(*(list(map(int, revs)) + [0] * (4 - G))),
-        _ptr(A), _ptr(D), _ptr(delta_bias), b, G * R, L, N, G,
-        us[0].stride(0), us[0].stride(1), deltas[0].stride(0), deltas[0].stride(1), out.stride(0), out.stride(2),
-        Bs[0].stride(0), Bs[0].stride(1), Cs[0].stride(0), Cs[0].stride(1), int(bool(delta_softplus)), _DT[us[0].dtype], _ptr(ckpt))
+        u=_ptr4(us), delta=_ptr4(deltas), Bm=_ptr4(Bs), Cm=_ptr4(Cs), out=_ptr4([out[:, g] for g in range(G)]), rev=_rev4(revs),
+        A=_ptr(A), D=_ptr(D), delta_bias=_ptr(delta_bias), batch=b, dim=G * R, seqlen=L, dstate=N, ngroups=G,
+        u_bs=us[0].stride(0), u_ds=us[0].stride(1), delta_bs=deltas[0].stride(0), delta_ds=deltas[0].stride(1),
+        out_bs=out.stride(0), out_ds=out.stride(2), B_bs=Bs[0].stride(0), B_ns=Bs[0].stride(1), C_bs=Cs[0].stride(0),
+        C_ns=Cs[0].stride(1), delta_softplus=int(bool(delta_softplus)), dtype=_DT[us[0].dtype], ckpt=_ptr(ckpt))
     es = us[0].element_size()
     n_u = len({t.data_ptr() for t in us})  # forward and reversed directions share one source tensor: counted once
     nbytes = es * b * L * (n_u * R + G * R + G * R + 2 * G * N) + 4 * (G * R * N + 2 * G * R)  # every unique operand / result once
     if ckpt is not None:
         nbytes += 4 * ckpt.numel()
-    _run("vmb_selective_scan_fwd_grouped", a, us[0], "scan_fwd", nbytes)
+    _run("vmb_selective_scan_fwd_grouped", us[0], "scan_fwd", a, nbytes=nbytes)
     return (out, ckpt) if need_ckpt else out
 
 
@@ -411,16 +419,15 @@ def selective_scan_bwd_grouped(us, deltas, Bs, Cs, douts, revs, A, D, delta_bias
     dA = torch.zeros_like(A) if zeroed is None else zeroed[0]
     dD = (torch.zeros_like(D) if zeroed is None else zeroed[1]) if D is not None else None
     dbias = (torch.zeros_like(delta_bias) if zeroed is None else zeroed[2]) if delta_bias is not None else None
-    arr = lambda lst: (C.c_void_p * 4)(*([t.data_ptr() for t in lst] + [0] * (4 - G)))
     a = _lib.ScanGroupedBwdArgs(
-        arr(us), arr(deltas), arr(Bs), arr(Cs), arr(douts), arr(dus), arr(dds), arr(dBs), arr(dCs),
-        (C.c_int * 4)(*(list(map(int, revs)) + [0] * (4 - G))),
-        _ptr(A), _ptr(D), _ptr(delta_bias), _ptr(ckpt), _ptr(dA), _ptr(dD), _ptr(dbias), None,
-        b, G * R, L, N, G,
-        us[0].stride(0), us[0].stride(1), deltas[0].stride(0), deltas[0].stride(1), douts[0].stride(0), douts[0].stride(1),
-        dus[0].stride(0), dus[0].stride(1), dds[0].stride(0), dds[0].stride(1),
-        Bs[0].stride(0), Bs[0].stride(1), Cs[0].stride(0), Cs[0].stride(1),
-        dBs[0].stride(0), dBs[0].stride(1), dCs[0].stride(0), dCs[0].stride(1), int(bool(delta_softplus)), _DT[dt], int(det))
+        u=_ptr4(us), delta=_ptr4(deltas), Bm=_ptr4(Bs), Cm=_ptr4(Cs), dout=_ptr4(douts), du=_ptr4(dus), ddelta=_ptr4(dds),
+        dB=_ptr4(dBs), dC=_ptr4(dCs), rev=_rev4(revs), A=_ptr(A), D=_ptr(D), delta_bias=_ptr(delta_bias), ckpt=_ptr(ckpt),
+        dA=_ptr(dA), dD=_ptr(dD), ddelta_bias=_ptr(dbias), batch=b, dim=G * R, seqlen=L, dstate=N, ngroups=G,
+        u_bs=us[0].stride(0), u_ds=us[0].stride(1), delta_bs=deltas[0].stride(0), delta_ds=deltas[0].stride(1),
+        dout_bs=douts[0].stride(0), dout_ds=douts[0].stride(1), du_bs=dus[0].stride(0), du_ds=dus[0].stride(1),
+        ddelta_bs=dds[0].stride(0), ddelta_ds=dds[0].stride(1), B_bs=Bs[0].stride(0), B_ns=Bs[0].stride(1),
+        C_bs=Cs[0].stride(0), C_ns=Cs[0].stride(1), dB_bs=dBs[0].stride(0), dB_ns=dBs[0].stride(1), dC_bs=dCs[0].stride(0),
+        dC_ns=dCs[0].stride(1), delta_softplus=int(bool(delta_softplus)), dtype=_DT[dt], deterministic=int(det))
     with torch.cuda.device(dev):
         nws = Lb.vmb_scan_grouped_bwd_det_workspace_bytes(C.byref(a)) if det else Lb.vmb_scan_bwd_workspace_bytes(b, G, N, L)
     ws = _workspace(nws, workspace, dev, "selective_scan_bwd_grouped")
@@ -428,8 +435,7 @@ def selective_scan_bwd_grouped(us, deltas, Bs, Cs, douts, revs, A, D, delta_bias
     es = us[0].element_size()
     uniq = lambda lst: len({t.data_ptr() for t in lst})  # directions that share a source tensor read it once
     nbytes = es * b * L * (R * (uniq(us) + G + uniq(douts) + 2 * G) + 4 * G * N) + (4 * ckpt.numel() if ckpt is not None else 0)
-    with torch.cuda.device(dev), _timed("scan_bwd_det" if det else "scan_bwd", nbytes, dev, 2):
-        _lib.check(Lb.vmb_selective_scan_bwd_grouped(C.byref(a), _stream(us[0])), "selective_scan_bwd_grouped")
+    _run("vmb_selective_scan_bwd_grouped", us[0], "scan_bwd_det" if det else "scan_bwd", a, nbytes=nbytes, kernels=2)
     return dus, dds, dA, dBs, dCs, dD, dbias
 
 
@@ -456,8 +462,9 @@ def _csc_args(x, xw, xb, dtw, dtb, A_logs, Ds, y, delta_softplus):
             continue
         if t.dtype != torch.float32 or not t.is_contiguous() or t.device != x.device or tuple(t.shape) != shp:
             raise RuntimeError(f"cross_selective_scan_c: {n} must be a contiguous float32 tensor of shape {shp} on x's device")
-    return _lib.CrossScanCArgs(_ptr(x), _ptr(xw), _ptr(xb), _ptr(dtw), _ptr(dtb), _ptr(A_logs), _ptr(Ds), _ptr(y),
-                               b, D, L, R, N, x.stride(0), x.stride(1), int(bool(delta_softplus)), _DT[x.dtype])
+    return _lib.CrossScanCArgs(x=_ptr(x), x_proj_weight=_ptr(xw), x_proj_bias=_ptr(xb), dt_projs_weight=_ptr(dtw),
+                               dt_projs_bias=_ptr(dtb), A_logs=_ptr(A_logs), Ds=_ptr(Ds), y=_ptr(y), batch=b, D=D, L=L, R=R, N=N,
+                               x_bs=x.stride(0), x_ds=x.stride(1), delta_softplus=int(bool(delta_softplus)), dtype=_DT[x.dtype])
 
 
 def cross_selective_scan_c_fwd(x, x_proj_weight, x_proj_bias, dt_projs_weight, dt_projs_bias, A_logs, Ds, delta_softplus=True):
@@ -467,7 +474,7 @@ def cross_selective_scan_c_fwd(x, x_proj_weight, x_proj_bias, dt_projs_weight, d
     b, D, L = x.shape
     y = torch.empty((b, L, D), dtype=torch.float32, device=x.device)
     a = _csc_args(x, x_proj_weight, x_proj_bias, dt_projs_weight, dt_projs_bias, A_logs, Ds, y, delta_softplus)
-    _run("vmb_cross_selective_scan_c_fwd", a, x, "cscan_c_fwd")
+    _run("vmb_cross_selective_scan_c_fwd", x, "cscan_c_fwd", a)
     return y
 
 
@@ -485,9 +492,10 @@ def cross_selective_scan_c_bwd(x, x_proj_weight, x_proj_bias, dt_projs_weight, d
              ("A_logs", (2 * D, N)), ("Ds", (2 * D,))]
     flat = torch.empty(sum(math.prod(s) for _, s in sizes), dtype=torch.float32, device=x.device)
     ws = torch.empty(_lib.lib().vmb_cross_selective_scan_c_workspace_bytes(b, D, R, N) // 4, dtype=torch.float32, device=x.device)
-    a = _lib.CrossScanCBwdArgs(_csc_args(x, x_proj_weight, x_proj_bias, dt_projs_weight, dt_projs_bias, A_logs, Ds, None, delta_softplus),
-                               _ptr(dy), _ptr(dx), _ptr(flat), _ptr(ws))
-    _run("vmb_cross_selective_scan_c_bwd", a, x, "cscan_c_bwd", 0, 2)
+    a = _lib.CrossScanCBwdArgs(
+        fwd=_csc_args(x, x_proj_weight, x_proj_bias, dt_projs_weight, dt_projs_bias, A_logs, Ds, None, delta_softplus),
+        dy=_ptr(dy), dx=_ptr(dx), d_params=_ptr(flat), workspace=_ptr(ws))
+    _run("vmb_cross_selective_scan_c_bwd", x, "cscan_c_bwd", a, kernels=2)
     grads, o = {}, 0
     for n, s in sizes:
         k = math.prod(s)
@@ -507,10 +515,8 @@ def merge_sum(ys, C_, H, W, in_place_order=False, out=None):
         out = torch.empty((B, C_, H * W), dtype=torch.float32, device=ys.device)
     assert out.dtype == torch.float32 and out.is_contiguous()
     ws = torch.empty(_lib.lib().vmb_merge_workspace_bytes(B, C_, H, W), dtype=torch.uint8, device=ys.device)
-    a = _lib.MergeArgs(_ptr(ys), None, None, None, None, None, B, C_, H, W, 0, 0, _DT[ys.dtype], _ptr(ws), int(in_place_order), 0, 0)
-    fn = _lib.lib().vmb_merge_sum
-    with torch.cuda.device(ys.device), _timed("merge", ys.element_size() * ys.numel() + 4 * out.numel(), ys.device, 1):
-        _lib.check(fn(C.byref(a), _ptr(out), _stream(ys)), "vmb_merge_sum")
+    a = _lib.MergeArgs(ys=_ptr(ys), batch=B, C=C_, H=H, W=W, dtype=_DT[ys.dtype], workspace=_ptr(ws), in_place_order=int(in_place_order))
+    _run("vmb_merge_sum", ys, "merge", a, _ptr(out), nbytes=ys.element_size() * ys.numel() + 4 * out.numel())
     return out
 
 
@@ -523,19 +529,24 @@ def merge_norm_gate(ys, z, ln_w, ln_b, C_, H, W, in_place_order=False, z_preact=
     y2 = torch.empty((B, C_, H * W), dtype=ys.dtype, device=ys.device)
     pooled = torch.empty((B, C_), dtype=torch.float32, device=ys.device)
     ws = torch.empty(_lib.lib().vmb_merge_workspace_bytes(B, C_, H, W), dtype=torch.uint8, device=ys.device)
-    a = _lib.MergeArgs(_ptr(ys), _ptr(z), _ptr(ln_w), _ptr(ln_b), _ptr(y2), _ptr(pooled), B, C_, H, W,
-                       z.stride(0), z.stride(1), _DT[ys.dtype], _ptr(ws), int(in_place_order), int(z_preact), int(return_ws))
-    _run("vmb_merge_norm_gate", a, ys, "merge", 0, 2)
+    a = _lib.MergeArgs(ys=_ptr(ys), z=_ptr(z), ln_w=_ptr(ln_w), ln_b=_ptr(ln_b), y2=_ptr(y2), pooled=_ptr(pooled), batch=B, C=C_, H=H,
+                       W=W, z_bs=z.stride(0), z_cs=z.stride(1), dtype=_DT[ys.dtype], workspace=_ptr(ws),
+                       in_place_order=int(in_place_order), z_preact=int(z_preact), save_ws=int(return_ws))
+    _run("vmb_merge_norm_gate", ys, "merge", a, kernels=2)
     return (y2, pooled, ws) if return_ws else (y2, pooled)
+
+
+def _channel_args(pooled, inv_count, prm, C_, c_out):
+    return _lib.ChannelArgs(pooled=_ptr(pooled), inv_count=inv_count, cin_w=_ptr(prm["cin_w"]), cin_b=_ptr(prm["cin_b"]),
+                            xc_proj=_ptr(prm["xc_proj"]), dtc_w=_ptr(prm["dtc_w"]), dtc_b=_ptr(prm["dtc_b"]), Ac_logs=_ptr(prm["Ac_logs"]),
+                            Dsc=_ptr(prm["Dsc"]), cout_w=_ptr(prm["cout_w"]), cout_b=_ptr(prm["cout_b"]), cn_w=_ptr(prm["cn_w"]),
+                            cn_b=_ptr(prm["cn_b"]), c_out=_ptr(c_out), batch=pooled.shape[0], C=C_, dc=prm["dc"], Rc=prm["Rc"], N=prm["N"])
 
 
 def channel_branch(pooled, inv_count, prm, C_):
     B = pooled.shape[0]
     c = torch.empty((B, C_), dtype=torch.float32, device=pooled.device)
-    a = _lib.ChannelArgs(_ptr(pooled), inv_count, _ptr(prm["cin_w"]), _ptr(prm["cin_b"]), _ptr(prm["xc_proj"]),
-                         _ptr(prm["dtc_w"]), _ptr(prm["dtc_b"]), _ptr(prm["Ac_logs"]), _ptr(prm["Dsc"]), _ptr(prm["cout_w"]),
-                         _ptr(prm["cout_b"]), _ptr(prm["cn_w"]), _ptr(prm["cn_b"]), _ptr(c), B, C_, prm["dc"], prm["Rc"], prm["N"])
-    _run("vmb_channel_branch", a, pooled, "channel")
+    _run("vmb_channel_branch", pooled, "channel", _channel_args(pooled, inv_count, prm, C_, c))
     return c
 
 
@@ -545,9 +556,9 @@ def layernorm_fwd(x, mode, w, b):
     B, C_, L = x.shape
     assert x.stride(2) == 1
     y = torch.empty((B, C_, L), dtype=x.dtype, device=x.device)
-    a = _lib.LnFwdArgs(_ptr(x), _ptr(w), _ptr(b), _ptr(y), None, B, C_, L, mode, x.stride(0), x.stride(1), y.stride(0), y.stride(1),
-                       _DT[x.dtype])
-    _run("vmb_layernorm_fwd", a, x, "ln_fwd")
+    a = _lib.LnFwdArgs(x=_ptr(x), w=_ptr(w), b=_ptr(b), y=_ptr(y), batch=B, C=C_, L=L, mode=mode, x_bs=x.stride(0), x_cs=x.stride(1),
+                       y_bs=y.stride(0), y_cs=y.stride(1), dtype=_DT[x.dtype])
+    _run("vmb_layernorm_fwd", x, "ln_fwd", a)
     return y
 
 
@@ -567,11 +578,11 @@ def layernorm_bwd(x, g, mode, w, add=None, need_param_grads=True, zeroed=None, p
         elif need_param_grads:
             dw = torch.zeros(C_, dtype=torch.float32, device=x.device)
             db = torch.zeros(C_, dtype=torch.float32, device=x.device) if mode == 1 else None
-    a = _lib.LnBwdArgs(_ptr(x), _ptr(g), _ptr(add), _ptr(w), _ptr(dx), _ptr(dw), _ptr(db), _ptr(stats), B, C_, L, mode,
-                       x.stride(0), x.stride(1), g.stride(0), g.stride(1), add.stride(0) if add is not None else 0,
-                       add.stride(1) if add is not None else 0, dx.stride(0) if dx is not None else 0, dx.stride(1) if dx is not None else 0,
-                       _DT[x.dtype])
-    _run("vmb_layernorm_bwd", a, x, "ln_bwd", 0, (1 if dx is not None else 0) + (1 if dw is not None else 0))
+    a = _lib.LnBwdArgs(x=_ptr(x), g=_ptr(g), add=_ptr(add), w=_ptr(w), dx=_ptr(dx), dw=_ptr(dw), db=_ptr(db), stats=_ptr(stats),
+                       batch=B, C=C_, L=L, mode=mode, x_bs=x.stride(0), x_cs=x.stride(1), g_bs=g.stride(0), g_cs=g.stride(1),
+                       a_bs=add.stride(0) if add is not None else 0, a_cs=add.stride(1) if add is not None else 0,
+                       dx_bs=dx.stride(0) if dx is not None else 0, dx_cs=dx.stride(1) if dx is not None else 0, dtype=_DT[x.dtype])
+    _run("vmb_layernorm_bwd", x, "ln_bwd", a, kernels=(1 if dx is not None else 0) + (1 if dw is not None else 0))
     if phase == "data":
         return dx, stats
     if phase == "params":
@@ -593,10 +604,11 @@ def merge_norm_gate_bwd(ws, z, dy2, dpooled, ln_w, ln_b, C_, L, dz_out, zeroed=N
     if phase != "data":
         dw = torch.zeros(C_, dtype=torch.float32, device=dy2.device) if zeroed is None else zeroed[0]
         db = torch.zeros(C_, dtype=torch.float32, device=dy2.device) if zeroed is None else zeroed[1]
-    a = _lib.MergeBwdArgs(_ptr(merged), _ptr(stats), _ptr(z), _ptr(dy2), _ptr(dpooled), _ptr(ln_w), _ptr(ln_b), _ptr(dm), _ptr(dz),
-                          _ptr(dw), _ptr(db), B, C_, L, z.stride(0), z.stride(1), dz.stride(0) if dz is not None else 0,
-                          dz.stride(1) if dz is not None else 0, _DT[dy2.dtype])
-    _run("vmb_merge_norm_gate_bwd", a, dy2, "merge_bwd", 0, (1 if dm is not None else 0) + (1 if dw is not None else 0))
+    a = _lib.MergeBwdArgs(merged=_ptr(merged), stats=_ptr(stats), z=_ptr(z), dy2=_ptr(dy2), dpooled=_ptr(dpooled), w=_ptr(ln_w),
+                          b=_ptr(ln_b), dm=_ptr(dm), dz=_ptr(dz), dw=_ptr(dw), db=_ptr(db), batch=B, C=C_, L=L, z_bs=z.stride(0),
+                          z_cs=z.stride(1), dz_bs=dz.stride(0) if dz is not None else 0, dz_cs=dz.stride(1) if dz is not None else 0,
+                          dtype=_DT[dy2.dtype])
+    _run("vmb_merge_norm_gate_bwd", dy2, "merge_bwd", a, kernels=(1 if dm is not None else 0) + (1 if dw is not None else 0))
     if phase == "data":
         return dm
     if phase == "params":
@@ -621,10 +633,11 @@ def dwconv3x3_bwd(x, w9, bias, g, c_out, H, W, mode, zeroed=None, phase="both", 
     if phase != "data":
         dw = torch.zeros((ch, 9), dtype=torch.float32, device=x.device) if zeroed is None else zeroed[0]
         dbias = (torch.zeros(ch, dtype=torch.float32, device=x.device) if zeroed is None else zeroed[1]) if bias is not None else None
-    a = _lib.DwconvBwdArgs(_ptr(x), _ptr(w9), _ptr(bias), _ptr(g), _ptr(dv), _ptr(dw), _ptr(dbias), B, c_out, H, W, mode,
-                           x.stride(0), x.stride(1), g.stride(0) if g is not None else 0, g.stride(1) if g is not None else 0,
-                           dv.stride(0), dv.stride(1), _DT[x.dtype])
-    _run("vmb_dwconv3x3_bwd", a, x, "dwconv_bwd", 0, (1 if g is not None else 0) + (1 if dw is not None else 0))
+    a = _lib.DwconvBwdArgs(x=_ptr(x), w=_ptr(w9), bias=_ptr(bias), g=_ptr(g), dv=_ptr(dv), dw=_ptr(dw), dbias=_ptr(dbias), batch=B,
+                           c_out=c_out, H=H, W=W, mode=mode, x_bs=x.stride(0), x_cs=x.stride(1),
+                           g_bs=g.stride(0) if g is not None else 0, g_cs=g.stride(1) if g is not None else 0,
+                           dv_bs=dv.stride(0), dv_cs=dv.stride(1), dtype=_DT[x.dtype])
+    _run("vmb_dwconv3x3_bwd", x, "dwconv_bwd", a, kernels=(1 if g is not None else 0) + (1 if dw is not None else 0))
     if phase == "data":
         return dv
     if phase == "params":
@@ -638,8 +651,9 @@ def channel_gate_bwd(dyg, y2, gate, mode):
     assert dyg.is_contiguous() and y2.is_contiguous() and gate.is_contiguous() and gate.dtype == torch.float32
     dy2 = torch.empty_like(y2)
     dg = torch.empty((B, C_), dtype=torch.float32, device=y2.device)
-    a = _lib.GateBwdArgs(_ptr(dyg), _ptr(y2), _ptr(gate), _ptr(dy2), _ptr(dg), B, C_, L, mode, _DT[y2.dtype])
-    _run("vmb_channel_gate_bwd", a, y2, "gate_bwd")
+    a = _lib.GateBwdArgs(dyg=_ptr(dyg), y2=_ptr(y2), gate=_ptr(gate), dy2=_ptr(dy2), dgate=_ptr(dg), batch=B, C=C_, L=L, mode=mode,
+                         dtype=_DT[y2.dtype])
+    _run("vmb_channel_gate_bwd", y2, "gate_bwd", a)
     return dy2, dg
 
 
@@ -668,26 +682,36 @@ def pixlin_wgrad(dy, x, per_batch=False, out=None, dbias=None, deterministic=Non
     if out is None:
         out = torch.zeros((B, M, K) if per_batch else (M, K), dtype=torch.float32, device=dy.device)
     det = _deterministic(deterministic)
-    a = _lib.WgradArgs(_ptr(dy), _ptr(x), _ptr(out), B, M, K, L, dy.stride(0), dy.stride(1), x.stride(0), x.stride(1),
-                       int(per_batch), _DT[dy.dtype], _ptr(dbias), None, int(det))
+    a = _lib.WgradArgs(dy=_ptr(dy), x=_ptr(x), out=_ptr(out), batch=B, M=M, K=K, L=L, dy_bs=dy.stride(0), dy_cs=dy.stride(1),
+                       x_bs=x.stride(0), x_cs=x.stride(1), per_batch=int(per_batch), dtype=_DT[dy.dtype], dbias=_ptr(dbias),
+                       deterministic=int(det))
     if not det:
-        _run("vmb_pixlin_wgrad", a, dy, "wgrad")
+        _run("vmb_pixlin_wgrad", dy, "wgrad", a)
         return out
     with torch.cuda.device(dy.device):
         ws = _workspace(_lib.lib().vmb_pixlin_wgrad_workspace_bytes(C.byref(a)), workspace, dy.device, "pixlin_wgrad")
     a.workspace = ws.data_ptr()
-    _run("vmb_pixlin_wgrad", a, dy, "wgrad_det", kernels=2)
+    _run("vmb_pixlin_wgrad", dy, "wgrad_det", a, kernels=2)
     return out
 
 
+# vmb_prep_job types (include/vmambair_b200.h, vmb_prep_block_weights): (M,K) -> (M,ld) converted, columns >= K zero;  (M,K) ->
+# (K,ld) transposed, columns >= M zero;  x_proj and dt_proj folded into one matrix and its transpose;  -exp(src);  taps flipped
+PREP_PAD_COPY, PREP_TRANSPOSE, PREP_FOLD, PREP_NEG_EXP, PREP_FLIP_TAPS = 0, 1, 2, 3, 4
+
+# one vmb_prep_job, tensors in place of its pointers.  type, src, dst, M and K are always given; src2, dst2, N2 and ld2 only for
+# PREP_FOLD, ld (the padded row length) only for the 16-bit outputs
+PrepJob = collections.namedtuple("PrepJob", "type src src2 dst dst2 M K N2 ld ld2", defaults=(None, None, None, 0, 0, 0, 0, 0))
+
+
 def prep_block_weights(jobs, dtype):
-    """jobs: list of (type, src, src2, dst, dst2, M, K, N2, ld, ld2) -- see vmb_prep_block_weights; one launch."""
-    a = _lib.PrepArgs()
-    a.njobs, a.dtype = len(jobs), _DT[dtype]
-    for i, (t, src, src2, dst, dst2, M, K, N2, ld, ld2) in enumerate(jobs):
-        a.jobs[i] = _lib.PrepJob(src.data_ptr(), src2.data_ptr() if src2 is not None else None, dst.data_ptr(),
-                                 dst2.data_ptr() if dst2 is not None else None, t, M, K, N2, ld, ld2)
-    _run("vmb_prep_block_weights", a, jobs[0][1], "prep")
+    """jobs: PrepJob or (type, src, src2, dst, dst2, M, K, N2, ld, ld2) tuples -- see vmb_prep_block_weights; one launch."""
+    jobs = [PrepJob._make(j) for j in jobs]
+    a = _lib.PrepArgs(njobs=len(jobs), dtype=_DT[dtype])
+    for i, j in enumerate(jobs):
+        a.jobs[i] = _lib.PrepJob(src=_ptr(j.src), src2=_ptr(j.src2), dst=_ptr(j.dst), dst2=_ptr(j.dst2), type=j.type, M=j.M, K=j.K,
+                                 N2=j.N2, ld=j.ld, ld2=j.ld2)
+    _run("vmb_prep_block_weights", jobs[0].src, "prep", a)
 
 
 def sum4_add(x4, add):
@@ -698,19 +722,8 @@ def sum4_add(x4, add):
     if add[0].numel() % (16 // add.element_size()) or x4.data_ptr() % 16 or add.data_ptr() % 16:
         return (add.float() + x4.float().sum(1)).to(add.dtype)
     out = torch.empty_like(add)
-    global _LAUNCHES
-    with torch.cuda.device(x4.device):
-        _lib.check(_lib.lib().vmb_sum4_add(x4.data_ptr(), add.data_ptr(), out.data_ptr(), B, add[0].numel(), _DT[x4.dtype],
-                                           torch.cuda.current_stream(x4.device).cuda_stream), "sum4_add")
-    _LAUNCHES += 1
+    _run("vmb_sum4_add", x4, None, _ptr(x4), _ptr(add), _ptr(out), B, add[0].numel(), _DT[x4.dtype])  # counted, not timed
     return out
-
-
-def _channel_args(pooled, inv_count, prm, C_, c_out):
-    B = pooled.shape[0]
-    return _lib.ChannelArgs(_ptr(pooled), inv_count, _ptr(prm["cin_w"]), _ptr(prm["cin_b"]), _ptr(prm["xc_proj"]),
-                            _ptr(prm["dtc_w"]), _ptr(prm["dtc_b"]), _ptr(prm["Ac_logs"]), _ptr(prm["Dsc"]), _ptr(prm["cout_w"]),
-                            _ptr(prm["cout_b"]), _ptr(prm["cn_w"]), _ptr(prm["cn_b"]), _ptr(c_out), B, C_, prm["dc"], prm["Rc"], prm["N"])
 
 
 def channel_branch_bwd_supported(C_, prm) -> bool:
@@ -742,10 +755,11 @@ def channel_branch_bwd(pooled, inv_count, prm, C_, dc_out, into=None):
     dpooled = torch.empty((B, C_), dtype=torch.float32, device=dev)
     scratch = torch.empty(_lib.lib().vmb_channel_branch_bwd_scratch_bytes(B, dc, C_) // 4, dtype=torch.float32, device=dev)
     dc_out = dc_out.float().contiguous()
-    a = _lib.ChannelBwdArgs(_channel_args(pooled, inv_count, prm, C_, None), _ptr(dc_out), _ptr(dpooled),
-                            _ptr(g["cin_w"]) if has_cin else None, _ptr(g["cin_b"]) if has_cin else None, _ptr(g["xc_proj"]),
-                            _ptr(g["dtc_w"]), _ptr(g["dtc_b"]), _ptr(g["Ac_logs"]), _ptr(g["Dsc"]),
-                            _ptr(g["cout_w"]) if has_cout else None, _ptr(g["cout_b"]) if has_cout else None, _ptr(g["cn_w"]),
-                            _ptr(g["cn_b"]), _ptr(scratch))
-    _run("vmb_channel_branch_bwd", a, pooled, "channel_bwd")
+    a = _lib.ChannelBwdArgs(fwd=_channel_args(pooled, inv_count, prm, C_, None), dc_out=_ptr(dc_out), d_pooled=_ptr(dpooled),
+                            d_cin_w=_ptr(g["cin_w"]) if has_cin else None, d_cin_b=_ptr(g["cin_b"]) if has_cin else None,
+                            d_xc_proj=_ptr(g["xc_proj"]), d_dtc_w=_ptr(g["dtc_w"]), d_dtc_b=_ptr(g["dtc_b"]), d_Ac_logs=_ptr(g["Ac_logs"]),
+                            d_Dsc=_ptr(g["Dsc"]), d_cout_w=_ptr(g["cout_w"]) if has_cout else None,
+                            d_cout_b=_ptr(g["cout_b"]) if has_cout else None, d_cn_w=_ptr(g["cn_w"]), d_cn_b=_ptr(g["cn_b"]),
+                            scratch=_ptr(scratch))
+    _run("vmb_channel_branch_bwd", pooled, "channel_bwd", a)
     return dpooled, g

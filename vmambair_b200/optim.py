@@ -56,10 +56,11 @@ class FlatAdam:
     def step(self, grad_scale: float = 1.0, zero_grad: bool = True):
         from . import fused_train
         fused_train.join_side_stream()  # normally already joined by the end-of-backward callback
-        a = _lib.AdamArgs(self.flat_param.data_ptr(), self.flat_grad.data_ptr(), self.exp_avg.data_ptr(), self.exp_avg_sq.data_ptr(),
-                          self.ema.data_ptr() if self.ema is not None else None, self.state.data_ptr(), self.n,
-                          self.lr, self.betas[0], self.betas[1], self.eps, self.weight_decay, int(self.decoupled),
-                          grad_scale, self.max_grad_norm, self.ema_decay, int(zero_grad))
+        a = _lib.AdamArgs(param=self.flat_param.data_ptr(), grad=self.flat_grad.data_ptr(), exp_avg=self.exp_avg.data_ptr(),
+                          exp_avg_sq=self.exp_avg_sq.data_ptr(), ema=self.ema.data_ptr() if self.ema is not None else None,
+                          state=self.state.data_ptr(), n=self.n, lr=self.lr, beta1=self.betas[0], beta2=self.betas[1], eps=self.eps,
+                          weight_decay=self.weight_decay, decoupled_weight_decay=int(self.decoupled), grad_scale=grad_scale,
+                          max_grad_norm=self.max_grad_norm, ema_decay=self.ema_decay, zero_grad=int(zero_grad))
         with torch.cuda.device(self.flat_param.device):
             st = C.c_void_p(torch.cuda.current_stream(self.flat_param.device).cuda_stream)
             _lib.check(_lib.lib().vmb_fused_adam(C.byref(a), st), "fused_adam")
