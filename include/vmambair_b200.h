@@ -47,8 +47,16 @@ int vmb_scan_ckpt_interval(void);
  * dt = softplus?(delta + delta_bias).  State and accumulation in fp32.
  *   out_f32       : 0 -> `out` has dtype `dt`;  1 (bf16 / fp16 `dt` only) -> `out` is fp32, the fp32 accumulator stored without
  *                   rounding: selective_scan_cuda_oflex.fwd(..., out_float=True) (cusoflex/selective_scan_oflex.cpp:157-243,
- *                   out allocated at :219, the <input_t, weight_t, float> kernel at :238).  Last member: a zero-initialised
- *                   struct keeps the plain operator. */
+ *                   out allocated at :219, the <input_t, weight_t, float> kernel at :238).  A zero-initialised tail (out_f32 and
+ *                   the members below) keeps the plain operator.
+ * The z gate and the last state of mamba_ssm's selective_scan_cuda.fwd(u, delta, A, B, C, D, z, delta_bias, delta_softplus)
+ * (its wrapper: Mamba/kernels/selective_scan/test_selective_scan.py:18-165; RealSR/VmambaIR/archs/MambaRealSR11_arch.py:294):
+ *   z, out_z      : (batch, dim, seqlen) dtype `dt`, last-dim stride 1, both given or both NULL.  out_z = out * z * sigmoid(z),
+ *                   from the fp32 accumulator, rounded once; `out` is still written, ungated.  Not with out_f32 (VMB_ERR_INVALID).
+ *   ckpt_pairs    : 1 -> ckpt is fp32 (batch, dim, n_ckpt, 2 dstate), 16 B aligned: ckpt[b,d,k,2n+1] = h_n after position
+ *                   min(interval (k+1), seqlen) - 1 and ckpt[b,d,k,2n] = 0, so ckpt[:, :, -1, 1::2] is the last state for every
+ *                   seqlen (the reference wrapper's `x[:, :, -1, 1::2]`, :79).  vmb_selective_scan_bwd reads the dense
+ *                   ckpt[..., 1::2] copy.  0 -> the layout above.  z with a ckpt buffer requires ckpt_pairs = 1. */
 typedef struct {
     const void* u; const void* delta; const float* A; const void* Bm; const void* Cm;
     const float* D; const float* delta_bias; void* out; float* ckpt;
@@ -61,8 +69,27 @@ typedef struct {
     int delta_softplus;
     int dtype; /* vmb_dtype of u, delta, Bm, Cm, out (out: fp32 when out_f32) */
     int out_f32;
+    const void* z; void* out_z;
+    int64_t z_bs, z_ds;         /* batch / dim strides of z       */
+    int64_t out_z_bs, out_z_ds; /* ... of out_z                   */
+    int ckpt_pairs;
 } vmb_scan_fwd_args;
 int vmb_selective_scan_fwd(const vmb_scan_fwd_args* a, void* stream);
+
+/* Backward of the z gate of vmb_selective_scan_fwd (mamba_ssm's selective_scan_cuda.bwd, which then runs the scan backward on
+ * dout_eff: here vmb_selective_scan_bwd with dout_f32 = 1, or plain for fp32).  Element-wise, fp32 math, s = sigmoid(z):
+ *   dout_eff = dout * z * s                      fp32 (batch, dim, seqlen) dense
+ *   dz       = dout * out * s * (1 + z (1 - s))  dtype `dt`, caller's buffer (strides dz_bs, dz_ds)
+ *   out_z    = out * z * s                       dtype `dt`, optional (NULL: not written; the reference's recompute_out_z)
+ * dout, out (the forward's ungated `out`), z: (batch, dim, seqlen) dtype `dt`.  Every tensor has last-dim stride 1. */
+typedef struct {
+    const void* dout; const void* out; const void* z;
+    float* dout_eff; void* dz; void* out_z;
+    int batch, dim, seqlen;
+    int64_t dout_bs, dout_ds, out_bs, out_ds, z_bs, z_ds, dz_bs, dz_ds, out_z_bs, out_z_ds;
+    int dtype;
+} vmb_scan_gate_args;
+int vmb_scan_gate_bwd(const vmb_scan_gate_args* a, void* stream);
 
 /* Direction-aware variant for the fused OSS path: group g (<= 4 groups, dim = ngroups * rows_per_group) reads its
  * rows from its own tensors and, when rev[g] != 0, walks them backwards (sequence position l <-> memory index

@@ -30,6 +30,17 @@ class ScanFwdArgs(C.Structure):
         ("u_bs", i64), ("u_ds", i64), ("delta_bs", i64), ("delta_ds", i64), ("out_bs", i64), ("out_ds", i64),
         ("B_bs", i64), ("B_gs", i64), ("B_ns", i64), ("C_bs", i64), ("C_gs", i64), ("C_ns", i64),
         ("delta_softplus", C.c_int), ("dtype", C.c_int), ("out_f32", C.c_int),
+        ("z", vp), ("out_z", vp), ("z_bs", i64), ("z_ds", i64), ("out_z_bs", i64), ("out_z_ds", i64), ("ckpt_pairs", C.c_int),
+    ]
+
+
+class ScanGateArgs(C.Structure):
+    _c_name_ = "vmb_scan_gate_args"
+    _fields_ = [
+        ("dout", vp), ("out", vp), ("z", vp), ("dout_eff", vp), ("dz", vp), ("out_z", vp),
+        ("batch", C.c_int), ("dim", C.c_int), ("seqlen", C.c_int),
+        ("dout_bs", i64), ("dout_ds", i64), ("out_bs", i64), ("out_ds", i64), ("z_bs", i64), ("z_ds", i64),
+        ("dz_bs", i64), ("dz_ds", i64), ("out_z_bs", i64), ("out_z_ds", i64), ("dtype", C.c_int),
     ]
 
 
@@ -233,6 +244,7 @@ SYMBOLS = {
     "vmb_scan_ckpt_interval": (C.c_int, []),
     "vmb_selective_scan_fwd": (C.c_int, [C.POINTER(ScanFwdArgs), vp]),
     "vmb_selective_scan_bwd": (C.c_int, [C.POINTER(ScanBwdArgs), vp]),
+    "vmb_scan_gate_bwd": (C.c_int, [C.POINTER(ScanGateArgs), vp]),
     "vmb_scan_bwd_workspace_bytes": (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int]),
     "vmb_scan_bwd_det_workspace_bytes": (C.c_int64, [C.POINTER(ScanBwdArgs)]),
     "vmb_pixlin": (C.c_int, [C.POINTER(PixlinArgs), vp]),

@@ -53,6 +53,11 @@ extern "C" int vmb_selective_scan_fwd(const vmb_scan_fwd_args* a, void* stream) 
     VMB_CHECK(a->batch <= 65535, "selective_scan_fwd: batch > 65535");
     VMB_CHECK(a->out_f32 == 0 || a->out_f32 == 1, "selective_scan_fwd: out_f32 must be 0 or 1 (got %d)", a->out_f32);
     VMB_CHECK(!a->out_f32 || a->dtype == VMB_BF16 || a->dtype == VMB_F16, "selective_scan_fwd: out_f32 needs bf16 / fp16 inputs");
+    VMB_CHECK((a->z == nullptr) == (a->out_z == nullptr), "selective_scan_fwd: z and out_z must both be given or both be NULL");
+    VMB_CHECK(!a->z || !a->out_f32, "selective_scan_fwd: the z gate has no fp32-output form (out_f32)");
+    VMB_CHECK(a->ckpt_pairs == 0 || a->ckpt_pairs == 1, "selective_scan_fwd: ckpt_pairs must be 0 or 1 (got %d)", a->ckpt_pairs);
+    VMB_CHECK(!a->z || !a->ckpt || a->ckpt_pairs, "selective_scan_fwd: with z, checkpoints are written in the pair layout (ckpt_pairs = 1)");
+    VMB_CHECK(!a->ckpt || !a->ckpt_pairs || aligned16(a->ckpt), "selective_scan_fwd: pair-layout checkpoints must be 16-byte aligned");
     ScanFwdParams p{};
     p.u = a->u; p.delta = a->delta; p.Bm = a->Bm; p.Cm = a->Cm; p.A = a->A; p.D = a->D; p.bias = a->delta_bias;
     p.out = a->out; p.ckpt = a->ckpt;
@@ -70,7 +75,30 @@ extern "C" int vmb_selective_scan_fwd(const vmb_scan_fwd_args* a, void* stream) 
                mult(a->u_bs) && mult(a->u_ds) && mult(a->delta_bs) && mult(a->delta_ds) && mult_o(a->out_bs) &&
                mult_o(a->out_ds) && mult(a->B_bs) && mult(a->B_gs) && mult(a->B_ns) && mult(a->C_bs) && mult(a->C_gs) &&
                mult(a->C_ns);
-    return scan_fwd_launch(p, a->dtype, static_cast<cudaStream_t>(stream), a->out_f32 != 0);
+    int ext = 0;
+    if (a->z) {
+        set_scan_gate(p, ScanGateDesc{a->z, a->out_z, a->z_bs, a->z_ds, a->out_z_bs, a->out_z_ds});
+        p.vec_ok = p.vec_ok && aligned16(a->z) && aligned16(a->out_z) && mult(a->z_bs) && mult(a->z_ds) && mult(a->out_z_bs) &&
+                   mult(a->out_z_ds);
+        ext |= kScanGate;
+    }
+    if (a->ckpt && a->ckpt_pairs) ext |= kScanPairCkpt;
+    return scan_fwd_launch(p, a->dtype, static_cast<cudaStream_t>(stream), a->out_f32 != 0, ext);
+}
+
+extern "C" int vmb_scan_gate_bwd(const vmb_scan_gate_args* a, void* stream) {
+    VMB_CHECK(a != nullptr, "scan_gate_bwd: null args");
+    VMB_CHECK(a->dtype == VMB_F32 || a->dtype == VMB_BF16 || a->dtype == VMB_F16, "scan_gate_bwd: dtype must be f32/bf16/f16 (got %d)",
+              a->dtype);
+    VMB_CHECK(a->dout && a->out && a->z && a->dout_eff && a->dz, "scan_gate_bwd: null tensor pointer");
+    VMB_CHECK(a->batch > 0 && a->dim > 0 && a->seqlen > 0 && (int64_t)a->batch * a->dim < (1LL << 31), "scan_gate_bwd: bad sizes");
+    const int v = 16 / elt_size(a->dtype);
+    auto mult = [v](int64_t s) { return s % v == 0; };
+    const bool vec_ok = aligned16(a->dout) && aligned16(a->out) && aligned16(a->z) && aligned16(a->dz) && aligned16(a->dout_eff) &&
+                        (!a->out_z || (aligned16(a->out_z) && mult(a->out_z_bs) && mult(a->out_z_ds))) && mult(a->dout_bs) &&
+                        mult(a->dout_ds) && mult(a->out_bs) && mult(a->out_ds) && mult(a->z_bs) && mult(a->z_ds) && mult(a->dz_bs) &&
+                        mult(a->dz_ds) && a->seqlen % 4 == 0;  // dout_eff: dense fp32 rows
+    return scan_gate_bwd_launch(*a, vec_ok, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int64_t vmb_scan_bwd_workspace_bytes(int batch, int ngroups, int dstate, int seqlen) {

@@ -116,6 +116,39 @@ __device__ __forceinline__ void convert_bc(float4* __restrict__ dst, const in_t*
         for (int i = 0; i < V / 2; ++i) d[i] = make_float4(f0[2 * i], f1[2 * i], f0[2 * i + 1], f1[2 * i + 1]);
     }
 }
+// z * sigmoid(z): the gate of the z-gated forward and of its backward (one expression, so a recomputed out_z equals the forward's
+// when `out` is fp32)
+__device__ __forceinline__ float silu_gate(float z) { return z / (1.f + __expf(-z)); }
 
+// out_z at positions [l0, l0+T) of row (b, d): y (the fp32 accumulator, already summed over state parts) * SiLU(z), rounded once
+template <typename in_t>
+__device__ __forceinline__ void store_gated(const ScanGateDesc& gt, int b, int d, int l0, const float* y, int valid, bool vec_ok) {
+    constexpr int V = Vec<in_t>::N;
+    const in_t* zr = reinterpret_cast<const in_t*>(gt.z) + (int64_t)b * gt.z_bs + (int64_t)d * gt.z_ds + l0;
+    in_t* ozr = reinterpret_cast<in_t*>(gt.out_z) + (int64_t)b * gt.oz_bs + (int64_t)d * gt.oz_ds + l0;
+#pragma unroll
+    for (int v = 0; v < T / V; ++v) {
+        float zv[V];
+        load_vec<in_t>(zr + v * V, zv, valid - v * V, vec_ok);
+#pragma unroll
+        for (int i = 0; i < V; ++i) zv[i] = y[v * V + i] * silu_gate(zv[i]);
+        store_vec<in_t>(ozr + v * V, zv, valid - v * V, vec_ok);
+    }
+}
+
+// pair-layout checkpoint (kScanPairCkpt): states n0, n0+1 after the last position of the lane's segment, written by the segment
+// that ends a 64-position interval or holds position L-1 (so row n_ckpt-1 is the last state for every L); row k, slots 2n / 2n+1 =
+// (0, h_n).  The base is 16 B aligned (vmb_selective_scan_fwd checks it), so with even N every pair is one 16 B store.
+__device__ __forceinline__ void store_ckpt_pair(const ScanFwdParams& p, int b, int d, int l0, int n0, float2 h) {
+    if (l0 >= p.L || ((l0 + T) % kScanCkpt != 0 && l0 + T < p.L)) return;
+    const int N = p.N;
+    float* ck = p.ckpt + (((int64_t)b * p.dim + d) * p.n_ckpt + (l0 + T - 1) / kScanCkpt) * (2 * N) + 2 * n0;
+    if ((N & 1) == 0 && n0 < N) {
+        *reinterpret_cast<float4*>(ck) = make_float4(0.f, h.x, 0.f, h.y);
+    } else {
+        if (n0 < N) { ck[0] = 0.f; ck[1] = h.x; }
+        if (n0 + 1 < N) { ck[2] = 0.f; ck[3] = h.y; }
+    }
+}
 
 }  // namespace vmb

@@ -120,6 +120,8 @@ __device__ __forceinline__ void stage_bc_cta(float4* __restrict__ dst, const in_
 // MODE 0: plain operator, no checkpoints (inference)   1: plain operator + checkpoints (training forward)
 //      2: direction-aware grouped sources (per-group bases, reversed walk), no checkpoints   3: 2 + checkpoints.
 // Each mode only compiles what it needs: the state loop sits at the 128-register limit.
+//      + kScanGate / kScanPairCkpt (scan_params.h) on MODE 0 / 1 with out_t = in_t: also out_z = out * SiLU(z); pair-layout
+//        checkpoints (selective_scan_cuda).
 // out_t: element type of `out` (float with 16-bit in_t, MODE 0 / 1 only: the fp32 accumulator stored without rounding).
 template <typename in_t, int RB, int WPC, int MODE, typename out_t>
 __global__ void __launch_bounds__(32 * WPC, 12 / WPC) scan_fwd_kernel(const ScanFwdParams p) {
@@ -130,6 +132,8 @@ __global__ void __launch_bounds__(32 * WPC, 12 / WPC) scan_fwd_kernel(const Scan
     constexpr int SEGW = Cfg::SEGW, CHUNK = Cfg::CHUNK, SEGQ = Cfg::SEGQ, SLOTS = Cfg::SLOTS;
     constexpr int V = Vec<in_t>::N, NT = 32 * WPC;
     constexpr int VO = Vec<out_t>::N;
+    constexpr int M = MODE & 3;  // base mode
+    constexpr bool GATE = (MODE & kScanGate) != 0, PAIR = (MODE & kScanPairCkpt) != 0;
 
     extern __shared__ float4 smem_f4[];
     float4* sB = smem_f4;                                                  // [8][SLOTS]   CTA-shared
@@ -149,12 +153,12 @@ __global__ void __launch_bounds__(32 * WPC, 12 / WPC) scan_fwd_kernel(const Scan
     const int g = d0 / p.rows_per_group;  // same for every warp of the CTA (RB*WPC divides the group)
     const int N = p.N, L = p.L, npad = p.npad;
     const bool async_ok = p.vec_ok;
-    constexpr bool HAS_REV = MODE >= 2;
+    constexpr bool HAS_REV = M >= 2;
 
     const in_t *Bg, *Cg, *ublk, *dblk;
     out_t* orow;
     bool rev = false;
-    if (MODE < 2) {
+    if (M < 2) {
         Bg = reinterpret_cast<const in_t*>(p.Bm) + (int64_t)b * p.B_bs + (int64_t)g * p.B_gs;
         Cg = reinterpret_cast<const in_t*>(p.Cm) + (int64_t)b * p.C_bs + (int64_t)g * p.C_gs;
         ublk = reinterpret_cast<const in_t*>(p.u) + (int64_t)b * p.u_bs + (int64_t)d0 * p.u_ds;
@@ -302,7 +306,9 @@ __global__ void __launch_bounds__(32 * WPC, 12 / WPC) scan_fwd_kernel(const Scan
                     h = fma2(a2[t + 1], h, mul2(make_float2(dtu[t + 1], dtu[t + 1]), make_float2(Bq.z, Bq.w)));
                     y[t + 1] = fmaf(h.y, Cq.w, fmaf(h.x, Cq.z, y[t + 1]));
                 }
-                if ((MODE == 1 || MODE == 3) && l0 < L && ((l0 + T) % kScanCkpt) == 0) {
+                if constexpr (PAIR) {
+                    store_ckpt_pair(p, b, d, l0, n0, h);
+                } else if ((M == 1 || M == 3) && l0 < L && ((l0 + T) % kScanCkpt) == 0) {
                     float* ck = p.ckpt + (((int64_t)b * p.dim + d) * p.n_ckpt + ((l0 + T) / kScanCkpt - 1)) * N + n0;
                     if (n0 < N) ck[0] = h.x;
                     if (n0 + 1 < N) ck[1] = h.y;
@@ -312,6 +318,7 @@ __global__ void __launch_bounds__(32 * WPC, 12 / WPC) scan_fwd_kernel(const Scan
         if (!HAS_REV || !rev) {
 #pragma unroll
             for (int v = 0; v < T / VO; ++v) store_vec<out_t>(orow + l0 + v * VO, y + v * VO, valid - v * VO, p.vec_ok);
+            if constexpr (GATE) store_gated<in_t>(scan_gate_desc(p), b, d, l0, y, valid, p.vec_ok);
         } else if (valid == T) {  // sequence l0+t -> memory L-1-l0-t: one reversed contiguous block
 #pragma unroll
             for (int v = 0; v < T / VO; ++v) {
@@ -343,7 +350,7 @@ static int launch_cfg2(const ScanFwdParams& p, cudaStream_t stream) {
 }
 
 template <typename in_t, int RB, int WPC, typename out_t>
-static int launch_cfg(const ScanFwdParams& p, cudaStream_t stream) {
+static int launch_cfg(const ScanFwdParams& p, int ext, cudaStream_t stream) {
     if constexpr (std::is_same<in_t, out_t>::value) {  // the grouped modes exist with the input's output type only
         if (p.ndesc) {
             if constexpr (RB <= 2) {
@@ -354,7 +361,17 @@ static int launch_cfg(const ScanFwdParams& p, cudaStream_t stream) {
         }
     }
     VMB_CHECK(p.ndesc == 0, "grouped scan: no fp32 output");
-    return p.ckpt ? launch_cfg2<in_t, RB, WPC, 1, out_t>(p, stream) : launch_cfg2<in_t, RB, WPC, 0, out_t>(p, stream);
+    if (ext == 0) return p.ckpt ? launch_cfg2<in_t, RB, WPC, 1, out_t>(p, stream) : launch_cfg2<in_t, RB, WPC, 0, out_t>(p, stream);
+    // gated / pair-checkpoint modes (input's output type only), instantiated after the plain ones so that those compile as before
+    if constexpr (std::is_same<in_t, out_t>::value) {
+        if (ext & kScanGate) {
+            return p.ckpt ? launch_cfg2<in_t, RB, WPC, 1 | kScanGate | kScanPairCkpt, out_t>(p, stream)
+                          : launch_cfg2<in_t, RB, WPC, kScanGate, out_t>(p, stream);
+        }
+        return launch_cfg2<in_t, RB, WPC, 1 | kScanPairCkpt, out_t>(p, stream);
+    }
+    set_error("selective_scan_fwd: no z gate / pair checkpoints with fp32 output");
+    return VMB_ERR_INVALID;
 }
 
 // (rows per warp RB, warps per CTA WPC): RB*WPC must divide the rows of a group.  Small RB = more warps and
@@ -378,42 +395,44 @@ static void pick_cfg(const ScanFwdParams& p, int& rb, int& wpc) {
 }
 
 template <typename in_t, int RB, typename out_t>
-static int launch_rb(const ScanFwdParams& p, int wpc, cudaStream_t stream) {
+static int launch_rb(const ScanFwdParams& p, int wpc, int ext, cudaStream_t stream) {
     switch (wpc) {
-        case 4: return launch_cfg<in_t, RB, 4, out_t>(p, stream);
-        case 2: return launch_cfg<in_t, RB, 2, out_t>(p, stream);
-        default: return launch_cfg<in_t, RB, 1, out_t>(p, stream);
+        case 4: return launch_cfg<in_t, RB, 4, out_t>(p, ext, stream);
+        case 2: return launch_cfg<in_t, RB, 2, out_t>(p, ext, stream);
+        default: return launch_cfg<in_t, RB, 1, out_t>(p, ext, stream);
     }
 }
 
 template <typename in_t, typename out_t = in_t>
-static int launch_t(const ScanFwdParams& p, cudaStream_t stream) {
+static int launch_t(const ScanFwdParams& p, int ext, cudaStream_t stream) {
     int rb, wpc;
     pick_cfg(p, rb, wpc);
     switch (rb) {
-        case 8: return launch_rb<in_t, 8, out_t>(p, wpc, stream);
-        case 4: return launch_rb<in_t, 4, out_t>(p, wpc, stream);
-        case 2: return launch_rb<in_t, 2, out_t>(p, wpc, stream);
-        default: return launch_rb<in_t, 1, out_t>(p, wpc, stream);
+        case 8: return launch_rb<in_t, 8, out_t>(p, wpc, ext, stream);
+        case 4: return launch_rb<in_t, 4, out_t>(p, wpc, ext, stream);
+        case 2: return launch_rb<in_t, 2, out_t>(p, wpc, ext, stream);
+        default: return launch_rb<in_t, 1, out_t>(p, wpc, ext, stream);
     }
 }
 
-int scan_fwd_launch(const ScanFwdParams& p, int dtype, cudaStream_t stream, bool out_f32) {
+int scan_fwd_launch(const ScanFwdParams& p, int dtype, cudaStream_t stream, bool out_f32, int ext) {
     VMB_CHECK((long)p.batch * p.dim < (1L << 31), "selective_scan_fwd: batch*dim too large");
     VMB_CHECK(!out_f32 || (p.ndesc == 0 && (dtype == VMB_BF16 || dtype == VMB_F16)),
               "selective_scan_fwd: fp32 output needs bf16 / fp16 inputs and the flat operator");
+    VMB_CHECK(ext == 0 || (p.ndesc == 0 && !out_f32), "selective_scan_fwd: the z gate exists for the flat operator without fp32 output");
+    VMB_CHECK(!(ext & kScanPairCkpt) || p.ckpt, "selective_scan_fwd: pair-layout checkpoints without a checkpoint buffer");
     {  // fast path: TMA-staged kernel (scan_fwd_tma.cu); this file keeps the generic shapes (unaligned rows, dstate > 16, short L)
         int rb, ss;
-        if (scan_fwd_tma_pick(p, rb, ss)) return scan_fwd_tma_launch(p, dtype, rb, ss, stream, out_f32);
+        if (scan_fwd_tma_pick(p, rb, ss)) return scan_fwd_tma_launch(p, dtype, rb, ss, stream, out_f32, ext);
     }
     if (p.ndesc) {
         VMB_CHECK(p.vec_ok && p.npad == 16, "grouped scan: needs 16 B-aligned rows (L %% 8 == 0) and dstate <= 16");
     }
-    if (out_f32) return dtype == VMB_BF16 ? launch_t<__nv_bfloat16, float>(p, stream) : launch_t<__half, float>(p, stream);
+    if (out_f32) return dtype == VMB_BF16 ? launch_t<__nv_bfloat16, float>(p, ext, stream) : launch_t<__half, float>(p, ext, stream);
     switch (dtype) {
-        case VMB_F32: return launch_t<float>(p, stream);
-        case VMB_BF16: return launch_t<__nv_bfloat16>(p, stream);
-        case VMB_F16: return launch_t<__half>(p, stream);
+        case VMB_F32: return launch_t<float>(p, ext, stream);
+        case VMB_BF16: return launch_t<__nv_bfloat16>(p, ext, stream);
+        case VMB_F16: return launch_t<__half>(p, ext, stream);
     }
     set_error("selective_scan_fwd: unsupported dtype %d", dtype);
     return VMB_ERR_INVALID;

@@ -38,6 +38,8 @@ struct TmaCfg {
 
 // MODE 0: plain operator   1: plain + checkpoints (training forward)   2: per-group sources, reversed walk (fused OSS block)
 //      3: per-group sources + checkpoints (cross_selective_scan forward; indexed by sequence position, like MODE 1 on gathered copies)
+//      + kScanGate / kScanPairCkpt (scan_params.h) on MODE 0 / 1 with out_t = in_t: also out_z = out * SiLU(z); pair-layout
+//        checkpoints (selective_scan_cuda)
 // out_t: element type of `out`; float with 16-bit in_t (MODE 0 / 1 only) stores the fp32 accumulator without rounding
 // (selective_scan_cuda_oflex, out_float=True)
 template <typename in_t, int RB, int NW, int SS, int MODE, typename out_t>
@@ -50,6 +52,8 @@ __global__ void __launch_bounds__(32 * NW, NW == 8 ? 2 : 3)
     constexpr int SEGW = Cfg::SEGW, CHUNK = Cfg::CHUNK, SEGQ = Cfg::SEGQ, SLOTS = Cfg::SLOTS;
     constexpr int V = Vec<in_t>::N, NT = 32 * NW, ROWS = K::ROWS, NPW = K::NPW;
     constexpr int VO = Vec<out_t>::N;
+    constexpr int M = MODE & 3;  // base mode
+    constexpr bool GATE = (MODE & kScanGate) != 0, PAIR = (MODE & kScanPairCkpt) != 0;
 
     extern __shared__ unsigned char smem_dyn[];
     unsigned char* smem_raw = smem_dyn + ((128u - (smem_addr(smem_dyn) & 127u)) & 127u);  // TMA destinations: 128 B aligned
@@ -78,7 +82,7 @@ __global__ void __launch_bounds__(32 * NW, NW == 8 ? 2 : 3)
     out_t* orow;
     bool rev = false;
     int gi = 0, zbc = g, urow0 = dc0;
-    if (MODE < 2) {
+    if (M < 2) {
         orow = reinterpret_cast<out_t*>(p.out) + (int64_t)b * p.o_bs + (int64_t)d * p.o_ds;
     } else {
         const ScanGroupDesc& gd = p.grp[g];
@@ -118,12 +122,12 @@ __global__ void __launch_bounds__(32 * NW, NW == 8 ? 2 : 3)
         mbarrier_wait(bar, phase);
         phase ^= 1;
         if (c0 > 0) __syncthreads();  // every warp is done with the previous fp32 tile
-        convert_bc_dense<in_t, RB, NT>(sB, rawB, tid, MODE >= 2 && rev);
-        convert_bc_dense<in_t, RB, NT>(sC, rawC, tid, MODE >= 2 && rev);
+        convert_bc_dense<in_t, RB, NT>(sB, rawB, tid, M >= 2 && rev);
+        convert_bc_dense<in_t, RB, NT>(sC, rawC, tid, M >= 2 && rev);
         {
             const in_t* ur = rawU + (rs * RB + r) * CHUNK;
             const in_t* dr = rawD + (rs * RB + r) * CHUNK;
-            if (MODE < 2 || !rev) {
+            if (M < 2 || !rev) {
 #pragma unroll
                 for (int v = 0; v < T / V; ++v) {
                     load_vec_smem<in_t>(ur + sl * T + v * V, uv + v * V);
@@ -281,7 +285,9 @@ __global__ void __launch_bounds__(32 * NW, NW == 8 ? 2 : 3)
                     y[t + 1] = fmaf(h.y, Cq.w, fmaf(h.x, Cq.z, y[t + 1]));
                 }
             }
-            if ((MODE == 1 || MODE == 3) && l0 < L && ((l0 + T) % kScanCkpt) == 0) {
+            if constexpr (PAIR) {
+                store_ckpt_pair(p, b, d, l0, n0, h);
+            } else if ((M == 1 || M == 3) && l0 < L && ((l0 + T) % kScanCkpt) == 0) {
                 float* ck = p.ckpt + (((int64_t)b * p.dim + d) * p.n_ckpt + ((l0 + T) / kScanCkpt - 1)) * N + n0;
                 if (n0 < N) ck[0] = h.x;
                 if (n0 + 1 < N) ck[1] = h.y;
@@ -301,9 +307,10 @@ __global__ void __launch_bounds__(32 * NW, NW == 8 ? 2 : 3)
 #pragma unroll
                 for (int t = 0; t < T; ++t) y[t] += yp[(s * T + t) * 32 + lane];
         }
-        if (MODE < 2 || !rev) {
+        if (M < 2 || !rev) {
 #pragma unroll
             for (int v = 0; v < T / VO; ++v) store_vec<out_t>(orow + l0 + v * VO, y + v * VO, valid - v * VO, true);
+            if constexpr (GATE) store_gated<in_t>(scan_gate_desc(p), b, d, l0, y, valid, true);
         } else if (valid == T) {  // sequence l0+t -> memory L-1-l0-t: one reversed contiguous block
 #pragma unroll
             for (int v = 0; v < T / VO; ++v) {
@@ -379,30 +386,41 @@ static int launch_tma4(const ScanFwdParams& p, const ScanTmaMaps& maps, cudaStre
 }
 
 template <typename in_t, int RB, int NW, int SS, typename out_t>
-static int launch_tma3(const ScanFwdParams& p, const ScanTmaMaps& maps, cudaStream_t stream) {
+static int launch_tma3(const ScanFwdParams& p, const ScanTmaMaps& maps, int ext, cudaStream_t stream) {
     if constexpr (std::is_same<in_t, out_t>::value) {  // the grouped modes exist with the input's output type only
         if (p.ndesc) return p.ckpt ? launch_tma4<in_t, RB, NW, SS, 3, out_t>(p, maps, stream) : launch_tma4<in_t, RB, NW, SS, 2, out_t>(p, maps, stream);
     }
     VMB_CHECK(p.ndesc == 0, "selective_scan_fwd_grouped: no fp32 output");
-    return p.ckpt ? launch_tma4<in_t, RB, NW, SS, 1, out_t>(p, maps, stream) : launch_tma4<in_t, RB, NW, SS, 0, out_t>(p, maps, stream);
+    if (ext == 0)
+        return p.ckpt ? launch_tma4<in_t, RB, NW, SS, 1, out_t>(p, maps, stream) : launch_tma4<in_t, RB, NW, SS, 0, out_t>(p, maps, stream);
+    // gated / pair-checkpoint modes (input's output type only), instantiated after the plain ones so that those compile as before
+    if constexpr (std::is_same<in_t, out_t>::value) {
+        if (ext & kScanGate) {
+            return p.ckpt ? launch_tma4<in_t, RB, NW, SS, 1 | kScanGate | kScanPairCkpt, out_t>(p, maps, stream)
+                          : launch_tma4<in_t, RB, NW, SS, kScanGate, out_t>(p, maps, stream);
+        }
+        return launch_tma4<in_t, RB, NW, SS, 1 | kScanPairCkpt, out_t>(p, maps, stream);
+    }
+    set_error("selective_scan_fwd: no z gate / pair checkpoints with fp32 output");
+    return VMB_ERR_INVALID;
 }
 
 // 4-warp CTAs, three resident per SM: 384 CTAs at (8, 384, 4096) spread 2-3 per SM (8-warp CTAs: 192 on 132 SMs, 1-2 per SM)
 constexpr int kTmaWarps = 4;
 
 template <typename in_t, int RB, typename out_t>
-static int launch_tma2(const ScanFwdParams& p, const ScanTmaMaps& maps, int ss, cudaStream_t stream) {
+static int launch_tma2(const ScanFwdParams& p, const ScanTmaMaps& maps, int ss, int ext, cudaStream_t stream) {
     switch (ss) {
-        case 4: return launch_tma3<in_t, RB, kTmaWarps, 4, out_t>(p, maps, stream);
-        case 2: return launch_tma3<in_t, RB, kTmaWarps, 2, out_t>(p, maps, stream);
-        default: return launch_tma3<in_t, RB, kTmaWarps, 1, out_t>(p, maps, stream);
+        case 4: return launch_tma3<in_t, RB, kTmaWarps, 4, out_t>(p, maps, ext, stream);
+        case 2: return launch_tma3<in_t, RB, kTmaWarps, 2, out_t>(p, maps, ext, stream);
+        default: return launch_tma3<in_t, RB, kTmaWarps, 1, out_t>(p, maps, ext, stream);
     }
 }
 
 template <typename in_t, typename out_t = in_t>
-static int launch_tma1(const ScanFwdParams& p, const ScanTmaMaps& maps, int ss, cudaStream_t stream) {
+static int launch_tma1(const ScanFwdParams& p, const ScanTmaMaps& maps, int ss, int ext, cudaStream_t stream) {
     // rows per warp: 2 (scan_fwd_tma_pick; tools/scan_sweep.py: RB = 4 / 8 lose at every batch size, not instantiated)
-    return launch_tma2<in_t, 2, out_t>(p, maps, ss, stream);
+    return launch_tma2<in_t, 2, out_t>(p, maps, ss, ext, stream);
 }
 
 // (rows per warp, state split) for the TMA kernel; false when the shape is left to the generic kernel.
@@ -426,7 +444,7 @@ bool scan_fwd_tma_pick(const ScanFwdParams& p, int& rb, int& ss) {
     return rpg % (rb * kTmaWarps / ss) == 0;
 }
 
-int scan_fwd_tma_launch(const ScanFwdParams& p_in, int dtype, int rb, int ss, cudaStream_t stream, bool out_f32) {
+int scan_fwd_tma_launch(const ScanFwdParams& p_in, int dtype, int rb, int ss, cudaStream_t stream, bool out_f32, int ext) {
     ScanFwdParams p = p_in;
     {
         p.num_sms = num_sms();
@@ -457,16 +475,16 @@ int scan_fwd_tma_launch(const ScanFwdParams& p_in, int dtype, int rb, int ss, cu
     }
     if (out_f32) {  // fp32 `out` from 16-bit inputs
         switch (dtype) {
-            case VMB_BF16: return launch_tma1<__nv_bfloat16, float>(p, maps, ss, stream);
-            case VMB_F16: return launch_tma1<__half, float>(p, maps, ss, stream);
+            case VMB_BF16: return launch_tma1<__nv_bfloat16, float>(p, maps, ss, ext, stream);
+            case VMB_F16: return launch_tma1<__half, float>(p, maps, ss, ext, stream);
         }
         set_error("selective_scan_fwd: fp32 output needs bf16 / fp16 inputs (dtype %d)", dtype);
         return VMB_ERR_INVALID;
     }
     switch (dtype) {
-        case VMB_F32: return launch_tma1<float>(p, maps, ss, stream);
-        case VMB_BF16: return launch_tma1<__nv_bfloat16>(p, maps, ss, stream);
-        case VMB_F16: return launch_tma1<__half>(p, maps, ss, stream);
+        case VMB_F32: return launch_tma1<float>(p, maps, ss, ext, stream);
+        case VMB_BF16: return launch_tma1<__nv_bfloat16>(p, maps, ss, ext, stream);
+        case VMB_F16: return launch_tma1<__half>(p, maps, ss, ext, stream);
     }
     set_error("selective_scan_fwd: unsupported dtype %d", dtype);
     return VMB_ERR_INVALID;

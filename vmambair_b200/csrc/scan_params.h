@@ -2,6 +2,9 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <string.h>
+
+#include "../../include/vmambair_b200.h"
 
 namespace vmb {
 
@@ -16,6 +19,17 @@ struct ScanGroupDesc {
     int rev;
 };
 
+// z-gated flat forward (selective_scan_cuda): out_z = out * SiLU(z), both (batch, dim, L) in the input dtype, last stride 1.
+struct ScanGateDesc {
+    const void* z;
+    void* out_z;
+    int64_t z_bs, z_ds, oz_bs, oz_ds;
+};
+
+// Forward MODE flags on top of the base modes 0..3 (flat modes 0 / 1 only): kScanGate also stores out_z; kScanPairCkpt writes the
+// checkpoints as (batch, dim, n_ckpt, 2 N) with h_n in slot 2n+1 and 0 in slot 2n, and row n_ckpt-1 always holds the last state.
+constexpr int kScanGate = 4, kScanPairCkpt = 8;
+
 struct ScanFwdParams {
     const void *u, *delta, *Bm, *Cm;
     const float *A, *D, *bias;
@@ -27,9 +41,21 @@ struct ScanFwdParams {
     int softplus;
     bool vec_ok;
     int ndesc;              // 0: flat tensors (B0 operator); else = G <= 4 group descriptors (strides shared, per-group bases)
-    ScanGroupDesc grp[4];
+    ScanGroupDesc grp[4];   // flat gated modes: the bytes of a ScanGateDesc (scan_gate_desc / set_scan_gate)
     int num_sms;
 };
+
+// The flat modes never read the group descriptors, so the gated ones carry their ScanGateDesc in that storage: the type of the
+// parameter block, and with it the code of every kernel that does not gate, stays as it was.
+static_assert(sizeof(ScanGateDesc) <= sizeof(ScanGroupDesc[4]), "the gate must fit in the group descriptors");
+inline void set_scan_gate(ScanFwdParams& p, const ScanGateDesc& g) { memcpy(p.grp, &g, sizeof(g)); }
+#ifdef __CUDACC__
+__device__ __forceinline__ ScanGateDesc scan_gate_desc(const ScanFwdParams& p) {
+    ScanGateDesc g;
+    memcpy(&g, p.grp, sizeof(g));
+    return g;
+}
+#endif
 
 // Per-group operands of the direction-aware backward: the forward's sources, the incoming gradient and the four gradient
 // outputs of group g, all in the memory order of that group's sources (rev: sequence position l <-> memory index L-1-l).
@@ -100,9 +126,12 @@ int64_t scan_bwd_grouped_det_workspace(const ScanBwdParams& p);
 
 // out_f32 / dout_f32 (16-bit dtype only): `out` / `dout` are fp32 (selective_scan_cuda_oflex).  They are launcher arguments, not
 // parameter-block members, so that the kernels instantiated without them keep their parameter layout.
-int scan_fwd_launch(const ScanFwdParams& p, int dtype, cudaStream_t stream, bool out_f32 = false);
+// ext: kScanGate | kScanPairCkpt (launcher argument as well; kScanPairCkpt only with checkpoints, neither with out_f32 or groups).
+int scan_fwd_launch(const ScanFwdParams& p, int dtype, cudaStream_t stream, bool out_f32 = false, int ext = 0);
 bool scan_fwd_tma_pick(const ScanFwdParams& p, int& rb, int& ss);
-int scan_fwd_tma_launch(const ScanFwdParams& p, int dtype, int rb, int ss, cudaStream_t stream, bool out_f32 = false);
+int scan_fwd_tma_launch(const ScanFwdParams& p, int dtype, int rb, int ss, cudaStream_t stream, bool out_f32 = false, int ext = 0);
+// elementwise backward of the z gate (vmb_scan_gate_bwd)
+int scan_gate_bwd_launch(const vmb_scan_gate_args& a, bool vec_ok, cudaStream_t stream);
 int scan_bwd_launch(const ScanBwdParams& p, int dtype, cudaStream_t stream, bool dout_f32 = false, bool det = false);
 bool scan_bwd_tma_pick(const ScanBwdParams& p, int dtype, int& rb, int& ss);
 int scan_bwd_tma_launch(const ScanBwdParams& p, int dtype, int rb, int ss, cudaStream_t stream, bool dout_f32 = false, bool det = false);

@@ -2,7 +2,9 @@
 
 Mirrors the reference binding `selective_scan_cuda_core.fwd/bwd`
 (Mamba/kernels/selective_scan/csrc/selective_scan/cus/selective_scan.cpp:157-349): same argument
-meaning, same checks, same RuntimeError behaviour.  Outputs are allocated here with torch (the
+meaning, same checks, same RuntimeError behaviour.  `selective_scan_fwd_z` and `scan_gate_bwd` add what mamba_ssm's
+`selective_scan_cuda` has on top (the z gate and its backward, pair-layout checkpoints holding the last state); the module
+`vmambair_b200.selective_scan_cuda` composes them with `selective_scan_bwd` into that module's fwd / bwd.  Outputs are allocated here with torch (the
 library owns nothing), on the input's device and current stream.
 """
 from __future__ import annotations
@@ -195,6 +197,64 @@ def selective_scan_bwd(u, delta, A, B, C_, D, delta_bias, dout, ckpt, delta_soft
     nbytes = es * (4 * b * d * l + 4 * b * g * n * l) + dout.element_size() * b * d * l + 4 * b * d * ((l + 63) // 64) * n
     _run("vmb_selective_scan_bwd", u, "scan_bwd_det" if det else "scan_bwd", a, nbytes=nbytes, kernels=2)
     return du, ddelta, dA, dB, dC, dD, dbias
+
+
+def _check_io(t, like, name, who):
+    if t.dtype != like.dtype or tuple(t.shape) != tuple(like.shape) or not t.is_cuda or (t.stride(-1) != 1 and t.size(-1) != 1):
+        raise RuntimeError(f"{who}: {name} must be a CUDA tensor of shape {tuple(like.shape)} and dtype {like.dtype} with stride(-1)==1")
+
+
+def selective_scan_fwd_z(u, delta, A, B, C_, D=None, z=None, delta_bias=None, delta_softplus=False, need_ckpt=True):
+    """The forward of mamba_ssm's selective_scan_cuda.fwd -> (out, x, out_z).
+    out: the ungated result, delta's dtype.  out_z = out * SiLU(z) from the fp32 accumulator, rounded once (None without z): the
+    same launch writes both.  x: fp32 (B, D, ceil(L/64), 2N) pair-layout checkpoints, x[:, :, -1, 1::2] the state after the last
+    position (None when need_ckpt is False).  The gradient path is selective_scan_bwd on x[..., 1::2] (after scan_gate_bwd with z)."""
+    b, d, l, n, g = _check_common(u, delta, A, B, C_, D, delta_bias, "selective_scan_fwd")
+    if z is not None:
+        _check_io(z, u, "z", "selective_scan_fwd")
+    out = torch.empty((b, d, l), dtype=u.dtype, device=u.device)
+    out_z = torch.empty_like(out) if z is not None else None
+    ck = ckpt_interval()
+    x = torch.empty((b, d, (l + ck - 1) // ck, 2 * n), dtype=torch.float32, device=u.device) if need_ckpt else None
+    a = _lib.ScanFwdArgs(
+        u=_ptr(u), delta=_ptr(delta), A=_ptr(A), Bm=_ptr(B), Cm=_ptr(C_), D=_ptr(D), delta_bias=_ptr(delta_bias), out=_ptr(out),
+        ckpt=_ptr(x), batch=b, dim=d, seqlen=l, dstate=n, ngroups=g,
+        u_bs=u.stride(0), u_ds=u.stride(1), delta_bs=delta.stride(0), delta_ds=delta.stride(1), out_bs=out.stride(0), out_ds=out.stride(1),
+        B_bs=B.stride(0), B_gs=B.stride(1), B_ns=B.stride(2), C_bs=C_.stride(0), C_gs=C_.stride(1), C_ns=C_.stride(2),
+        delta_softplus=int(bool(delta_softplus)), dtype=_DT[u.dtype], out_f32=0,
+        z=_ptr(z), out_z=_ptr(out_z), z_bs=z.stride(0) if z is not None else 0, z_ds=z.stride(1) if z is not None else 0,
+        out_z_bs=out_z.stride(0) if z is not None else 0, out_z_ds=out_z.stride(1) if z is not None else 0,
+        ckpt_pairs=int(need_ckpt))
+    es = u.element_size()
+    nbytes = es * ((2 + (3 if z is not None else 1)) * b * d * l + 2 * b * g * n * l) + 4 * (d * n + 2 * d)
+    _run("vmb_selective_scan_fwd", u, "scan_fwd_z" if z is not None else "scan_fwd", a, nbytes=nbytes)
+    return out, x, out_z
+
+
+def scan_gate_bwd(dout, out, z, dz=None, recompute_out_z=False):
+    """Backward of out_z = out * SiLU(z) (the gate of selective_scan_fwd_z), one launch -> (dout_eff, dz, out_z).
+    dout_eff = dout * SiLU(z), fp32: the gradient w.r.t. the ungated out, for selective_scan_bwd(..., dout_float=True).
+    dz = dout * out * s * (1 + z (1 - s)), s = sigmoid(z), in z's dtype, written into `dz` when given (any view with stride(-1)==1).
+    out_z: out * SiLU(z) when recompute_out_z, else None."""
+    who = "scan_gate_bwd"
+    _check_io(z, z, "z", who)
+    _check_io(dout, z, "dout", who)
+    _check_io(out, z, "out", who)
+    b, d, l = z.shape
+    if dz is None:
+        dz = torch.empty((b, d, l), dtype=z.dtype, device=z.device)
+    else:
+        _check_io(dz, z, "dz", who)
+    dout_eff = torch.empty((b, d, l), dtype=torch.float32, device=z.device)
+    out_z = torch.empty((b, d, l), dtype=z.dtype, device=z.device) if recompute_out_z else None
+    a = _lib.ScanGateArgs(
+        dout=_ptr(dout), out=_ptr(out), z=_ptr(z), dout_eff=_ptr(dout_eff), dz=_ptr(dz), out_z=_ptr(out_z), batch=b, dim=d, seqlen=l,
+        dout_bs=dout.stride(0), dout_ds=dout.stride(1), out_bs=out.stride(0), out_ds=out.stride(1), z_bs=z.stride(0), z_ds=z.stride(1),
+        dz_bs=dz.stride(0), dz_ds=dz.stride(1), out_z_bs=out_z.stride(0) if recompute_out_z else 0,
+        out_z_ds=out_z.stride(1) if recompute_out_z else 0, dtype=_DT[z.dtype])
+    es = z.element_size()
+    _run("vmb_scan_gate_bwd", z, "scan_gate_bwd", a, nbytes=(es * (4 + int(bool(recompute_out_z))) + 4) * b * d * l)
+    return dout_eff, dz, out_z
 
 
 # ----------------------------------------------------------------------------- fused OSS-block stages

@@ -7,7 +7,7 @@ from __future__ import annotations
 
 import torch
 
-from . import ops
+from . import ops, selective_scan_cuda
 
 
 class SelectiveScanFn(torch.autograd.Function):
@@ -76,3 +76,56 @@ def selective_scan_fn(u, delta, A, B, C, D=None, delta_bias=None, delta_softplus
 
 
 selective_scan_fn_v1 = selective_scan_fn
+
+
+class MambaSelectiveScanFn(torch.autograd.Function):
+    """mamba_ssm's SelectiveScanFn over selective_scan_cuda (the reference's wrapper, Mamba/kernels/selective_scan/
+    test_selective_scan.py:18-165, MODE "mamba_ssm")"""
+
+    @staticmethod
+    def forward(ctx, u, delta, A, B, C, D=None, z=None, delta_bias=None, delta_softplus=False, return_last_state=False):
+        u, delta, B, C = (t if t.stride(-1) == 1 else t.contiguous() for t in (u, delta, B, C))
+        if z is not None and z.stride(-1) != 1:
+            z = z.contiguous()
+        ctx._d_dtype = None if D is None else D.dtype
+        ctx._b_dtype = None if delta_bias is None else delta_bias.dtype
+        if D is not None:
+            D = D.contiguous().float()
+        if delta_bias is not None:
+            delta_bias = delta_bias.float()
+        A = A.contiguous()
+        out, x, *rest = selective_scan_cuda.fwd(u, delta, A, B, C, D, z, delta_bias, delta_softplus)
+        ctx.delta_softplus = delta_softplus
+        ctx.has_z = z is not None
+        ctx.save_for_backward(u, delta, A, B, C, D, z, delta_bias, x, out if z is not None else None)
+        y = rest[0] if z is not None else out
+        if not return_last_state:
+            return y
+        last_state = x[:, :, -1, 1::2]
+        ctx.mark_non_differentiable(last_state)
+        return y, last_state
+
+    @staticmethod
+    def backward(ctx, dout, *args):
+        u, delta, A, B, C, D, z, delta_bias, x, out = ctx.saved_tensors
+        du, ddelta, dA, dB, dC, dD, dbias, *rest = selective_scan_cuda.bwd(
+            u, delta, A, B, C, D, z, delta_bias, dout, x, out, None, ctx.delta_softplus, False)
+        dz = rest[0] if ctx.has_z else None
+        if dD is not None and ctx._d_dtype not in (None, dD.dtype):
+            dD = dD.to(ctx._d_dtype)
+        if dbias is not None and ctx._b_dtype not in (None, dbias.dtype):
+            dbias = dbias.to(ctx._b_dtype)
+        return du, ddelta, dA, dB, dC, dD, dz, dbias, None, None
+
+
+def mamba_selective_scan_fn(u, delta, A, B, C, D=None, z=None, delta_bias=None, delta_softplus=False, return_last_state=False):
+    """mamba_ssm's selective_scan_fn: out = selective_scan(u, delta, A, B, C, D, delta_bias, delta_softplus), times SiLU(z) when z
+    is given, with autograd (dz included).  Its 7th positional argument is z, where selective_scan_fn's is delta_bias.
+    return_last_state: also return the state after the last position, (batch, dim, dstate) fp32, which has no gradient.
+    B, C: (batch, dstate, L) or (batch, G, dstate, L); A real.  Mixed input dtypes are promoted to fp32 as in selective_scan_fn.
+    Under torch.use_deterministic_algorithms(True) the gradients are bitwise reproducible."""
+    ts = (u, delta, B, C) + ((z,) if z is not None else ())
+    if any(t.dtype != u.dtype for t in ts):
+        u, delta, B, C = u.float(), delta.float(), B.float(), C.float()
+        z = z.float() if z is not None else None
+    return MambaSelectiveScanFn.apply(u, delta, A, B, C, D, z, delta_bias, delta_softplus, return_last_state)
