@@ -482,6 +482,69 @@ typedef struct {
 } vmb_adam_args;
 int vmb_fused_adam(const vmb_adam_args* a, void* stream);
 
+/* ---- image-level I/O: the host-side conversions of RealESRGANer.enhance (RealSR/VmambaIR/utils.py:174-243) ----------------------
+ * Images are 8- or 16-bit (u16 = 0 / 1), H x W pixels of `channels` (1 gray, 3 BGR, 4 BGRA) values; element strides between rows,
+ * pixels and channels are given separately, so crops, flips and channel views need no copy.  Planes are NCHW in the compute dtype. */
+
+/* largest value of an image (every channel) -> *max_out (uint32, device); the library zero-fills it first on `stream`.  enhance() reads
+ * it back once to choose 8- or 16-bit processing (np.max(img) > 256, utils.py:178). */
+typedef struct {
+    const void* img;
+    int H, W, channels, u16;
+    int64_t row_stride, pixel_stride, channel_stride;
+    unsigned int* max_out;
+} vmb_image_max_args;
+int vmb_image_max(const vmb_image_max_args* a, void* stream);
+
+/* image -> planes (pre_process + the colour conversions of enhance, utils.py:71-91,177-196), one pass:
+ *   v = img / max_range (an IEEE float division, as numpy's), BGR -> RGB, a gray channel repeated three times;
+ *   out (1 + alpha_plane, 3, Hp, Wp) dense in `dtype`; alpha_plane = 1 (channels 4 only): image 1 of the batch is the alpha channel
+ *   repeated three times (the 'realesrgan' alpha upsampler runs it through the network);
+ *   pad_h[i] / pad_w[i]: three successive bottom / right reflect pads (F.pad 'reflect'): pre_pad, the mod pad, the pad to the
+ *   network's multiple; each smaller than the size it pads.  Hp = H + sum pad_h, Wp = W + sum pad_w. */
+typedef struct {
+    const void* img; void* out;
+    int H, W, channels, u16;
+    int64_t row_stride, pixel_stride, channel_stride;
+    float max_range;
+    int pad_h[3], pad_w[3];
+    int alpha_plane;
+    int dtype;
+} vmb_image_to_planes_args;
+int vmb_image_to_planes(const vmb_image_to_planes_args* a, void* stream);
+
+/* planes -> image (post_process + the output half of enhance, utils.py:162-171,205-234), one pass:
+ *   planes (batch, 3, *, *) in `dtype` with element strides p_bs, p_cs, p_rs (pixels contiguous); the top-left H x W pixels are read
+ *   (post_process's crops); v = clamp(plane, 0, 1); RGB -> BGR;
+ *   channels 1: the gray value fma(r, 0.299f, fma(b, 0.114f, g * 0.587f)) (cv2 COLOR_BGR2GRAY on float32);
+ *   channels 4: alpha_mode 0 -> the gray value of planes image 1;  alpha_mode 1 -> cv2.resize(alpha_src / max_range, (W, H),
+ *     INTER_LINEAR) of the source image's alpha channel (alpha_src: alpha_H x alpha_W, uint8 or uint16 (alpha_u16), strides
+ *     alpha_rs / alpha_ps): half-pixel centres, replicated border, s0 a0 + s1 a1 per row then per column in float32;
+ *   out = saturate(rint(v * max_range)) (numpy's round half to even), uint8 or uint16 (u16) HWC, element strides out_rs (rows),
+ *   out_ps (pixels); channels stride 1. */
+typedef struct {
+    const void* planes; void* out; const void* alpha_src;
+    int H, W, channels, u16;
+    int64_t p_bs, p_cs, p_rs;
+    int64_t out_rs, out_ps;
+    int alpha_mode, alpha_H, alpha_W, alpha_u16;
+    int64_t alpha_rs, alpha_ps;
+    float max_range;
+    int dtype;
+} vmb_planes_to_image_args;
+int vmb_planes_to_image(const vmb_planes_to_image_args* a, void* stream);
+
+/* cv2.resize(src, (dW, dH), interpolation=cv2.INTER_LANCZOS4) on uint8 / uint16 HWC images (enhance's outscale, utils.py:236-241):
+ * sample x = (dx + 0.5) sW / dW - 0.5 (OpenCV's float rounding of it), 8 x 8 taps at floor(x) - 3 .. floor(x) + 4 clamped to the
+ * image, Lanczos weights normalised in float; 8-bit: 11-bit fixed-point weights, int32 sums, the 22-bit result rounded; 16-bit:
+ * float sums, row pass then column pass, rounded half to even and saturated.  Strides in elements; channels stride 1. */
+typedef struct {
+    const void* src; void* dst;
+    int sH, sW, dH, dW, channels, u16;
+    int64_t src_rs, src_ps, dst_rs, dst_ps;
+} vmb_resize_lanczos4_args;
+int vmb_resize_lanczos4(const vmb_resize_lanczos4_args* a, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -237,6 +237,33 @@ class AdamArgs(C.Structure):
                 ("grad_scale", C.c_float), ("max_grad_norm", C.c_float), ("ema_decay", C.c_float), ("zero_grad", C.c_int)]
 
 
+class ImageMaxArgs(C.Structure):
+    _c_name_ = "vmb_image_max_args"
+    _fields_ = [("img", vp), ("H", C.c_int), ("W", C.c_int), ("channels", C.c_int), ("u16", C.c_int),
+                ("row_stride", i64), ("pixel_stride", i64), ("channel_stride", i64), ("max_out", vp)]
+
+
+class ImageToPlanesArgs(C.Structure):
+    _c_name_ = "vmb_image_to_planes_args"
+    _fields_ = [("img", vp), ("out", vp), ("H", C.c_int), ("W", C.c_int), ("channels", C.c_int), ("u16", C.c_int),
+                ("row_stride", i64), ("pixel_stride", i64), ("channel_stride", i64), ("max_range", C.c_float),
+                ("pad_h", C.c_int * 3), ("pad_w", C.c_int * 3), ("alpha_plane", C.c_int), ("dtype", C.c_int)]
+
+
+class PlanesToImageArgs(C.Structure):
+    _c_name_ = "vmb_planes_to_image_args"
+    _fields_ = [("planes", vp), ("out", vp), ("alpha_src", vp), ("H", C.c_int), ("W", C.c_int), ("channels", C.c_int), ("u16", C.c_int),
+                ("p_bs", i64), ("p_cs", i64), ("p_rs", i64), ("out_rs", i64), ("out_ps", i64),
+                ("alpha_mode", C.c_int), ("alpha_H", C.c_int), ("alpha_W", C.c_int), ("alpha_u16", C.c_int),
+                ("alpha_rs", i64), ("alpha_ps", i64), ("max_range", C.c_float), ("dtype", C.c_int)]
+
+
+class ResizeLanczos4Args(C.Structure):
+    _c_name_ = "vmb_resize_lanczos4_args"
+    _fields_ = [("src", vp), ("dst", vp), ("sH", C.c_int), ("sW", C.c_int), ("dH", C.c_int), ("dW", C.c_int),
+                ("channels", C.c_int), ("u16", C.c_int), ("src_rs", i64), ("src_ps", i64), ("dst_rs", i64), ("dst_ps", i64)]
+
+
 # every symbol include/vmambair_b200.h declares: name -> (restype, argtypes)
 SYMBOLS = {
     "vmb_last_error": (C.c_char_p, []),
@@ -280,6 +307,10 @@ SYMBOLS = {
     "vmb_cross_selective_scan_c_workspace_bytes": (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int]),
     "vmb_prep_block_weights": (C.c_int, [C.POINTER(PrepArgs), vp]),
     "vmb_sum4_add": (C.c_int, [vp, vp, vp, C.c_int, C.c_long, C.c_int, vp]),
+    "vmb_image_max": (C.c_int, [C.POINTER(ImageMaxArgs), vp]),
+    "vmb_image_to_planes": (C.c_int, [C.POINTER(ImageToPlanesArgs), vp]),
+    "vmb_planes_to_image": (C.c_int, [C.POINTER(PlanesToImageArgs), vp]),
+    "vmb_resize_lanczos4": (C.c_int, [C.POINTER(ResizeLanczos4Args), vp]),
 }
 
 

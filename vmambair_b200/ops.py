@@ -823,3 +823,82 @@ def channel_branch_bwd(pooled, inv_count, prm, C_, dc_out, into=None):
                             scratch=_ptr(scratch))
     _run("vmb_channel_branch_bwd", pooled, "channel_bwd", a)
     return dpooled, g
+
+
+# ---- image-level I/O (vmambair_b200.enhance; RealSR/VmambaIR/utils.py:174-243) ----
+
+def _image_geom(img, who):
+    """(H, W, channels, u16, row / pixel / channel element strides) of a uint8 / uint16 (H, W) or (H, W, C) CUDA tensor"""
+    if img.dtype not in (torch.uint8, torch.uint16):
+        raise RuntimeError(f"{who}: image dtype must be uint8 or uint16, got {img.dtype}")
+    if not img.is_cuda:
+        raise RuntimeError(f"{who}: image must be a CUDA tensor")
+    if img.dim() == 2:
+        (H, W), (rs, ps), c, cs = img.shape, img.stride(), 1, 0
+    elif img.dim() == 3 and img.shape[2] in (1, 3, 4):
+        (H, W, c), (rs, ps, cs) = img.shape, img.stride()
+    else:
+        raise RuntimeError(f"{who}: image must be (H, W) or (H, W, C) with C in 1, 3, 4; got {tuple(img.shape)}")
+    return H, W, c, int(img.dtype == torch.uint16), rs, ps, cs
+
+
+def image_max(img):
+    """largest value of a uint8 / uint16 image as a 1-element int32 CUDA tensor (read it back once: enhance's 16-bit test)"""
+    H, W, c, u16, rs, ps, cs = _image_geom(img, "image_max")
+    out = torch.empty(1, dtype=torch.int32, device=img.device)
+    a = _lib.ImageMaxArgs(img=_ptr(img), H=H, W=W, channels=c, u16=u16, row_stride=rs, pixel_stride=ps, channel_stride=cs,
+                          max_out=_ptr(out))
+    _run("vmb_image_max", img, "image_max", a, nbytes=H * W * c * img.element_size())
+    return out
+
+
+def image_to_planes(img, max_range, pad_h=(0, 0, 0), pad_w=(0, 0, 0), alpha_plane=False, dtype=torch.float32):
+    """uint8 / uint16 HWC image -> (1 + alpha_plane, 3, H + sum(pad_h), W + sum(pad_w)) planes in `dtype`: img / max_range, BGR -> RGB
+    (gray repeated), three successive bottom / right reflect pads; alpha_plane: image 1 of the batch is the alpha channel x 3."""
+    H, W, c, u16, rs, ps, cs = _image_geom(img, "image_to_planes")
+    Hp, Wp = H + sum(pad_h), W + sum(pad_w)
+    out = torch.empty((1 + int(alpha_plane), 3, Hp, Wp), dtype=dtype, device=img.device)
+    a = _lib.ImageToPlanesArgs(img=_ptr(img), out=_ptr(out), H=H, W=W, channels=c, u16=u16, row_stride=rs, pixel_stride=ps,
+                               channel_stride=cs, max_range=float(max_range), pad_h=(C.c_int * 3)(*pad_h),
+                               pad_w=(C.c_int * 3)(*pad_w), alpha_plane=int(bool(alpha_plane)), dtype=_DT[dtype])
+    _run("vmb_image_to_planes", img, "image_to_planes", a, nbytes=H * W * c * img.element_size() + out.numel() * out.element_size())
+    return out
+
+
+def planes_to_image(planes, H, W, channels, max_range, out_dtype, alpha_src=None, out=None):
+    """(batch, 3, >= H, >= W) planes (pixel-contiguous rows) -> uint8 / uint16 image (H, W) for channels 1, else (H, W, channels):
+    top-left crop, clamp to [0, 1], RGB -> BGR, BGR2GRAY for channels 1; channels 4: alpha from planes image 1 (BGR2GRAY), or, with
+    alpha_src (the source image's alpha channel, (h, w) uint8 / uint16 view), cv2 INTER_LINEAR from it; x max_range, rounded half to
+    even, saturated."""
+    if planes.dtype not in _DT or planes.dim() != 4 or planes.shape[1] != 3 or planes.stride(3) != 1 or not planes.is_cuda:
+        raise RuntimeError("planes_to_image: planes must be a (B, 3, H, W) float32 / bf16 / fp16 CUDA tensor with stride(3) == 1")
+    if planes.shape[2] < H or planes.shape[3] < W or (channels == 4 and alpha_src is None and planes.shape[0] < 2):
+        raise RuntimeError(f"planes_to_image: planes {tuple(planes.shape)} too small for a {H} x {W} x {channels} image")
+    shape = (H, W) if channels == 1 else (H, W, channels)
+    if out is None:
+        out = torch.empty(shape, dtype=out_dtype, device=planes.device)
+    if tuple(out.shape) != shape or out.dtype not in (torch.uint8, torch.uint16) or (channels > 1 and out.stride(2) != 1):
+        raise RuntimeError(f"planes_to_image: out must be a uint8 / uint16 {shape} tensor with contiguous channels")
+    ah = aw = ars = aps = au16 = 0
+    if alpha_src is not None:
+        ah, aw, _, au16, ars, aps, _ = _image_geom(alpha_src, "planes_to_image")
+    a = _lib.PlanesToImageArgs(planes=_ptr(planes), out=_ptr(out), alpha_src=_ptr(alpha_src), H=H, W=W, channels=channels,
+                               u16=int(out.dtype == torch.uint16), p_bs=planes.stride(0), p_cs=planes.stride(1), p_rs=planes.stride(2),
+                               out_rs=out.stride(0), out_ps=out.stride(1), alpha_mode=int(alpha_src is not None), alpha_H=ah,
+                               alpha_W=aw, alpha_u16=au16, alpha_rs=ars, alpha_ps=aps, max_range=float(max_range),
+                               dtype=_DT[planes.dtype])
+    _run("vmb_planes_to_image", planes, "planes_to_image", a,
+         nbytes=H * W * (planes.element_size() * 3 * (1 + int(channels == 4 and alpha_src is None)) + channels * out.element_size()))
+    return out
+
+
+def resize_lanczos4(img, width, height):
+    """cv2.resize(img, (width, height), interpolation=cv2.INTER_LANCZOS4) of a uint8 / uint16 (H, W) or (H, W, C) CUDA image"""
+    H, W, c, u16, rs, ps, cs = _image_geom(img, "resize_lanczos4")
+    if c > 1 and cs != 1:
+        raise RuntimeError("resize_lanczos4: the channels of a pixel must be contiguous")
+    out = torch.empty((height, width) if img.dim() == 2 else (height, width, c), dtype=img.dtype, device=img.device)
+    a = _lib.ResizeLanczos4Args(src=_ptr(img), dst=_ptr(out), sH=H, sW=W, dH=height, dW=width, channels=c, u16=u16,
+                                src_rs=rs, src_ps=ps, dst_rs=out.stride(0), dst_ps=out.stride(1))
+    _run("vmb_resize_lanczos4", img, "resize_lanczos4", a, nbytes=(H * W + height * width) * c * img.element_size())
+    return out
