@@ -126,3 +126,43 @@ def scan_bwd(u, delta, A, B, C, D, delta_bias, dout, delta_softplus=False):
                            _p(dD), _p(db), b, Dm, L, N, G)
     t = lambda a: None if a is None else torch.from_numpy(a)
     return tuple(map(t, (du, dd, dA, dB, dC, dD, db)))
+
+
+def scan_fwd_mag(u, delta, A, B, C, D=None, delta_bias=None, delta_softplus=False):
+    """scan_fwd(fp64=True) and the magnitude S of every output (oracle/scan_bound.py) -> (out, S), float64 torch tensors"""
+    b, Dm, L, N, G = _shapes(u, A, B)
+    un, dn, An, Bn, Cn, Dn, bn = map(_f32, (u, delta, A, B, C, D, delta_bias))
+    out, S = np.empty((b, Dm, L), np.float64), np.empty((b, Dm, L), np.float64)
+    lib().scan_ref_fwd_mag(_p(un), _p(dn), _p(An), _p(Bn), _p(Cn), _p(Dn), _p(bn), int(delta_softplus), _p(out), _p(S),
+                           b, Dm, L, N, G)
+    return torch.from_numpy(out), torch.from_numpy(S)
+
+
+def _bwd_outputs(b, Dm, L, N, G, has_D, has_bias, dt):
+    return [np.zeros((b, Dm, L), dt), np.zeros((b, Dm, L), dt), np.zeros((Dm, N), dt), np.zeros((b, G, N, L), dt),
+            np.zeros((b, G, N, L), dt), np.zeros((Dm,), dt) if has_D else None, np.zeros((Dm,), dt) if has_bias else None]
+
+
+def _t(a):
+    return None if a is None else torch.from_numpy(a)
+
+
+def scan_bwd_mag(u, delta, A, B, C, D, delta_bias, dout, delta_softplus=False):
+    """scan_bwd and the magnitude S of every gradient -> ((du, ddelta, dA, dB, dC, dD, dbias), (S_du, ..., S_dbias)), float64"""
+    b, Dm, L, N, G = _shapes(u, A, B)
+    un, dn, An, Bn, Cn, Dn, bn, gn = map(_f32, (u, delta, A, B, C, D, delta_bias, dout))
+    g = _bwd_outputs(b, Dm, L, N, G, D is not None, delta_bias is not None, np.float64)
+    s = _bwd_outputs(b, Dm, L, N, G, D is not None, delta_bias is not None, np.float64)
+    lib().scan_ref_bwd_mag(_p(un), _p(dn), _p(An), _p(Bn), _p(Cn), _p(Dn), _p(bn), int(delta_softplus), _p(gn),
+                           *map(_p, g), *map(_p, s), b, Dm, L, N, G)
+    return tuple(map(_t, g)), tuple(map(_t, s))
+
+
+def scan_bwd_f32(u, delta, A, B, C, D, delta_bias, dout, delta_softplus=False):
+    """the analytic backward evaluated sequentially in fp32 -> (du, ddelta, dA, dB, dC, dD, dbias), float32"""
+    b, Dm, L, N, G = _shapes(u, A, B)
+    un, dn, An, Bn, Cn, Dn, bn, gn = map(_f32, (u, delta, A, B, C, D, delta_bias, dout))
+    g = _bwd_outputs(b, Dm, L, N, G, D is not None, delta_bias is not None, np.float32)
+    lib().scan_ref_bwd_f32(_p(un), _p(dn), _p(An), _p(Bn), _p(Cn), _p(Dn), _p(bn), int(delta_softplus), _p(gn),
+                           *map(_p, g), b, Dm, L, N, G)
+    return tuple(map(_t, g))
