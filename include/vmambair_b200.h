@@ -545,6 +545,79 @@ typedef struct {
 } vmb_resize_lanczos4_args;
 int vmb_resize_lanczos4(const vmb_resize_lanczos4_args* a, void* stream);
 
+/* ---- image metrics: PSNR and SSIM of Deraining/basicsr/metrics/psnr_ssim.py and Deraining/Deraining/utils.py ----------------------
+ * A source is `batch` images of H x W pixels of `channels` values (1 gray, or 3 in BGR order), already cropped: element (b, y, x, c) is
+ * at img + b batch_stride + y row_stride + x pixel_stride + c channel_stride (element strides; any sign, so an RGB planar network
+ * output is read as BGR through a negative channel stride).  `dtype` says how an element becomes the reference's float64 value:
+ *   VMB_MSRC_U8 / U16 / F32 / F64 : the value itself (img.astype(np.float64));
+ *   VMB_MSRC_Q_F32 / Q_BF16 / Q_F16: tensor2img (SRGAN/VmambaIR/utils/img_util.py:36-): rint(clamp(float(v), 0, 1) * 255.f) in float32,
+ *                                    half to even, as uint8.
+ * y_channel = 1: every metric sees to_y_channel(img) (metrics/metric_util.py, utils/matlab_functions.py:207-238,305-361) instead:
+ *   3 channels: x_c = fl32(fl32(v_c) / 255);  Y = fl32(fl32((x_B 24.966 + x_G 128.553 + x_R 65.481 + 16) / 255) * 255), the sum
+ *               in float64 left to right, never contracted;  1 channel: Y = fl32(fl32(fl32(v) / 255) * 255). */
+#define VMB_MSRC_U8 0
+#define VMB_MSRC_U16 1
+#define VMB_MSRC_F32 2
+#define VMB_MSRC_F64 3
+#define VMB_MSRC_Q_F32 4
+#define VMB_MSRC_Q_BF16 5
+#define VMB_MSRC_Q_F16 6
+typedef struct {
+    const void* img;
+    int dtype;
+    int64_t batch_stride, row_stride, pixel_stride, channel_stride;
+} vmb_metric_src;
+
+/* to_y_channel (metrics/metric_util.py) of every pixel of `src` -> out (batch, H, W) dense float32.  channels 1 or 3. */
+typedef struct {
+    vmb_metric_src src;
+    int batch, H, W, channels;
+    float* out;
+} vmb_to_y_args;
+int vmb_to_y_channel(const vmb_to_y_args* a, void* stream);
+
+/* PSNR of each image pair (calculate_psnr, psnr_ssim.py:9-63; utils.py:10-25), deterministic: per-CTA float64 partial sums of the
+ * squared differences in a fixed order, then one CTA per image adds them in index order.  The squared difference is float64, or with
+ * y_channel float32 (a - b) squared in float32, as the reference forms it.  Per image b:
+ *   mse[b] = sum / (H W channels') (channels' = 1 with y_channel), max_value[b] = the largest value of img1 (after y_channel),
+ *   psnr[b] = mse == 0 ? inf : 20 log10(m / sqrt(mse)), m = 1 if max_value[b] <= 1 else 255 (device log10).
+ * workspace: vmb_psnr_workspace_bytes(a) bytes of device memory. */
+typedef struct {
+    vmb_metric_src img1, img2;
+    int batch, H, W, channels, y_channel;
+    double *mse, *max_value, *psnr;
+    void* workspace;
+} vmb_psnr_args;
+int vmb_psnr(const vmb_psnr_args* a, void* stream);
+int64_t vmb_psnr_workspace_bytes(const vmb_psnr_args* a);
+
+/* SSIM of each image pair in float64, from 11 x 11 Gaussian moments (x, y, x^2, y^2, xy) filtered separably from a shared-memory tile
+ * with its 5-pixel halo; taps: cv2.getGaussianKernel(11, 1.5).  ssim[b] is the mean of the SSIM map:
+ *   VMB_SSIM_VALID       the map where the window fits, (H - 10) x (W - 10) per channel, averaged per channel, then over the channels
+ *                        (_ssim, psnr_ssim.py:66-99; ssim / calculate_ssim, utils.py:31-78); nan when H or W < 11;
+ *   VMB_SSIM_REPLICATE   full-size map, borders replicated (_ssim_cly, psnr_ssim.py:184-222); one channel (y_channel or gray);
+ *   VMB_SSIM_REPLICATE3D as REPLICATE, and the channels filtered too, by the 11-tap filter with replicated ends across them
+ *                        (_ssim_3d, psnr_ssim.py:131-182): moment[c] = sum_c' mix[c][c'] moment2d[c'] (mix: channels x channels,
+ *                        row-major, the taps folded onto the clamped channel indices).
+ * C1 = (0.01 m)^2, C2 = (0.03 m)^2 with m = 255, except in REPLICATE3D, where m = 1 if max_value[b] <= 1 else 255 (max_value: device,
+ * per image, e.g. vmb_psnr's).  Partial sums per CTA and channel, added in index order by one CTA per image: deterministic.
+ * workspace: vmb_ssim_workspace_bytes(a) bytes of device memory. */
+#define VMB_SSIM_VALID 0
+#define VMB_SSIM_REPLICATE 1
+#define VMB_SSIM_REPLICATE3D 2
+typedef struct {
+    vmb_metric_src img1, img2;
+    int batch, H, W, channels, y_channel;
+    int mode;
+    double taps[11];
+    double mix[9];
+    const double* max_value;
+    double* ssim;
+    void* workspace;
+} vmb_ssim_args;
+int vmb_ssim(const vmb_ssim_args* a, void* stream);
+int64_t vmb_ssim_workspace_bytes(const vmb_ssim_args* a);
+
 #ifdef __cplusplus
 }
 #endif

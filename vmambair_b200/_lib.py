@@ -264,6 +264,30 @@ class ResizeLanczos4Args(C.Structure):
                 ("channels", C.c_int), ("u16", C.c_int), ("src_rs", i64), ("src_ps", i64), ("dst_rs", i64), ("dst_ps", i64)]
 
 
+class MetricSrc(C.Structure):
+    _c_name_ = "vmb_metric_src"
+    _fields_ = [("img", vp), ("dtype", C.c_int), ("batch_stride", i64), ("row_stride", i64), ("pixel_stride", i64),
+                ("channel_stride", i64)]
+
+
+class ToYArgs(C.Structure):
+    _c_name_ = "vmb_to_y_args"
+    _fields_ = [("src", MetricSrc), ("batch", C.c_int), ("H", C.c_int), ("W", C.c_int), ("channels", C.c_int), ("out", vp)]
+
+
+class PsnrArgs(C.Structure):
+    _c_name_ = "vmb_psnr_args"
+    _fields_ = [("img1", MetricSrc), ("img2", MetricSrc), ("batch", C.c_int), ("H", C.c_int), ("W", C.c_int), ("channels", C.c_int),
+                ("y_channel", C.c_int), ("mse", vp), ("max_value", vp), ("psnr", vp), ("workspace", vp)]
+
+
+class SsimArgs(C.Structure):
+    _c_name_ = "vmb_ssim_args"
+    _fields_ = [("img1", MetricSrc), ("img2", MetricSrc), ("batch", C.c_int), ("H", C.c_int), ("W", C.c_int), ("channels", C.c_int),
+                ("y_channel", C.c_int), ("mode", C.c_int), ("taps", C.c_double * 11), ("mix", C.c_double * 9), ("max_value", vp),
+                ("ssim", vp), ("workspace", vp)]
+
+
 # every symbol include/vmambair_b200.h declares: name -> (restype, argtypes)
 SYMBOLS = {
     "vmb_last_error": (C.c_char_p, []),
@@ -311,6 +335,11 @@ SYMBOLS = {
     "vmb_image_to_planes": (C.c_int, [C.POINTER(ImageToPlanesArgs), vp]),
     "vmb_planes_to_image": (C.c_int, [C.POINTER(PlanesToImageArgs), vp]),
     "vmb_resize_lanczos4": (C.c_int, [C.POINTER(ResizeLanczos4Args), vp]),
+    "vmb_to_y_channel": (C.c_int, [C.POINTER(ToYArgs), vp]),
+    "vmb_psnr": (C.c_int, [C.POINTER(PsnrArgs), vp]),
+    "vmb_psnr_workspace_bytes": (C.c_int64, [C.POINTER(PsnrArgs)]),
+    "vmb_ssim": (C.c_int, [C.POINTER(SsimArgs), vp]),
+    "vmb_ssim_workspace_bytes": (C.c_int64, [C.POINTER(SsimArgs)]),
 }
 
 

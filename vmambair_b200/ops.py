@@ -902,3 +902,54 @@ def resize_lanczos4(img, width, height):
                                 src_rs=rs, src_ps=ps, dst_rs=out.stride(0), dst_ps=out.stride(1))
     _run("vmb_resize_lanczos4", img, "resize_lanczos4", a, nbytes=(H * W + height * width) * c * img.element_size())
     return out
+
+
+# ---- image metrics (csrc/metrics.cu): PSNR / SSIM of the reference's psnr_ssim.py and Deraining/utils.py ----
+MSRC = {torch.uint8: 0, torch.uint16: 1, torch.float32: 2, torch.float64: 3}   # VMB_MSRC_*: the value itself
+MSRC_Q = {torch.float32: 4, torch.bfloat16: 5, torch.float16: 6}                 # VMB_MSRC_Q_*: tensor2img's uint8 of the value
+SSIM_MODES = {"valid": 0, "replicate": 1, "replicate3d": 2}                       # VMB_SSIM_*
+
+
+def metric_src(t, offset, strides, quantize=False):
+    """vmb_metric_src of the (batch, H, W, channels) view of CUDA tensor t's storage that starts `offset` elements after t.data_ptr()
+    with element strides (batch, row, pixel, channel); a stride may be negative (an RGB planar tensor read as BGR)."""
+    table = MSRC_Q if quantize else MSRC
+    if t.dtype not in table:
+        raise RuntimeError(f"metrics: {'quantized ' if quantize else ''}source dtype {t.dtype} not in {list(table)}")
+    return _lib.MetricSrc(img=C.c_void_p(t.data_ptr() + offset * t.element_size()), dtype=table[t.dtype], batch_stride=strides[0],
+                          row_stride=strides[1], pixel_stride=strides[2], channel_stride=strides[3])
+
+
+def to_y_channel_planes(t, src, batch, H, W, channels):
+    """to_y_channel of `src` (a metric_src view of CUDA tensor t) -> (batch, H, W) float32"""
+    out = torch.empty((batch, H, W), dtype=torch.float32, device=t.device)
+    a = _lib.ToYArgs(src=src, batch=batch, H=H, W=W, channels=channels, out=_ptr(out))
+    _run("vmb_to_y_channel", t, "to_y_channel", a, nbytes=batch * H * W * (channels * t.element_size() + 4))
+    return out
+
+
+def psnr_sums(t, src1, src2, batch, H, W, channels, y_channel):
+    """-> (mse, max of image 1, psnr), three (batch,) float64 tensors on t's device (vmb_psnr)"""
+    out = torch.empty((3, batch), dtype=torch.float64, device=t.device)
+    a = _lib.PsnrArgs(img1=src1, img2=src2, batch=batch, H=H, W=W, channels=channels, y_channel=int(y_channel),
+                      mse=_ptr(out[0]), max_value=_ptr(out[1]), psnr=_ptr(out[2]))
+    ws = torch.empty(_lib.lib().vmb_psnr_workspace_bytes(C.byref(a)), dtype=torch.uint8, device=t.device)
+    a.workspace = _ptr(ws)
+    _run("vmb_psnr", t, "psnr", a, nbytes=2 * batch * H * W * channels * t.element_size(), kernels=2)
+    return out[0], out[1], out[2]
+
+
+def ssim_mean(t, src1, src2, batch, H, W, channels, y_channel, mode, taps, mix=None, max_value=None):
+    """-> (batch,) float64: the mean SSIM map of each pair (vmb_ssim; mode a key of SSIM_MODES; taps: 11 floats; mix: the
+    channels x channels filter across channels of 'replicate3d', with max_value (batch,) float64 for its constants)"""
+    out = torch.empty(batch, dtype=torch.float64, device=t.device)
+    mix9 = [0.0] * 9
+    for i, v in enumerate([] if mix is None else [v for row in mix for v in row]):
+        mix9[i] = float(v)
+    a = _lib.SsimArgs(img1=src1, img2=src2, batch=batch, H=H, W=W, channels=channels, y_channel=int(y_channel), mode=SSIM_MODES[mode],
+                      taps=(C.c_double * 11)(*taps), mix=(C.c_double * 9)(*mix9), max_value=_ptr(max_value), ssim=_ptr(out))
+    ws = torch.empty(_lib.lib().vmb_ssim_workspace_bytes(C.byref(a)), dtype=torch.uint8, device=t.device)
+    a.workspace = _ptr(ws)
+    empty = mode == "valid" and (H <= 10 or W <= 10)  # no map: only the kernel that writes nan runs
+    _run("vmb_ssim", t, "ssim", a, nbytes=2 * batch * H * W * channels * t.element_size(), kernels=1 if empty else 2)
+    return out
