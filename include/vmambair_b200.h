@@ -618,6 +618,80 @@ typedef struct {
 int vmb_ssim(const vmb_ssim_args* a, void* stream);
 int64_t vmb_ssim_workspace_bytes(const vmb_ssim_args* a);
 
+/* ---- degradations: the Real-ESRGAN synthesis operators of basicsr that RealSR/VmambaIR/models/MambaRealSR_model.py:145-260 uses --
+ * Every image is float32 NCHW, contiguous: `batch` images of `channels` planes of H x W.  Nothing reads the host. */
+
+/* filter2D (basicsr.utils.img_process_util): out = the k x k cross-correlation of each plane with `kernel` (k x k float32, one shared
+ * kernel, per_image = 0, or one per image, per_image = 1, (batch, k, k)), pads of k / 2 with torch's 'reflect' semantics.  k odd,
+ * 1..51; H and W > k / 2 (where torch's reflect pad works).  quantize_out: out = clamp(rint(v 255), 0, 255) / 255. */
+typedef struct {
+    const float* img;
+    float* out;
+    const float* kernel;
+    int batch, channels, H, W, k, per_image, quantize_out;
+} vmb_filter2d_args;
+int vmb_filter2d(const vmb_filter2d_args* a, void* stream);
+
+/* USMSharp(radius).forward(img, weight, threshold) (basicsr.utils.img_process_util) with the separable kernel taps x taps^T (taps:
+ * cv2.getGaussianKernel(k, sigma) in float32, k odd <= 51): blur = G * img, residual = img - blur,
+ * mask = |residual| 255 > threshold, soft = G * mask, out = soft clip(img + weight residual, 0, 1) + (1 - soft) img.  Two launches;
+ * workspace: batch channels H W floats (the mask).  img, out and workspace must not alias. */
+typedef struct {
+    const float* img;
+    float* out;
+    float* workspace;
+    int batch, channels, H, W, k;
+    float taps[51];
+    float weight, threshold;
+} vmb_usm_sharp_args;
+int vmb_usm_sharp(const vmb_usm_sharp_args* a, void* stream);
+
+/* DiffJPEG(differentiable=False)(img, quality) (basicsr.utils.diffjpeg) of 3-channel RGB images in [0, 1]: zero pads to multiples of
+ * 16, x 255, YCbCr (JFIF matrix, shift 128), 4:2:0 by 2 x 2 averages, orthonormal 8 x 8 DCT-II, rint(D / (T factor)) (T factor) with
+ * basicsr's transposed tables, inverse DCT, chroma repeated 2 x 2, back to RGB, clamped to [0, 255], / 255, cropped.  One CTA per four
+ * 16 x 16 MCUs.  quality: (batch,) device float32, factor = (q < 50 ? 5000 / q : 200 - 2 q) / 100 per image in float32 (not
+ * modified); NULL: the host-computed `factor` for every image.  A zero step (quality 100) keeps the coefficient: the lossless limit.
+ * clamp_in: clamp(img, 0, 1) on load.  quantize_out: as in vmb_filter2d_args. */
+typedef struct {
+    const float* img;
+    float* out;
+    const float* quality;
+    float factor;
+    int batch, H, W, clamp_in, quantize_out;
+} vmb_jpeg_args;
+int vmb_jpeg(const vmb_jpeg_args* a, void* stream);
+
+/* The levels of generate_poisson_noise_pt (basicsr.data.degradations) of 3-channel images, without a host read: q = clamp(rint(x 255),
+ * 0, 255) / 255 per element and qg the same of torchvision's gray 0.2989 r + 0.587 g + 0.114 b (separate float32 roundings);
+ * vals[b] = 2^ceil(log2(distinct q of image b)), vals_gray[b] likewise of qg (256-bit presence masks, atomicOr: deterministic);
+ * rates = q vals (batch, 3, H, W), rates_gray = qg vals_gray (batch, 1, H, W).  workspace: 64 batch bytes. */
+typedef struct {
+    const float* img;
+    float *rates, *rates_gray, *vals, *vals_gray;
+    void* workspace;
+    int batch, H, W;
+} vmb_noise_levels_args;
+int vmb_noise_levels(const vmb_noise_levels_args* a, void* stream);
+
+/* out = img + noise of random_add_gaussian_noise_pt / random_add_poisson_noise_pt, from torch's draws:
+ *   param[b] = u_param[b] param_span + param_lo (sigma or scale), g[b] = (u_gray[b] < gray_prob);
+ *   GAUSSIAN: noise = randn(b, c, H, W) sigma / 255, noise_gray = randn(H, W) sigma / 255, mixed noise (1 - g) + noise_gray g;
+ *   POISSON (3 channels): noise = P / vals - q, noise_gray = Pg / vals_gray - qg (P, Pg: torch.poisson of vmb_noise_levels' rates,
+ *            rates_gray), mixed as above, times scale.
+ * Then clip and rounds as the reference: clamp(rint(v 255), 0, 255) / 255, clamp(v, 0, 1), or rint(v 255) / 255.  Every operation is
+ * one float32 rounding, in the reference's order.  out must not alias img. */
+#define VMB_NOISE_GAUSSIAN 0
+#define VMB_NOISE_POISSON 1
+typedef struct {
+    const float* img;
+    float* out;
+    const float *noise, *noise_gray, *u_param, *u_gray;
+    float param_lo, param_span, gray_prob;
+    const float *vals, *vals_gray;
+    int kind, batch, channels, H, W, clip, rounds;
+} vmb_noise_apply_args;
+int vmb_noise_apply(const vmb_noise_apply_args* a, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

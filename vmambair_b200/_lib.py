@@ -288,6 +288,38 @@ class SsimArgs(C.Structure):
                 ("ssim", vp), ("workspace", vp)]
 
 
+class Filter2dArgs(C.Structure):
+    _c_name_ = "vmb_filter2d_args"
+    _fields_ = [("img", vp), ("out", vp), ("kernel", vp), ("batch", C.c_int), ("channels", C.c_int), ("H", C.c_int), ("W", C.c_int),
+                ("k", C.c_int), ("per_image", C.c_int), ("quantize_out", C.c_int)]
+
+
+class UsmSharpArgs(C.Structure):
+    _c_name_ = "vmb_usm_sharp_args"
+    _fields_ = [("img", vp), ("out", vp), ("workspace", vp), ("batch", C.c_int), ("channels", C.c_int), ("H", C.c_int), ("W", C.c_int),
+                ("k", C.c_int), ("taps", C.c_float * 51), ("weight", C.c_float), ("threshold", C.c_float)]
+
+
+class JpegArgs(C.Structure):
+    _c_name_ = "vmb_jpeg_args"
+    _fields_ = [("img", vp), ("out", vp), ("quality", vp), ("factor", C.c_float), ("batch", C.c_int), ("H", C.c_int), ("W", C.c_int),
+                ("clamp_in", C.c_int), ("quantize_out", C.c_int)]
+
+
+class NoiseLevelsArgs(C.Structure):
+    _c_name_ = "vmb_noise_levels_args"
+    _fields_ = [("img", vp), ("rates", vp), ("rates_gray", vp), ("vals", vp), ("vals_gray", vp), ("workspace", vp),
+                ("batch", C.c_int), ("H", C.c_int), ("W", C.c_int)]
+
+
+class NoiseApplyArgs(C.Structure):
+    _c_name_ = "vmb_noise_apply_args"
+    _fields_ = [("img", vp), ("out", vp), ("noise", vp), ("noise_gray", vp), ("u_param", vp), ("u_gray", vp),
+                ("param_lo", C.c_float), ("param_span", C.c_float), ("gray_prob", C.c_float), ("vals", vp), ("vals_gray", vp),
+                ("kind", C.c_int), ("batch", C.c_int), ("channels", C.c_int), ("H", C.c_int), ("W", C.c_int), ("clip", C.c_int),
+                ("rounds", C.c_int)]
+
+
 # every symbol include/vmambair_b200.h declares: name -> (restype, argtypes)
 SYMBOLS = {
     "vmb_last_error": (C.c_char_p, []),
@@ -340,6 +372,11 @@ SYMBOLS = {
     "vmb_psnr_workspace_bytes": (C.c_int64, [C.POINTER(PsnrArgs)]),
     "vmb_ssim": (C.c_int, [C.POINTER(SsimArgs), vp]),
     "vmb_ssim_workspace_bytes": (C.c_int64, [C.POINTER(SsimArgs)]),
+    "vmb_filter2d": (C.c_int, [C.POINTER(Filter2dArgs), vp]),
+    "vmb_usm_sharp": (C.c_int, [C.POINTER(UsmSharpArgs), vp]),
+    "vmb_jpeg": (C.c_int, [C.POINTER(JpegArgs), vp]),
+    "vmb_noise_levels": (C.c_int, [C.POINTER(NoiseLevelsArgs), vp]),
+    "vmb_noise_apply": (C.c_int, [C.POINTER(NoiseApplyArgs), vp]),
 }
 
 

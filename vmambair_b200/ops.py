@@ -953,3 +953,64 @@ def ssim_mean(t, src1, src2, batch, H, W, channels, y_channel, mode, taps, mix=N
     empty = mode == "valid" and (H <= 10 or W <= 10)  # no map: only the kernel that writes nan runs
     _run("vmb_ssim", t, "ssim", a, nbytes=2 * batch * H * W * channels * t.element_size(), kernels=1 if empty else 2)
     return out
+
+
+# ---- degradations (csrc/degrade.cu): basicsr's Real-ESRGAN synthesis operators; float32 NCHW, contiguous, nothing read on the host ----
+NOISE_GAUSSIAN, NOISE_POISSON = 0, 1  # VMB_NOISE_*
+
+
+def filter2d(img, kernel, per_image, quantize_out=False):
+    """(b, c, H, W) img cross-correlated with the (k, k) kernel(s) `kernel` ((1, k, k) shared or (b, k, k) per image), reflect pads"""
+    b, c, H, W = img.shape
+    k = kernel.shape[-1]
+    out = torch.empty_like(img)
+    a = _lib.Filter2dArgs(img=_ptr(img), out=_ptr(out), kernel=_ptr(kernel), batch=b, channels=c, H=H, W=W, k=k,
+                          per_image=int(per_image), quantize_out=int(quantize_out))
+    _run("vmb_filter2d", img, "filter2d", a, nbytes=2 * img.numel() * 4)
+    return out
+
+
+def usm_sharp(img, taps, weight, threshold):
+    """USMSharp of (b, c, H, W) img with the separable kernel outer(taps, taps)"""
+    b, c, H, W = img.shape
+    out, ws = torch.empty_like(img), torch.empty_like(img)
+    a = _lib.UsmSharpArgs(img=_ptr(img), out=_ptr(out), workspace=_ptr(ws), batch=b, channels=c, H=H, W=W, k=len(taps),
+                          taps=(C.c_float * 51)(*taps), weight=float(weight), threshold=float(threshold))
+    _run("vmb_usm_sharp", img, "usm_sharp", a, nbytes=7 * img.numel() * 4, kernels=2)
+    return out
+
+
+def jpeg(img, quality=None, factor=0.0, clamp_in=False, quantize_out=False):
+    """DiffJPEG(differentiable=False) of (b, 3, H, W) img: quality a (b,) float32 device tensor, or None and the scalar `factor`"""
+    b, _, H, W = img.shape
+    out = torch.empty_like(img)
+    a = _lib.JpegArgs(img=_ptr(img), out=_ptr(out), quality=_ptr(quality), factor=float(factor), batch=b, H=H, W=W,
+                      clamp_in=int(clamp_in), quantize_out=int(quantize_out))
+    _run("vmb_jpeg", img, "jpeg", a, nbytes=2 * img.numel() * 4)
+    return out
+
+
+def noise_levels(img):
+    """-> (rates (b, 3, H, W), rates_gray (b, 1, H, W), vals (b,), vals_gray (b,)) of generate_poisson_noise_pt, on the device"""
+    b, _, H, W = img.shape
+    rates = torch.empty_like(img)
+    rates_gray = torch.empty((b, 1, H, W), dtype=torch.float32, device=img.device)
+    vals = torch.empty((2, b), dtype=torch.float32, device=img.device)
+    ws = torch.empty(64 * b, dtype=torch.uint8, device=img.device)
+    a = _lib.NoiseLevelsArgs(img=_ptr(img), rates=_ptr(rates), rates_gray=_ptr(rates_gray), vals=_ptr(vals[0]), vals_gray=_ptr(vals[1]),
+                             workspace=_ptr(ws), batch=b, H=H, W=W)
+    _run("vmb_noise_levels", img, "noise_levels", a, nbytes=(2 * img.numel() + rates.numel() + rates_gray.numel()) * 4, kernels=2)
+    return rates, rates_gray, vals[0], vals[1]
+
+
+def noise_apply(img, kind, noise, noise_gray, u_param, u_gray, param_range, gray_prob, clip, rounds, vals=None, vals_gray=None):
+    """img + the Gaussian / Poisson noise of basicsr from torch's draws (vmb_noise_apply_args); -> a new tensor"""
+    b, c, H, W = img.shape
+    out = torch.empty_like(img)
+    lo, hi = param_range
+    a = _lib.NoiseApplyArgs(img=_ptr(img), out=_ptr(out), noise=_ptr(noise), noise_gray=_ptr(noise_gray), u_param=_ptr(u_param),
+                            u_gray=_ptr(u_gray), param_lo=float(lo), param_span=float(hi - lo), gray_prob=float(gray_prob),
+                            vals=_ptr(vals), vals_gray=_ptr(vals_gray), kind=kind, batch=b, channels=c, H=H, W=W, clip=int(clip),
+                            rounds=int(rounds))
+    _run("vmb_noise_apply", img, "noise_apply", a, nbytes=(3 * img.numel() + noise_gray.numel()) * 4)
+    return out
