@@ -692,6 +692,115 @@ typedef struct {
 } vmb_noise_apply_args;
 int vmb_noise_apply(const vmb_noise_apply_args* a, void* stream);
 
+/* ---- GAN stage: UNetDiscriminatorSN (RealSR/VmambaIR/archs/discriminator_arch.py:19-67) between its convolutions, and basicsr's
+ * vanilla GANLoss (MambaRealSRGAN_model.py:289-359 calls both).  Activations are NCHW contiguous, fp32 or bf16 (dtype VMB_F32 /
+ * VMB_BF16); all math is fp32.  No atomics: every reduction has one fixed order, so results are bitwise reproducible. */
+
+/* torch.nn.utils.spectral_norm (dim 0, one power iteration) of up to VMB_SN_MAX_LAYERS layers in one call (discriminator_arch.py:
+ * 28-38 wraps conv1..conv8).  Layer i: w[i] = weight_orig viewed as (rows[i], cols[i]) fp32; u[i] (rows), v[i] (cols) fp32.
+ *   train = 1: v = normalize(W^T u), u = normalize(W v) (normalize(x) = x / max(|x|, eps)), written back to u[i], v[i];
+ *   train = 0: u, v as stored.
+ * Then sigma[i] = u . (W v), wn[i] = W / sigma[i] in `dtype`, and the u, v used are copied to u_save[i], v_save[i] (the backward's
+ * constants).  Four launches in train mode, two in eval mode, whatever the layer count.
+ * workspace: vmb_sn_workspace_bytes(layers, rows, cols) bytes; columns <= 56 K (v is staged in shared memory). */
+#define VMB_SN_MAX_LAYERS 8
+typedef struct {
+    const float* w[VMB_SN_MAX_LAYERS];
+    void* wn[VMB_SN_MAX_LAYERS];
+    float* u[VMB_SN_MAX_LAYERS];
+    float* v[VMB_SN_MAX_LAYERS];
+    float* u_save[VMB_SN_MAX_LAYERS];
+    float* v_save[VMB_SN_MAX_LAYERS];
+    int rows[VMB_SN_MAX_LAYERS], cols[VMB_SN_MAX_LAYERS];
+    float* sigma;
+    void* workspace;
+    int layers, train, dtype;
+    float eps;
+} vmb_sn_fwd_args;
+int vmb_sn_fwd(const vmb_sn_fwd_args* a, void* stream);
+int64_t vmb_sn_workspace_bytes(int layers, const int* rows, const int* cols);
+
+/* Backward of vmb_sn_fwd with u, v constant (as spectral_norm's clones): g[i] = dL/dwn (dtype), then
+ * dW_orig = g / sigma - (<g, W_orig> / sigma^2) u v^T, written to grad[i] (fp32), or added to it where accumulate[i] != 0 (the
+ * .grad accumulation of the parameter).  Two launches: per-chunk partials of <g, W_orig>, then the update, which adds each
+ * layer's partials in index order.  workspace: vmb_sn_bwd_workspace_bytes(layers, rows, cols) bytes. */
+typedef struct {
+    const void* g[VMB_SN_MAX_LAYERS];
+    const float* w[VMB_SN_MAX_LAYERS];
+    const float* u[VMB_SN_MAX_LAYERS];
+    const float* v[VMB_SN_MAX_LAYERS];
+    float* grad[VMB_SN_MAX_LAYERS];
+    int rows[VMB_SN_MAX_LAYERS], cols[VMB_SN_MAX_LAYERS], accumulate[VMB_SN_MAX_LAYERS];
+    const float* sigma;
+    void* workspace;
+    int layers, dtype;
+} vmb_sn_bwd_args;
+int vmb_sn_bwd(const vmb_sn_bwd_args* a, void* stream);
+int64_t vmb_sn_bwd_workspace_bytes(int layers, const int* rows, const int* cols);
+
+/* Decoder junction (discriminator_arch.py:49-56): out = F.interpolate(leaky_relu(pre, 0.2) [+ skip], scale_factor=2,
+ * mode='bilinear', align_corners=False) of `planes` planes of H x W into 2H x 2W; weights 0.75 / 0.25 with clamped borders, in
+ * torch's order of operations.  skip: NULL for none. */
+typedef struct {
+    const void *pre, *skip;
+    void* out;
+    int planes, H, W, dtype;
+} vmb_gan_up_args;
+int vmb_gan_up(const vmb_gan_up_args* a, void* stream);
+
+/* Its backward: adj = up2^T(dout) as a gather (each input element sums its 4 x 4 output neighbourhood in a fixed order; torch's
+ * upsample_bilinear2d_backward scatters with atomics), dskip = adj (NULL: not written), dpre = adj leaky'(pre). */
+typedef struct {
+    const void *dout, *pre;
+    void *dpre, *dskip;
+    int planes, H, W, dtype;
+} vmb_gan_up_bwd_args;
+int vmb_gan_up_bwd(const vmb_gan_up_bwd_args* a, void* stream);
+
+/* Encoder activation (discriminator_arch.py:42-45, 59-63): out = leaky_relu(x, 0.2) [+ skip] over n elements; out may be x. */
+typedef struct {
+    const void *x, *skip;
+    void* out;
+    int64_t n;
+    int dtype;
+} vmb_gan_act_args;
+int vmb_gan_act(const vmb_gan_act_args* a, void* stream);
+
+/* Its backward: dx = (g [+ g2]) leaky'(ref), ref the pre-activation or the in-place result (same sign); g2 NULL for none, dx may
+ * be g.  At x0, x1, x2 g2 is the skip connection's gradient, so the sum is never stored. */
+typedef struct {
+    const void *g, *g2, *ref;
+    void* dx;
+    int64_t n;
+    int dtype;
+} vmb_gan_act_bwd_args;
+int vmb_gan_act_bwd(const vmb_gan_act_bwd_args* a, void* stream);
+
+/* basicsr GANLoss(gan_type='vanilla'): *loss = weight mean(BCEWithLogits(x, target)) over n logits, per element
+ * max(x, 0) - x target + log1p(exp(-|x|)).  Per-CTA partials, then one CTA adds them in order.
+ * workspace: vmb_bce_logits_workspace_bytes(n) bytes. */
+typedef struct {
+    const void* x;
+    float* loss;
+    void* workspace;
+    int64_t n;
+    float target, weight;
+    int dtype;
+} vmb_bce_logits_args;
+int vmb_bce_logits(const vmb_bce_logits_args* a, void* stream);
+int64_t vmb_bce_logits_workspace_bytes(int64_t n);
+
+/* Its backward: grad_x = grad_loss weight (sigmoid(x) - target) / n, grad_loss read from the device (fp32 scalar). */
+typedef struct {
+    const void* x;
+    const float* grad_loss;
+    void* grad_x;
+    int64_t n;
+    float target, weight;
+    int dtype;
+} vmb_bce_logits_bwd_args;
+int vmb_bce_logits_bwd(const vmb_bce_logits_bwd_args* a, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

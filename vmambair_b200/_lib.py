@@ -320,6 +320,57 @@ class NoiseApplyArgs(C.Structure):
                 ("rounds", C.c_int)]
 
 
+SN_MAX_LAYERS = 8  # VMB_SN_MAX_LAYERS
+
+
+class SnFwdArgs(C.Structure):
+    _c_name_ = "vmb_sn_fwd_args"
+    _fields_ = [("w", vp * SN_MAX_LAYERS), ("wn", vp * SN_MAX_LAYERS), ("u", vp * SN_MAX_LAYERS), ("v", vp * SN_MAX_LAYERS),
+                ("u_save", vp * SN_MAX_LAYERS), ("v_save", vp * SN_MAX_LAYERS), ("rows", C.c_int * SN_MAX_LAYERS),
+                ("cols", C.c_int * SN_MAX_LAYERS), ("sigma", vp), ("workspace", vp), ("layers", C.c_int), ("train", C.c_int),
+                ("dtype", C.c_int), ("eps", C.c_float)]
+
+
+class SnBwdArgs(C.Structure):
+    _c_name_ = "vmb_sn_bwd_args"
+    _fields_ = [("g", vp * SN_MAX_LAYERS), ("w", vp * SN_MAX_LAYERS), ("u", vp * SN_MAX_LAYERS), ("v", vp * SN_MAX_LAYERS),
+                ("grad", vp * SN_MAX_LAYERS), ("rows", C.c_int * SN_MAX_LAYERS), ("cols", C.c_int * SN_MAX_LAYERS),
+                ("accumulate", C.c_int * SN_MAX_LAYERS), ("sigma", vp), ("workspace", vp), ("layers", C.c_int), ("dtype", C.c_int)]
+
+
+class GanUpArgs(C.Structure):
+    _c_name_ = "vmb_gan_up_args"
+    _fields_ = [("pre", vp), ("skip", vp), ("out", vp), ("planes", C.c_int), ("H", C.c_int), ("W", C.c_int), ("dtype", C.c_int)]
+
+
+class GanUpBwdArgs(C.Structure):
+    _c_name_ = "vmb_gan_up_bwd_args"
+    _fields_ = [("dout", vp), ("pre", vp), ("dpre", vp), ("dskip", vp), ("planes", C.c_int), ("H", C.c_int), ("W", C.c_int),
+                ("dtype", C.c_int)]
+
+
+class GanActArgs(C.Structure):
+    _c_name_ = "vmb_gan_act_args"
+    _fields_ = [("x", vp), ("skip", vp), ("out", vp), ("n", i64), ("dtype", C.c_int)]
+
+
+class GanActBwdArgs(C.Structure):
+    _c_name_ = "vmb_gan_act_bwd_args"
+    _fields_ = [("g", vp), ("g2", vp), ("ref", vp), ("dx", vp), ("n", i64), ("dtype", C.c_int)]
+
+
+class BceLogitsArgs(C.Structure):
+    _c_name_ = "vmb_bce_logits_args"
+    _fields_ = [("x", vp), ("loss", vp), ("workspace", vp), ("n", i64), ("target", C.c_float), ("weight", C.c_float),
+                ("dtype", C.c_int)]
+
+
+class BceLogitsBwdArgs(C.Structure):
+    _c_name_ = "vmb_bce_logits_bwd_args"
+    _fields_ = [("x", vp), ("grad_loss", vp), ("grad_x", vp), ("n", i64), ("target", C.c_float), ("weight", C.c_float),
+                ("dtype", C.c_int)]
+
+
 # every symbol include/vmambair_b200.h declares: name -> (restype, argtypes)
 SYMBOLS = {
     "vmb_last_error": (C.c_char_p, []),
@@ -377,6 +428,17 @@ SYMBOLS = {
     "vmb_jpeg": (C.c_int, [C.POINTER(JpegArgs), vp]),
     "vmb_noise_levels": (C.c_int, [C.POINTER(NoiseLevelsArgs), vp]),
     "vmb_noise_apply": (C.c_int, [C.POINTER(NoiseApplyArgs), vp]),
+    "vmb_sn_fwd": (C.c_int, [C.POINTER(SnFwdArgs), vp]),
+    "vmb_sn_workspace_bytes": (C.c_int64, [C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "vmb_sn_bwd": (C.c_int, [C.POINTER(SnBwdArgs), vp]),
+    "vmb_sn_bwd_workspace_bytes": (C.c_int64, [C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "vmb_gan_up": (C.c_int, [C.POINTER(GanUpArgs), vp]),
+    "vmb_gan_up_bwd": (C.c_int, [C.POINTER(GanUpBwdArgs), vp]),
+    "vmb_gan_act": (C.c_int, [C.POINTER(GanActArgs), vp]),
+    "vmb_gan_act_bwd": (C.c_int, [C.POINTER(GanActBwdArgs), vp]),
+    "vmb_bce_logits": (C.c_int, [C.POINTER(BceLogitsArgs), vp]),
+    "vmb_bce_logits_workspace_bytes": (C.c_int64, [C.c_int64]),
+    "vmb_bce_logits_bwd": (C.c_int, [C.POINTER(BceLogitsBwdArgs), vp]),
 }
 
 

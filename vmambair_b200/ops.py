@@ -1014,3 +1014,111 @@ def noise_apply(img, kind, noise, noise_gray, u_param, u_gray, param_range, gray
                             rounds=int(rounds))
     _run("vmb_noise_apply", img, "noise_apply", a, nbytes=(3 * img.numel() + noise_gray.numel()) * 4)
     return out
+
+
+# ---- GAN stage (csrc/gan.cu): UNetDiscriminatorSN between its convolutions and the vanilla GAN loss; fp32 or bf16 activations,
+# contiguous; every reduction in a fixed order (bitwise reproducible), nothing read on the host ----
+def _gan_dt(t):
+    if t.dtype not in (torch.float32, torch.bfloat16):
+        raise ValueError(f"the GAN kernels take float32 or bfloat16 tensors, not {t.dtype}")
+    return _DT[t.dtype]
+
+
+def _rows_cols(ws):
+    n = len(ws)
+    rows, cols = (C.c_int * _lib.SN_MAX_LAYERS)(), (C.c_int * _lib.SN_MAX_LAYERS)()
+    for i, w in enumerate(ws):
+        rows[i], cols[i] = w.shape[0], w[0].numel()
+    return n, rows, cols
+
+
+def spectral_norm(ws, us, vs, train, dtype, eps=1e-12):
+    """torch.nn.utils.spectral_norm of the fp32 weights `ws` (weight_orig, contiguous) with their u / v buffers `us` / `vs`, all
+    layers in one call: train advances u and v in place.  -> (W / sigma per layer in `dtype`, sigma (layers,), the u and v used)"""
+    n, rows, cols = _rows_cols(ws)
+    dev = ws[0].device
+    wn_flat = torch.empty(sum(w.numel() for w in ws), dtype=dtype, device=dev)
+    uv_flat = torch.empty(sum(rows[:n]) + sum(cols[:n]), dtype=torch.float32, device=dev)
+    sigma = torch.empty(n, dtype=torch.float32, device=dev)
+    ws_bytes = _lib.lib().vmb_sn_workspace_bytes(n, rows, cols)
+    work = torch.empty(ws_bytes // 4, dtype=torch.float32, device=dev)
+    wns, us_save, vs_save, o, ouv = [], [], [], 0, 0
+    for i, w in enumerate(ws):
+        wns.append(wn_flat[o:o + w.numel()].view(w.shape))
+        us_save.append(uv_flat[ouv:ouv + rows[i]])
+        vs_save.append(uv_flat[ouv + rows[i]:ouv + rows[i] + cols[i]])
+        o, ouv = o + w.numel(), ouv + rows[i] + cols[i]
+    P = lambda ts: (C.c_void_p * _lib.SN_MAX_LAYERS)(*[t.data_ptr() for t in ts])
+    a = _lib.SnFwdArgs(w=P(ws), wn=P(wns), u=P(us), v=P(vs), u_save=P(us_save), v_save=P(vs_save), rows=rows, cols=cols,
+                       sigma=_ptr(sigma), workspace=_ptr(work), layers=n, train=int(train), dtype=_gan_dt(wn_flat), eps=float(eps))
+    _run("vmb_sn_fwd", ws[0], "sn_fwd", a, nbytes=(2 if train else 1) * 4 * o + wn_flat.numel() * wn_flat.element_size(),
+         kernels=4 if train else 2)
+    return wns, sigma, us_save, vs_save
+
+
+def spectral_norm_bwd(gs, ws, us, vs, sigma, grads, accumulate):
+    """dW_orig of every layer of `spectral_norm` from the gradients `gs` of its outputs W / sigma (u, v, sigma: the saved ones),
+    written to the fp32 tensors `grads`, or added to those where accumulate[i]"""
+    n, rows, cols = _rows_cols(ws)
+    work = torch.empty(_lib.lib().vmb_sn_bwd_workspace_bytes(n, rows, cols) // 4, dtype=torch.float32, device=ws[0].device)
+    P = lambda ts: (C.c_void_p * _lib.SN_MAX_LAYERS)(*[t.data_ptr() for t in ts])
+    acc = (C.c_int * _lib.SN_MAX_LAYERS)(*map(int, accumulate))
+    a = _lib.SnBwdArgs(g=P(gs), w=P(ws), u=P(us), v=P(vs), grad=P(grads), rows=rows, cols=cols, accumulate=acc, sigma=_ptr(sigma),
+                       workspace=_ptr(work), layers=n, dtype=_gan_dt(gs[0]))
+    nel = sum(w.numel() for w in ws)
+    _run("vmb_sn_bwd", ws[0], "sn_bwd", a, nbytes=nel * (2 * gs[0].element_size() + 4 * 4), kernels=2)
+
+
+def gan_up(pre, skip=None):
+    """F.interpolate(leaky_relu(pre, 0.2) [+ skip], scale_factor=2, mode='bilinear', align_corners=False) of (b, c, h, w) tensors"""
+    b, c, h, w = pre.shape
+    out = torch.empty((b, c, 2 * h, 2 * w), dtype=pre.dtype, device=pre.device)
+    a = _lib.GanUpArgs(pre=_ptr(pre), skip=_ptr(skip), out=_ptr(out), planes=b * c, H=h, W=w, dtype=_gan_dt(pre))
+    _run("vmb_gan_up", pre, "gan_up", a, nbytes=(pre.numel() * (2 if skip is not None else 1) + out.numel()) * pre.element_size())
+    return out
+
+
+def gan_up_bwd(dout, pre, want_skip):
+    """-> (dpre, dskip or None) of gan_up from its output gradient: the adjoint of up2 gathered, times leaky'(pre) for dpre"""
+    b, c, h, w = pre.shape
+    dpre = torch.empty_like(pre)
+    dskip = torch.empty_like(pre) if want_skip else None
+    a = _lib.GanUpBwdArgs(dout=_ptr(dout), pre=_ptr(pre), dpre=_ptr(dpre), dskip=_ptr(dskip), planes=b * c, H=h, W=w, dtype=_gan_dt(pre))
+    _run("vmb_gan_up_bwd", pre, "gan_up_bwd", a, nbytes=(dout.numel() + pre.numel() * (3 if want_skip else 2)) * pre.element_size())
+    return dpre, dskip
+
+
+def gan_act(x, skip=None, out=None):
+    """leaky_relu(x, 0.2) [+ skip] into `out` (default: x itself, in place)"""
+    out = x if out is None else out
+    a = _lib.GanActArgs(x=_ptr(x), skip=_ptr(skip), out=_ptr(out), n=x.numel(), dtype=_gan_dt(x))
+    _run("vmb_gan_act", x, "gan_act", a, nbytes=x.numel() * x.element_size() * (3 if skip is not None else 2))
+    return out
+
+
+def gan_act_bwd(g, ref, g2=None, out=None):
+    """(g [+ g2]) * leaky'(ref) into `out` (default: g itself, in place)"""
+    out = g if out is None else out
+    a = _lib.GanActBwdArgs(g=_ptr(g), g2=_ptr(g2), ref=_ptr(ref), dx=_ptr(out), n=g.numel(), dtype=_gan_dt(g))
+    _run("vmb_gan_act_bwd", g, "gan_act_bwd", a, nbytes=g.numel() * g.element_size() * (4 if g2 is not None else 3))
+    return out
+
+
+def bce_logits(x, target, weight):
+    """weight * mean(BCEWithLogits(x, full_like(x, target))) -> 0-dim float32 tensor"""
+    n = x.numel()
+    loss = torch.empty((), dtype=torch.float32, device=x.device)
+    work = torch.empty(_lib.lib().vmb_bce_logits_workspace_bytes(n) // 4, dtype=torch.float32, device=x.device)
+    a = _lib.BceLogitsArgs(x=_ptr(x), loss=_ptr(loss), workspace=_ptr(work), n=n, target=float(target), weight=float(weight),
+                           dtype=_gan_dt(x))
+    _run("vmb_bce_logits", x, "bce_logits", a, nbytes=n * x.element_size(), kernels=2)
+    return loss
+
+
+def bce_logits_bwd(x, grad_loss, target, weight):
+    """gradient of bce_logits with respect to x, for the upstream 0-dim float32 gradient grad_loss (read on the device)"""
+    gx = torch.empty_like(x)
+    a = _lib.BceLogitsBwdArgs(x=_ptr(x), grad_loss=_ptr(grad_loss), grad_x=_ptr(gx), n=x.numel(), target=float(target),
+                              weight=float(weight), dtype=_gan_dt(x))
+    _run("vmb_bce_logits_bwd", x, "bce_logits_bwd", a, nbytes=2 * x.numel() * x.element_size())
+    return gx
