@@ -801,6 +801,91 @@ typedef struct {
 } vmb_bce_logits_bwd_args;
 int vmb_bce_logits_bwd(const vmb_bce_logits_bwd_args* a, void* stream);
 
+/* ---- Perceptual loss: basicsr's PerceptualLoss (losses/basic_loss.py) on VGGFeatureExtractor (archs/vgg_arch.py), the generator
+ * step's perceptual_opt of both GAN recipes, between its convolutions.  It replaces the extractor's ReLU and MaxPool2d modules, the
+ * feature clone()s, the subtractions and the L1Loss / MSELoss / torch.norm of every feature, and their autograd backward.  The
+ * output x and the ground truth gt run as one 2B batch: images 0..B-1 are x's, B..2B-1 gt's.  Activations are NCHW contiguous,
+ * fp32 or bf16 (dtype VMB_F32 / VMB_BF16); all math is fp32.  No atomics: every reduction has one fixed order. */
+#define VMB_PERCEP_L1 0  /* criterion 'l1': mean |d| */
+#define VMB_PERCEP_L2 1  /* 'l2': mean d^2 */
+#define VMB_PERCEP_FRO 2 /* 'fro': sqrt(sum d^2) */
+#define VMB_PERCEP_MAX_FEATS 37 /* every layer name of vgg19 */
+
+/* The extractor's input (vgg_arch.py forward, range_norm then use_input_norm): out[b] = norm(x[b]), out[B + b] = norm(gt[b]) with
+ * norm(v) = ((v + 1) / 2 - mean[c]) / std[c], the first step only when range_norm, the second only when mean / std are given (the
+ * module's fp32 buffers, read on the device; NULL for neither).  x, gt: fp32 (B, 3, H, W) through element strides; out (2B, 3, H, W). */
+typedef struct {
+    const float *x, *gt;
+    int64_t x_stride[4], gt_stride[4];
+    const float *mean, *std;
+    void* out;
+    int B, H, W, range_norm, dtype;
+} vmb_percep_norm_args;
+int vmb_percep_norm(const vmb_percep_norm_args* a, void* stream);
+
+/* Its backward for x: dx = g / std[c] (when std), then / 2 (when range_norm); g (B, 3, H, W) dtype, dx fp32 contiguous. */
+typedef struct {
+    const void* g;
+    float* dx;
+    const float* std;
+    int B, H, W, range_norm, dtype;
+} vmb_percep_norm_bwd_args;
+int vmb_percep_norm_bwd(const vmb_percep_norm_bwd_args* a, void* stream);
+
+/* One stage after a convolution: y (2B, C, H, W) is the conv output (with bias).  Three feature sites: 0 conv (y before the ReLU;
+ * basicsr clones it because the ReLU is in place), 1 relu (after it), 2 pool (after MaxPool2d(2, 2), floor sizes, the first maximum
+ * of the row-major window wins).  feat[k] != 0: site k is a feature, and partial[k][cta] receives the CTA's sum of |d| (l1) or d^2
+ * (l2, fro) of d = x half - gt half there, vmb_percep_stage_ctas(B, C, H, W) CTAs.
+ * relu: y = max(y, 0) in place (not written back when pool: only the pooled tensor is read again); pool: pooled (2B, C, H/2, W/2).
+ * Saved for the backward, x half only, per 2 x 2 cell of ceil(H/2) x ceil(W/2): code[cell] bits 0-3 = [y > 0] of the cell's
+ * elements in row-major order, bits 4-5 the pool argmax (code NULL: nothing saved).  save[k] (NULL: nothing saved) for l1 a byte per
+ * cell with 2 bits per element (bit 0 d > 0, bit 1 d < 0), at the pool site a byte per pooled element; for l2 / fro d itself in fp32
+ * (the site's x-half shape). */
+typedef struct {
+    void* y;
+    void* pooled;
+    uint8_t* code;
+    void* save[3];
+    float* partial[3];
+    int feat[3];
+    int B, C, H, W, relu, pool, crit, dtype;
+} vmb_percep_stage_args;
+int vmb_percep_stage(const vmb_percep_stage_args* a, void* stream);
+int vmb_percep_stage_ctas(int B, int C, int H, int W);
+
+/* The loss in one CTA: feature k's partials are partial[offset[k] .. offset[k + 1]), added in index order; value[k] = sum / numel[k]
+ * (l1, l2) or sqrt(sum) (fro), and *loss = perceptual_weight * sum_k value[k] weight[k], k ascending (basicsr's order). */
+typedef struct {
+    const float* partial;
+    float* loss;
+    float* value;
+    int offset[VMB_PERCEP_MAX_FEATS + 1];
+    int64_t numel[VMB_PERCEP_MAX_FEATS];
+    float weight[VMB_PERCEP_MAX_FEATS];
+    int feats, crit;
+    float perceptual_weight;
+} vmb_percep_loss_args;
+int vmb_percep_loss(const vmb_percep_loss_args* a, void* stream);
+
+/* Backward of one stage for the x half: g_out (B, C, H, W) = [y > 0] (dpost) + c0 crit'(d at the conv site), where dpost = the
+ * pool adjoint of g_in (+ c2 crit'), a gather through the saved argmax, or g_in itself without a pool, + c1 crit' at the relu site.
+ * g_in: the gradient at the stage's output ((B, C, H/2, W/2) with pool, else (B, C, H, W)); NULL at the deepest stage.
+ * c_k = *grad_loss scale[k] (scale = pw w_k / N_k for l1, 2 pw w_k / N_k for l2, pw w_k for fro), for fro divided by
+ * value[feat_index[k]] (0 where that norm is 0).  grad_loss: the upstream fp32 scalar, read on the device.  Without relu (a stage
+ * cut before its ReLU) the mask is all ones and code may be NULL. */
+typedef struct {
+    const void* g_in;
+    void* g_out;
+    const uint8_t* code;
+    const void* save[3];
+    const float* grad_loss;
+    const float* value;
+    int feat[3], feat_index[3];
+    float scale[3];
+    int B, C, H, W, relu, pool, crit, dtype;
+} vmb_percep_stage_bwd_args;
+int vmb_percep_stage_bwd(const vmb_percep_stage_bwd_args* a, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -371,6 +371,43 @@ class BceLogitsBwdArgs(C.Structure):
                 ("dtype", C.c_int)]
 
 
+PERCEP_L1, PERCEP_L2, PERCEP_FRO = 0, 1, 2  # VMB_PERCEP_L1 / _L2 / _FRO
+PERCEP_MAX_FEATS = 37  # VMB_PERCEP_MAX_FEATS
+
+
+class PercepNormArgs(C.Structure):
+    _c_name_ = "vmb_percep_norm_args"
+    _fields_ = [("x", vp), ("gt", vp), ("x_stride", i64 * 4), ("gt_stride", i64 * 4), ("mean", vp), ("std", vp), ("out", vp),
+                ("B", C.c_int), ("H", C.c_int), ("W", C.c_int), ("range_norm", C.c_int), ("dtype", C.c_int)]
+
+
+class PercepNormBwdArgs(C.Structure):
+    _c_name_ = "vmb_percep_norm_bwd_args"
+    _fields_ = [("g", vp), ("dx", vp), ("std", vp), ("B", C.c_int), ("H", C.c_int), ("W", C.c_int), ("range_norm", C.c_int),
+                ("dtype", C.c_int)]
+
+
+class PercepStageArgs(C.Structure):
+    _c_name_ = "vmb_percep_stage_args"
+    _fields_ = [("y", vp), ("pooled", vp), ("code", vp), ("save", vp * 3), ("partial", vp * 3), ("feat", C.c_int * 3),
+                ("B", C.c_int), ("C", C.c_int), ("H", C.c_int), ("W", C.c_int), ("relu", C.c_int), ("pool", C.c_int),
+                ("crit", C.c_int), ("dtype", C.c_int)]
+
+
+class PercepLossArgs(C.Structure):
+    _c_name_ = "vmb_percep_loss_args"
+    _fields_ = [("partial", vp), ("loss", vp), ("value", vp), ("offset", C.c_int * (PERCEP_MAX_FEATS + 1)),
+                ("numel", i64 * PERCEP_MAX_FEATS), ("weight", C.c_float * PERCEP_MAX_FEATS), ("feats", C.c_int), ("crit", C.c_int),
+                ("perceptual_weight", C.c_float)]
+
+
+class PercepStageBwdArgs(C.Structure):
+    _c_name_ = "vmb_percep_stage_bwd_args"
+    _fields_ = [("g_in", vp), ("g_out", vp), ("code", vp), ("save", vp * 3), ("grad_loss", vp), ("value", vp),
+                ("feat", C.c_int * 3), ("feat_index", C.c_int * 3), ("scale", C.c_float * 3), ("B", C.c_int), ("C", C.c_int),
+                ("H", C.c_int), ("W", C.c_int), ("relu", C.c_int), ("pool", C.c_int), ("crit", C.c_int), ("dtype", C.c_int)]
+
+
 # every symbol include/vmambair_b200.h declares: name -> (restype, argtypes)
 SYMBOLS = {
     "vmb_last_error": (C.c_char_p, []),
@@ -439,6 +476,12 @@ SYMBOLS = {
     "vmb_bce_logits": (C.c_int, [C.POINTER(BceLogitsArgs), vp]),
     "vmb_bce_logits_workspace_bytes": (C.c_int64, [C.c_int64]),
     "vmb_bce_logits_bwd": (C.c_int, [C.POINTER(BceLogitsBwdArgs), vp]),
+    "vmb_percep_norm": (C.c_int, [C.POINTER(PercepNormArgs), vp]),
+    "vmb_percep_norm_bwd": (C.c_int, [C.POINTER(PercepNormBwdArgs), vp]),
+    "vmb_percep_stage": (C.c_int, [C.POINTER(PercepStageArgs), vp]),
+    "vmb_percep_stage_ctas": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int]),
+    "vmb_percep_loss": (C.c_int, [C.POINTER(PercepLossArgs), vp]),
+    "vmb_percep_stage_bwd": (C.c_int, [C.POINTER(PercepStageBwdArgs), vp]),
 }
 
 

@@ -1122,3 +1122,92 @@ def bce_logits_bwd(x, grad_loss, target, weight):
                               weight=float(weight), dtype=_gan_dt(x))
     _run("vmb_bce_logits_bwd", x, "bce_logits_bwd", a, nbytes=2 * x.numel() * x.element_size())
     return gx
+
+
+# ---- perceptual loss (csrc/perceptual.cu): basicsr's PerceptualLoss between the VGG convolutions; output and ground truth as one
+# 2B batch, fp32 or bf16 activations, contiguous; every reduction in a fixed order, nothing read on the host ----
+PERCEP_CRIT = {"l1": _lib.PERCEP_L1, "l2": _lib.PERCEP_L2, "fro": _lib.PERCEP_FRO}
+
+
+def percep_norm(x, gt, mean, std, range_norm, dtype):
+    """(B, 3, H, W) fp32 x and gt, any strides -> (2B, 3, H, W) `dtype`: [x; gt] through (v + 1) / 2 (range_norm) and
+    (v - mean) / std (mean, std: the (1, 3, 1, 1) fp32 buffers, or None)"""
+    B, _, H, W = x.shape
+    out = torch.empty((2 * B, 3, H, W), dtype=dtype, device=x.device)
+    a = _lib.PercepNormArgs(x=_ptr(x), gt=_ptr(gt), x_stride=(C.c_int64 * 4)(*x.stride()), gt_stride=(C.c_int64 * 4)(*gt.stride()),
+                            mean=_ptr(mean), std=_ptr(std), out=_ptr(out), B=B, H=H, W=W, range_norm=int(range_norm),
+                            dtype=_gan_dt(out))
+    _run("vmb_percep_norm", x, "percep_norm", a, nbytes=2 * x.numel() * (4 + out.element_size()))
+    return out
+
+
+def percep_norm_bwd(g, std, range_norm):
+    """gradient at x (fp32, contiguous) of percep_norm from the gradient g (B, 3, H, W) at its x half"""
+    B, _, H, W = g.shape
+    dx = torch.empty(g.shape, dtype=torch.float32, device=g.device)
+    a = _lib.PercepNormBwdArgs(g=_ptr(g), dx=_ptr(dx), std=_ptr(std), B=B, H=H, W=W, range_norm=int(range_norm), dtype=_gan_dt(g))
+    _run("vmb_percep_norm_bwd", g, "percep_norm_bwd", a, nbytes=g.numel() * (4 + g.element_size()))
+    return dx
+
+
+def percep_stage_ctas(B, C, H, W):
+    """CTAs of vmb_percep_stage at this x-half shape: the partials it writes per feature site"""
+    return _lib.lib().vmb_percep_stage_ctas(B, C, H, W)
+
+
+def percep_stage(y, relu, pool, feat, partial, crit, save):
+    """One stage after a VGG convolution, y (2B, C, H, W) = [x half; gt half]: ReLU in place (relu), the 2 x 2 max-pool (pool), and
+    at each feature site k (0 conv, 1 relu, 2 pool) with feat[k] the criterion's per-CTA partials into partial[k].  With `save`, the
+    backward's state for the x half.  -> (pooled or None, code or None, [save of each site or None])"""
+    B2, Cc, H, W = y.shape
+    B = B2 // 2
+    dev = y.device
+    pooled = torch.empty((B2, Cc, H // 2, W // 2), dtype=y.dtype, device=dev) if pool else None
+    cells = (B, Cc, (H + 1) // 2, (W + 1) // 2)
+    code = torch.empty(cells, dtype=torch.uint8, device=dev) if save and relu else None
+    saves = [None] * 3
+    if save:
+        for k in range(3):
+            if not feat[k]:
+                continue
+            if crit == "l1":  # a byte of sign codes per cell, or per pooled element
+                saves[k] = torch.empty((B, Cc, H // 2, W // 2) if k == 2 else cells, dtype=torch.uint8, device=dev)
+            else:
+                saves[k] = torch.empty((B, Cc, H // 2, W // 2) if k == 2 else (B, Cc, H, W), dtype=torch.float32, device=dev)
+    a = _lib.PercepStageArgs(y=_ptr(y), pooled=_ptr(pooled), code=_ptr(code), save=(C.c_void_p * 3)(*[0 if s is None else s.data_ptr()
+                             for s in saves]), partial=(C.c_void_p * 3)(*[0 if p is None else p.data_ptr() for p in partial]),
+                             feat=(C.c_int * 3)(*map(int, feat)), B=B, C=Cc, H=H, W=W, relu=int(relu), pool=int(pool),
+                             crit=PERCEP_CRIT[crit], dtype=_gan_dt(y))
+    nbytes = y.numel() * y.element_size() * (1 if pool or not relu else 2) + (pooled.numel() * y.element_size() if pool else 0)
+    _run("vmb_percep_stage", y, "percep_stage", a, nbytes=nbytes)
+    return pooled, code, saves
+
+
+def percep_loss(partial, offsets, numels, weights, crit, perceptual_weight):
+    """perceptual_weight * sum_k weights[k] crit_k from the features' partials (feature k at partial[offsets[k]:offsets[k + 1]])
+    -> (0-dim fp32 loss, per-feature criterion values (fp32, the norms the fro backward divides by))"""
+    n = len(weights)
+    loss = torch.empty((), dtype=torch.float32, device=partial.device)
+    value = torch.empty(n, dtype=torch.float32, device=partial.device)
+    a = _lib.PercepLossArgs(partial=_ptr(partial), loss=_ptr(loss), value=_ptr(value),
+                            offset=(C.c_int * (_lib.PERCEP_MAX_FEATS + 1))(*offsets),
+                            numel=(C.c_int64 * _lib.PERCEP_MAX_FEATS)(*numels), weight=(C.c_float * _lib.PERCEP_MAX_FEATS)(*weights),
+                            feats=n, crit=PERCEP_CRIT[crit], perceptual_weight=float(perceptual_weight))
+    _run("vmb_percep_loss", partial, "percep_loss", a, nbytes=partial.numel() * 4)
+    return loss, value
+
+
+def percep_stage_bwd(g_in, code, saves, feat, feat_index, scale, grad_loss, value, shape, relu, pool, crit, dtype):
+    """Gradient at a stage's conv output, x half (B, C, H, W) = `shape`, from the gradient g_in at its output (None at the deepest
+    stage) and the saved state of percep_stage; the loss terms' factors are grad_loss (device scalar) * scale[k]"""
+    dev = grad_loss.device
+    g_out = torch.empty(shape, dtype=dtype, device=dev)
+    B, Cc, H, W = shape
+    a = _lib.PercepStageBwdArgs(g_in=_ptr(g_in), g_out=_ptr(g_out), code=_ptr(code),
+                                save=(C.c_void_p * 3)(*[0 if s is None else s.data_ptr() for s in saves]), grad_loss=_ptr(grad_loss),
+                                value=_ptr(value), feat=(C.c_int * 3)(*map(int, feat)), feat_index=(C.c_int * 3)(*feat_index),
+                                scale=(C.c_float * 3)(*scale), B=B, C=Cc, H=H, W=W, relu=int(relu), pool=int(pool),
+                                crit=PERCEP_CRIT[crit], dtype=_gan_dt(g_out))
+    nbytes = g_out.numel() * g_out.element_size() + (g_in.numel() * g_in.element_size() if g_in is not None else 0)
+    _run("vmb_percep_stage_bwd", grad_loss, "percep_stage_bwd", a, nbytes=nbytes)
+    return g_out
