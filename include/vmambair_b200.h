@@ -886,6 +886,94 @@ typedef struct {
 } vmb_percep_stage_bwd_args;
 int vmb_percep_stage_bwd(const vmb_percep_stage_bwd_args* a, void* stream);
 
+/* ---- Perceptual metrics: LPIPS (lpips.LPIPS(net='vgg'), version 0.1; RealSR/Metric/LPIPS.py) and DISTS (RealSR/Metric/dists.py)
+ * between the VGG16 convolutions.  The two images of each pair run as one 2B batch: images 0..B-1 are the first of each pair,
+ * B..2B-1 the second.  Activations are fp32 NCHW contiguous; the ReLU (and LPIPS's max-pool) between the convolutions is
+ * vmb_percep_stage.  No atomics: every partial has one writer and the final kernels add them in index order. */
+#define VMB_PMETRIC_LPIPS 0
+#define VMB_PMETRIC_DISTS 1
+#define VMB_PMETRIC_MAX_LAYERS 6 /* DISTS: the input and relu1_2 .. relu5_3 */
+
+/* An input image batch: element (b, c, h, w) at data + b stride[0] + c stride[1] + h stride[2] + w stride[3] (elements, c in RGB
+ * order; a BGR image is addressed from its channel 2 with a negative channel stride).  u8 = 0: fp32 values; 1: uint8 levels. */
+typedef struct {
+    const void* data;
+    int64_t stride[4];
+    int u8;
+} vmb_pmetric_src;
+
+/* The input preparation of both metrics in one launch (replaces LPIPS's `2 * in0 - 1` and ScalingLayer, LPIPS.py:25-31's
+ * `/ 255.` and normalize(mean=.5, std=.5); DISTS's forward_once `(x - self.mean) / self.std` (dists.py:71), prepare_image's
+ * ToTensor (:117-121) and the layer-0 statistics of forward's loop (:99-109)).  out[b] from src[0], out[B + b] from src[1], (2B, 3, H, W) fp32:
+ *   LPIPS: v = u / 255 then (v - .5) / .5 (uint8), or 2 v - 1 (fp32 with normalize), or v; out = (v - shift[c]) / scale[c].
+ *   DISTS: v = u / 255 (uint8) or v; out = (v - shift[c]) / scale[c] (the ImageNet mean / std), and when stats != NULL the
+ *   statistics of the raw v as vmb_dists_layer writes them, C = 3, tiles = vmb_pmetric_tiles(3 B, H W) over pixels.
+ * Each step is one IEEE fp32 operation, as the scripts' numpy / torch conversions.  shift, scale: 3 fp32 on the device. */
+typedef struct {
+    vmb_pmetric_src src[2];
+    const float *shift, *scale;
+    float* out;
+    double* stats;
+    int B, H, W, metric, normalize;
+} vmb_pmetric_prep_args;
+int vmb_pmetric_prep(const vmb_pmetric_prep_args* a, void* stream);
+/* CTAs per plane of the statistics kernels: `items` (pixels or 2 x 2 cells) of each of `planes` planes, split so that a
+ * layer fills the GPU even at B = 1 (a fixed rule, not the device's SM count, so the partials do not depend on the device). */
+int vmb_pmetric_tiles(int planes, int64_t items);
+
+/* One LPIPS feature layer (replaces lpips.normalize_tensor, (f0 - f1) ** 2, lin{k} and spatial_average's sum): y (2B, C, H, W) is
+ * the conv output before the ReLU, applied on load.  Per pixel n_i = sqrt(sum_c f_i^2) + 1e-10, then
+ * sum_c w[c] (f0 / n0 - f1 / n1)^2 (two passes over the channels, held in registers; the square is never expanded).
+ * partial[b * ctas + cta] = the CTA's sum of that over its pixels of image b, ctas = vmb_lpips_layer_ctas(B, H, W).
+ * C / 16 must be 4, 8, 16 or 32 (VGG16: 64 .. 512). */
+typedef struct {
+    const float* y;
+    const float* w;
+    float* partial;
+    int B, C, H, W;
+} vmb_lpips_layer_args;
+int vmb_lpips_layer(const vmb_lpips_layer_args* a, void* stream);
+int vmb_lpips_layer_ctas(int B, int H, int W);
+
+/* LPIPS's result in one CTA (replaces spatial_average's division and `val += res[l]`): layer k's partials of image b are
+ * partial[offset[k] + b * ctas[k] + i], i ascending; layer[k * B + b] = their sum / hw[k]; out[b] = sum over k ascending. */
+typedef struct {
+    const float* partial;
+    float *layer, *out;
+    int offset[VMB_PMETRIC_MAX_LAYERS], ctas[VMB_PMETRIC_MAX_LAYERS];
+    int64_t hw[VMB_PMETRIC_MAX_LAYERS];
+    int B, layers;
+} vmb_lpips_final_args;
+int vmb_lpips_final(const vmb_lpips_final_args* a, void* stream);
+
+/* One DISTS feature layer (replaces the stage's ReLU, the next stage's L2pooling (dists.py:24-27) and the means / variances /
+ * covariance of forward's loop (:100-108)): y (2B, C, H, W) is the conv output before the ReLU, applied on load.  stats[((b C + c) tiles + t) 5 + s], s = sum f0,
+ * sum f1, sum f0^2, sum f1^2, sum f0 f1 over tile t of the 2 x 2 cells of plane c of pair b (tiles = vmb_pmetric_tiles(B C,
+ * ceil(H/2) ceil(W/2))), accumulated in fp64.  pooled (NULL: none): L2pooling, sqrt(sum 3 x 3 [.25 .5 .25]^T [.25 .5 .25] f^2 +
+ * 1e-12) with stride 2 and zero padding 1, (2B, C, ceil(H/2), ceil(W/2)). */
+typedef struct {
+    const float* y;
+    float* pooled;
+    double* stats;
+    int B, C, H, W;
+} vmb_dists_layer_args;
+int vmb_dists_layer(const vmb_dists_layer_args* a, void* stream);
+
+/* DISTS's score in one CTA (replaces forward's S1, S2, the alpha / beta sums and batch_average, dists.py:92-115): layer k's statistics start at entry offset[k]
+ * (entries of 5 doubles), C[k] channels, tiles[k] tiles per channel, n[k] pixels per plane.  Per channel, in fp64: the tiles added
+ * in order, mu = sum / n, var = sum f^2 / n - mu^2, cov = sum f0 f1 / n - mu0 mu1, S1 = (2 mu0 mu1 + 1e-6) / (mu0^2 + mu1^2 + 1e-6),
+ * S2 = (2 cov + 1e-6) / (var0 + var1 + 1e-6); score[b] = 1 - sum_j (alpha_j S1_j + beta_j S2_j) / (sum alpha + sum beta) over all
+ * channels j in layer order.  alpha, beta: sum C[k] fp32 on the device.  mean (NULL: not written): the mean of score over b. */
+typedef struct {
+    const double* stats;
+    const float *alpha, *beta;
+    float *score, *mean;
+    int64_t offset[VMB_PMETRIC_MAX_LAYERS], n[VMB_PMETRIC_MAX_LAYERS];
+    int C[VMB_PMETRIC_MAX_LAYERS], tiles[VMB_PMETRIC_MAX_LAYERS];
+    int B, layers;
+} vmb_dists_final_args;
+int vmb_dists_final(const vmb_dists_final_args* a, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

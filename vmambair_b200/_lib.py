@@ -408,6 +408,44 @@ class PercepStageBwdArgs(C.Structure):
                 ("H", C.c_int), ("W", C.c_int), ("relu", C.c_int), ("pool", C.c_int), ("crit", C.c_int), ("dtype", C.c_int)]
 
 
+PMETRIC_LPIPS, PMETRIC_DISTS = 0, 1  # VMB_PMETRIC_LPIPS / _DISTS
+PMETRIC_MAX_LAYERS = 6  # VMB_PMETRIC_MAX_LAYERS
+
+
+class PmetricSrc(C.Structure):
+    _c_name_ = "vmb_pmetric_src"
+    _fields_ = [("data", vp), ("stride", i64 * 4), ("u8", C.c_int)]
+
+
+class PmetricPrepArgs(C.Structure):
+    _c_name_ = "vmb_pmetric_prep_args"
+    _fields_ = [("src", PmetricSrc * 2), ("shift", vp), ("scale", vp), ("out", vp), ("stats", vp), ("B", C.c_int), ("H", C.c_int),
+                ("W", C.c_int), ("metric", C.c_int), ("normalize", C.c_int)]
+
+
+class LpipsLayerArgs(C.Structure):
+    _c_name_ = "vmb_lpips_layer_args"
+    _fields_ = [("y", vp), ("w", vp), ("partial", vp), ("B", C.c_int), ("C", C.c_int), ("H", C.c_int), ("W", C.c_int)]
+
+
+class LpipsFinalArgs(C.Structure):
+    _c_name_ = "vmb_lpips_final_args"
+    _fields_ = [("partial", vp), ("layer", vp), ("out", vp), ("offset", C.c_int * PMETRIC_MAX_LAYERS),
+                ("ctas", C.c_int * PMETRIC_MAX_LAYERS), ("hw", i64 * PMETRIC_MAX_LAYERS), ("B", C.c_int), ("layers", C.c_int)]
+
+
+class DistsLayerArgs(C.Structure):
+    _c_name_ = "vmb_dists_layer_args"
+    _fields_ = [("y", vp), ("pooled", vp), ("stats", vp), ("B", C.c_int), ("C", C.c_int), ("H", C.c_int), ("W", C.c_int)]
+
+
+class DistsFinalArgs(C.Structure):
+    _c_name_ = "vmb_dists_final_args"
+    _fields_ = [("stats", vp), ("alpha", vp), ("beta", vp), ("score", vp), ("mean", vp), ("offset", i64 * PMETRIC_MAX_LAYERS),
+                ("n", i64 * PMETRIC_MAX_LAYERS), ("C", C.c_int * PMETRIC_MAX_LAYERS), ("tiles", C.c_int * PMETRIC_MAX_LAYERS),
+                ("B", C.c_int), ("layers", C.c_int)]
+
+
 # every symbol include/vmambair_b200.h declares: name -> (restype, argtypes)
 SYMBOLS = {
     "vmb_last_error": (C.c_char_p, []),
@@ -482,6 +520,13 @@ SYMBOLS = {
     "vmb_percep_stage_ctas": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int]),
     "vmb_percep_loss": (C.c_int, [C.POINTER(PercepLossArgs), vp]),
     "vmb_percep_stage_bwd": (C.c_int, [C.POINTER(PercepStageBwdArgs), vp]),
+    "vmb_pmetric_prep": (C.c_int, [C.POINTER(PmetricPrepArgs), vp]),
+    "vmb_pmetric_tiles": (C.c_int, [C.c_int, C.c_int64]),
+    "vmb_lpips_layer": (C.c_int, [C.POINTER(LpipsLayerArgs), vp]),
+    "vmb_lpips_layer_ctas": (C.c_int, [C.c_int, C.c_int, C.c_int]),
+    "vmb_lpips_final": (C.c_int, [C.POINTER(LpipsFinalArgs), vp]),
+    "vmb_dists_layer": (C.c_int, [C.POINTER(DistsLayerArgs), vp]),
+    "vmb_dists_final": (C.c_int, [C.POINTER(DistsFinalArgs), vp]),
 }
 
 

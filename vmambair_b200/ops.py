@@ -1211,3 +1211,77 @@ def percep_stage_bwd(g_in, code, saves, feat, feat_index, scale, grad_loss, valu
     nbytes = g_out.numel() * g_out.element_size() + (g_in.numel() * g_in.element_size() if g_in is not None else 0)
     _run("vmb_percep_stage_bwd", grad_loss, "percep_stage_bwd", a, nbytes=nbytes)
     return g_out
+
+
+# ---- perceptual metrics (csrc/percep_metrics.cu): LPIPS (VGG) and DISTS between the VGG16 convolutions; the two images of each
+# pair as one 2B batch, fp32 activations, contiguous; every reduction in a fixed order, nothing read on the host ----
+PMETRIC = {"lpips": _lib.PMETRIC_LPIPS, "dists": _lib.PMETRIC_DISTS}
+
+
+def pmetric_src(t, offset, strides):
+    """vmb_pmetric_src of the (B, 3, H, W) view (RGB channel order) of CUDA tensor t's storage that starts `offset` elements after
+    t.data_ptr(), element strides (b, c, h, w); t is float32 or uint8"""
+    if t.dtype not in (torch.float32, torch.uint8):
+        raise RuntimeError(f"perceptual metrics: source dtype {t.dtype} is not float32 or uint8")
+    return _lib.PmetricSrc(data=C.c_void_p(t.data_ptr() + offset * t.element_size()), stride=(C.c_int64 * 4)(*strides),
+                           u8=int(t.dtype == torch.uint8))
+
+
+def pmetric_tiles(planes, items):
+    """CTAs per plane of the statistics kernels (vmb_pmetric_tiles)"""
+    return _lib.lib().vmb_pmetric_tiles(planes, items)
+
+
+def pmetric_prep(t, src0, src1, B, H, W, metric, shift, scale, normalize=False, stats=None):
+    """-> (2B, 3, H, W) fp32: [prep(src0); prep(src1)] for `metric` ('lpips' or 'dists'); shift, scale: the (1, 3, 1, 1) fp32
+    buffers; stats: DISTS's fp64 layer-0 statistics buffer, or None.  t: a tensor on the sources' device (stream and count)."""
+    out = torch.empty((2 * B, 3, H, W), dtype=torch.float32, device=t.device)
+    a = _lib.PmetricPrepArgs(src=(_lib.PmetricSrc * 2)(src0, src1), shift=_ptr(shift), scale=_ptr(scale), out=_ptr(out),
+                             stats=_ptr(stats), B=B, H=H, W=W, metric=PMETRIC[metric], normalize=int(normalize))
+    _run("vmb_pmetric_prep", t, "pmetric_prep", a, nbytes=2 * B * 3 * H * W * (t.element_size() + 4))
+    return out
+
+
+def lpips_layer_ctas(B, H, W):
+    """CTAs per image of vmb_lpips_layer at this shape: its partials per image"""
+    return _lib.lib().vmb_lpips_layer_ctas(B, H, W)
+
+
+def lpips_layer(y, w, partial):
+    """LPIPS's per-CTA partials of one feature layer into `partial` (B * lpips_layer_ctas): y (2B, C, H, W) the conv output before
+    the ReLU, w the (1, C, 1, 1) lin weight"""
+    B2, Cc, H, W = y.shape
+    a = _lib.LpipsLayerArgs(y=_ptr(y), w=_ptr(w), partial=_ptr(partial), B=B2 // 2, C=Cc, H=H, W=W)
+    _run("vmb_lpips_layer", y, "lpips_layer", a, nbytes=y.numel() * 4)
+
+
+def lpips_final(partial, offsets, ctas, hws, B):
+    """-> (val (B,), per-layer values (layers, B)), fp32: each layer's partials added in order, / H W, summed over the layers"""
+    n = len(ctas)
+    layer = torch.empty((n + 1, B), dtype=torch.float32, device=partial.device)
+    L = _lib.PMETRIC_MAX_LAYERS
+    a = _lib.LpipsFinalArgs(partial=_ptr(partial), layer=_ptr(layer), out=_ptr(layer[n]), offset=(C.c_int * L)(*offsets),
+                            ctas=(C.c_int * L)(*ctas), hw=(C.c_int64 * L)(*hws), B=B, layers=n)
+    _run("vmb_lpips_final", partial, "lpips_final", a, nbytes=partial.numel() * 4)
+    return layer[n], layer[:n]
+
+
+def dists_layer(y, stats, pool):
+    """DISTS's fp64 statistics of one feature layer into `stats`, and with `pool` -> the L2-pooled (2B, C, ceil(H/2), ceil(W/2))
+    input of the next convolution (else None); y (2B, C, H, W) the conv output before the ReLU"""
+    B2, Cc, H, W = y.shape
+    pooled = torch.empty((B2, Cc, (H + 1) // 2, (W + 1) // 2), dtype=torch.float32, device=y.device) if pool else None
+    a = _lib.DistsLayerArgs(y=_ptr(y), pooled=_ptr(pooled), stats=_ptr(stats), B=B2 // 2, C=Cc, H=H, W=W)
+    _run("vmb_dists_layer", y, "dists_layer", a, nbytes=y.numel() * 4 + (pooled.numel() * 4 if pool else 0))
+    return pooled
+
+
+def dists_final(stats, alpha, beta, offsets, channels, tiles, ns, B, batch_average):
+    """-> the (B,) fp32 scores, and with batch_average their mean (0-dim) as well (else None)"""
+    score = torch.empty(B + 1, dtype=torch.float32, device=stats.device)
+    L = _lib.PMETRIC_MAX_LAYERS
+    a = _lib.DistsFinalArgs(stats=_ptr(stats), alpha=_ptr(alpha), beta=_ptr(beta), score=_ptr(score),
+                            mean=_ptr(score[B]) if batch_average else None, offset=(C.c_int64 * L)(*offsets), n=(C.c_int64 * L)(*ns),
+                            C=(C.c_int * L)(*channels), tiles=(C.c_int * L)(*tiles), B=B, layers=len(channels))
+    _run("vmb_dists_final", stats, "dists_final", a, nbytes=stats.numel() * 8)
+    return score[:B], (score[B] if batch_average else None)

@@ -41,15 +41,15 @@ def weights_file_name(vgg_type):
     return os.path.basename(torchvision.models.get_model_weights(vgg_type).IMAGENET1K_V1.url)
 
 
-def find_weights(vgg_type):
+def find_weights(vgg_type, who="PerceptualLoss"):
     """basicsr's lookup of the pretrained weights, without the download: experiments/pretrained_models/<file>, then the torch hub
-    cache's checkpoints/<file>"""
+    cache's checkpoints/<file>; `who` names the caller in the error"""
     name = weights_file_name(vgg_type)
     paths = [os.path.join("experiments", "pretrained_models", name), os.path.join(torch.hub.get_dir(), "checkpoints", name)]
     for p in paths:
         if os.path.isfile(p):
             return p
-    raise FileNotFoundError(f"PerceptualLoss: the {vgg_type} weights are in neither {paths[0]} nor {paths[1]}; place "
+    raise FileNotFoundError(f"{who}: the {vgg_type} weights are in neither {paths[0]} nor {paths[1]}; place "
                             f"torchvision's {name} there, or pass weights=<path> (nothing is downloaded)")
 
 
