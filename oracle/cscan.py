@@ -128,6 +128,28 @@ def scan_bwd(u, delta, A, B, C, D, delta_bias, dout, delta_softplus=False):
     return tuple(map(t, (du, dd, dA, dB, dC, dD, db)))
 
 
+class Scan(torch.autograd.Function):
+    """The sequential oracle as a differentiable function: Scan.apply(u, delta, A, B, C, D, delta_bias, delta_softplus).
+    float64 inputs run scan_fwd(fp64=True) / scan_bwd, any other dtype scan_fwd / scan_bwd_f32.  The group count comes from B.shape as
+    in _shapes; results (output and gradients) come back in u's dtype and on u's device, gradients shaped like their inputs, None for an
+    absent D or delta_bias.  The C oracle reads fp32 inputs: a float64 caller's inputs and incoming gradient are rounded to fp32
+    (relative 6e-8) before the float64 recurrence."""
+
+    @staticmethod
+    def forward(ctx, u, delta, A, B, C, D=None, delta_bias=None, delta_softplus=False):
+        ctx.save_for_backward(u, delta, A, B, C, D, delta_bias)
+        ctx.delta_softplus = delta_softplus
+        out = scan_fwd(u, delta, A, B, C, D, delta_bias, delta_softplus, fp64=u.dtype == torch.float64)
+        return out.to(device=u.device, dtype=u.dtype)
+
+    @staticmethod
+    def backward(ctx, dout):
+        ins = ctx.saved_tensors
+        bwd = scan_bwd if ins[0].dtype == torch.float64 else scan_bwd_f32
+        grads = bwd(*ins, dout, ctx.delta_softplus)
+        return tuple(None if g is None else g.view(t.shape).to(device=t.device, dtype=t.dtype) for g, t in zip(grads, ins)) + (None,)
+
+
 def scan_fwd_mag(u, delta, A, B, C, D=None, delta_bias=None, delta_softplus=False):
     """scan_fwd(fp64=True) and the magnitude S of every output (oracle/scan_bound.py) -> (out, S), float64 torch tensors"""
     b, Dm, L, N, G = _shapes(u, A, B)

@@ -1,6 +1,6 @@
-"""CPU oracle of the OSS block / network forward.  TEST INFRASTRUCTURE ONLY.
+"""CPU oracle of the OSS block / network, forward and (under autograd) backward.  TEST INFRASTRUCTURE ONLY.
 
-A functional (state_dict-driven) restatement in plain fp32 torch of the reference modules
+A functional (state_dict-driven) restatement in plain torch of the reference modules
   LayerNorm          SRGAN/VmambaIR/archs/MambaSISR6_arch.py:166-195
   FeedForward        MambaSISR6_arch.py:201-218
   SS2D_1.forward     MambaSISR6_arch.py:395-498 (and the Mamber32/33, RealSR variants, SURVEY.md 0.2)
@@ -10,6 +10,30 @@ with the scan evaluated by the sequential C oracle (oracle/cscan.py).  Pinned ag
 real reference modules by tests/test_oracle_modules.py (fixtures from tests/golden/make_golden.py).
 Used by tests, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference leg; the product
 (vmambair_b200) never imports it.
+
+The torch ops run in the dtype and on the device of their inputs (the GPU tests evaluate the oracle in float64 on CUDA); the scan
+always runs on the CPU.  With grad enabled and an input that requires grad, the scan is cscan.Scan (the C oracle's analytic backward),
+so the whole block / net is differentiable: tests/test_oracle_grad_cpu.py pins that backward against the real reference's autograd.
+
+Storage-precision emulation (STORE_DTYPE, test infrastructure): when set to a dtype (torch.bfloat16), every tensor the fused pipeline
+keeps in that dtype between kernels is rounded to it here as well and back to its own dtype (arithmetic stays in the input dtype, like
+the kernels' fp32 accumulators), and GEMM / conv weights are rounded once.  Gives the error a "bf16 storage, fp32 accumulate" evaluation
+of the SAME network is expected to have against the unrounded oracle -- the yardstick for the bf16 bounds of
+tests/test_bench_parity_gpu.py (inference) and tests/test_train_net_gpu.py (training).  Under autograd the rounding points act on the
+backward too, as the training path (vmambair_b200.fused_train) stores them:
+  _q    an activation the forward stores AND whose gradient the backward stores in the compute dtype: value and gradient rounded
+        -- xz's x half (_Front.forward pixlin -> xz / backward dxz[:, :C] from the flipped dwconv), xc (dwconv3x3 + SiLU / sum4_add
+        -> dxc), delta, B, C (dbl4 / ddbl), the scan outputs (ys / dys = the gathered merge gradient dm), y2 (merge_norm_gate / the
+        dy2 _Tail hands back), the FFN's t (_Tail.forward pixlin + norm2 / dt) and gg (dwconv3x3 GELU gate / dgg);
+  _qs   the residual stream, likewise: x1 (out_conv + residual / dx1 = layernorm_bwd(add=dout)) and the block output (/ dout);
+  _qg   a gradient the backward stores with no stored forward value behind it: gradient only -- the scan's du per direction
+        (selective_scan_bwd), dv in front of both depthwise convs (dwconv3x3_bwd phase "data"), dxn / dx1n at the norm1 / norm2
+        outputs (pixlin with WinT / WpinT), norm1's dx (layernorm_bwd, before autograd adds the residual's), z_pre's gradient
+        (merge_norm_gate_bwd dz_out), and dyg in front of the channel gate (_out_conv_bwd pixlin with WoutT);
+  _qw   GEMM weights (prepare_block's kernel-layout copies): forward only -- parameter gradients are fp32 accumulators, never rounded.
+Not emulated: z_pre's stored value (the training path keeps z_pre and applies SiLU in fp32; the inference path, emulated here, stores
+SiLU(z)), and the single rounding of the x_proj data gradient summed over the four directions (pixlin with WbigT).
+With STORE_DTYPE unset, or without grad, the oracle computes exactly what it computes without these rules.
 """
 from __future__ import annotations
 
@@ -18,24 +42,45 @@ import torch.nn.functional as F
 
 from . import cscan
 
-# Storage-precision emulation (test infrastructure): when set to a dtype (torch.bfloat16), every tensor the fused pipeline
-# keeps in that dtype between kernels is rounded to it here as well (arithmetic stays fp32, like the kernels' accumulators), and
-# GEMM / conv weights are rounded once.  Gives the error a "bf16 storage, fp32 accumulate" evaluation of the SAME network is
-# expected to have against the fp32 oracle -- the yardstick for the bf16 parity bound in tests/test_bench_parity_gpu.py.
 STORE_DTYPE = None
 STREAM_FP32 = False  # with STORE_DTYPE set: keep the residual stream (block inputs / outputs) un-rounded
 
 
+class _Store(torch.autograd.Function):
+    """value and / or incoming gradient rounded to STORE_DTYPE and back to their own dtype"""
+
+    @staticmethod
+    def forward(ctx, t, value, grad):
+        ctx.grad = grad
+        return t.to(STORE_DTYPE).to(t.dtype) if value else t.view_as(t)
+
+    @staticmethod
+    def backward(ctx, g):
+        return (g.to(STORE_DTYPE).to(g.dtype) if ctx.grad else g), None, None
+
+
+def _store(t, value=True, grad=True):
+    if STORE_DTYPE is None:
+        return t
+    if torch.is_grad_enabled() and t.requires_grad:
+        return _Store.apply(t, value, grad)
+    return t.to(STORE_DTYPE).to(t.dtype) if value else t
+
+
 def _q(t):
-    return t if STORE_DTYPE is None else t.to(STORE_DTYPE).float()
+    return _store(t)
 
 
 def _qs(t):  # residual stream
-    return t if (STORE_DTYPE is None or STREAM_FP32) else t.to(STORE_DTYPE).float()
+    return t if STREAM_FP32 else _store(t)
+
+
+def _qg(t):
+    return _store(t, value=False)
 
 
 def _qw(w):
-    return w if (STORE_DTYPE is None or w is None or w.dim() < 2) else w.to(STORE_DTYPE).float()
+    return w if (w is None or w.dim() < 2) else _store(w, grad=False)
 
 
 def _ln(x, w, b):  # per-pixel LayerNorm over channels of (B,C,H,W)
@@ -47,7 +92,10 @@ def _ln(x, w, b):  # per-pixel LayerNorm over channels of (B,C,H,W)
 
 
 def _scan(u, dt, A, B, C, D, bias):
-    return cscan.scan_fwd(u, dt, A, B, C, D, bias, True)
+    ins = (u, dt, A, B, C, D, bias)
+    if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in ins):
+        return cscan.Scan.apply(*ins, True)
+    return cscan.scan_fwd(*ins, True, fp64=u.dtype == torch.float64).to(device=u.device, dtype=u.dtype)
 
 
 def ss2d(sd, pre, x, gate):
@@ -56,8 +104,8 @@ def ss2d(sd, pre, x, gate):
     L = H * W
     xz = F.conv2d(x, _qw(g("in_conv.weight")), g("in_conv.bias"))
     xi, z = xz.chunk(2, 1)
-    z = _q(F.silu(z))
-    xi = _q(F.silu(F.conv2d(_q(xi), g("conv2d.weight"), g("conv2d.bias"), padding=1, groups=C)))
+    z = _store(F.silu(_qg(z)), grad=False)
+    xi = _q(F.silu(_qg(F.conv2d(_q(xi), g("conv2d.weight"), g("conv2d.bias"), padding=1, groups=C))))
     # four spatial directions: row-major, column-major, and their reversals (:401-404)
     rows = xi.flatten(2)
     cols = xi.transpose(2, 3).flatten(2)
@@ -73,7 +121,7 @@ def ss2d(sd, pre, x, gate):
         dts = _q(torch.einsum("bkcl,kdc->bkdl", xs, big))
         xq = torch.einsum("bkdl,kcd->bkcl", xs, _qw(xw))
         Bs, Cs = _q(xq[:, :, R:R + N]), _q(xq[:, :, R + N:])
-    oy = _scan(xs.reshape(B_, 4 * C, L), dts.reshape(B_, 4 * C, L), -torch.exp(g("A_logs")), Bs, Cs, g("Ds"),
+    oy = _scan(_qg(xs).reshape(B_, 4 * C, L), dts.reshape(B_, 4 * C, L), -torch.exp(g("A_logs")), Bs, Cs, g("Ds"),
                g("dt_projs_bias").reshape(-1)).view(B_, 4, C, L)
     oy = _q(oy)
     y = oy[:, 0] + oy[:, 2].flip(-1)
@@ -82,7 +130,7 @@ def ss2d(sd, pre, x, gate):
     y1 = _ln(y.view(B_, C, H, W), g("out_norm.body.weight"), g("out_norm.body.bias"))
     y2 = _q(y1 * z)
     c = channel(sd, pre, y2.mean((2, 3)))[:, :, None, None]  # (B,C,1,1)
-    y2 = y2 * c + y2 if gate == "mul" else y2 + c
+    y2 = _qg(y2 * c + y2 if gate == "mul" else y2 + c)
     return F.conv2d(y2, _qw(g("out_conv.weight")), g("out_conv.bias"))
 
 
@@ -111,14 +159,14 @@ def channel(sd, pre, pooled):
 
 def ffn(sd, pre, x):
     t = _q(F.conv2d(x, _qw(sd[pre + "project_in.weight"]), sd.get(pre + "project_in.bias")))
-    t = F.conv2d(t, sd[pre + "dwconv.weight"], sd.get(pre + "dwconv.bias"), padding=1, groups=t.shape[1])
+    t = _qg(F.conv2d(t, sd[pre + "dwconv.weight"], sd.get(pre + "dwconv.bias"), padding=1, groups=t.shape[1]))
     a, b = t.chunk(2, 1)
     return F.conv2d(_q(F.gelu(a) * b), _qw(sd[pre + "project_out.weight"]), sd.get(pre + "project_out.bias"))
 
 
 def block(sd, pre, x, gate="mul"):
-    x = _qs(x + ss2d(sd, pre + "attn.", _ln(x, sd[pre + "norm1.body.weight"], sd.get(pre + "norm1.body.bias")), gate))
-    return _qs(x + ffn(sd, pre + "ffn.", _ln(x, sd[pre + "norm2.body.weight"], sd.get(pre + "norm2.body.bias"))))
+    x = _qs(x + ss2d(sd, pre + "attn.", _qg(_ln(_qg(x), sd[pre + "norm1.body.weight"], sd.get(pre + "norm1.body.bias"))), gate))
+    return _qs(x + ffn(sd, pre + "ffn.", _qg(_ln(x, sd[pre + "norm2.body.weight"], sd.get(pre + "norm2.body.bias")))))
 
 
 def _stage(sd, name, x, gate):
