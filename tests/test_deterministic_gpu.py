@@ -382,9 +382,9 @@ print("CHILD OK")
 """
 
 
-def _in_child(fn, extra_env=None):
+def _in_child(fn):
     """runs fn of this module in a fresh interpreter with CUBLAS_WORKSPACE_CONFIG set (torch's cuBLAS needs it under the flag)"""
-    env = dict(os.environ, CUBLAS_WORKSPACE_CONFIG=":4096:8", **(extra_env or {}))
+    env = dict(os.environ, CUBLAS_WORKSPACE_CONFIG=":4096:8")
     r = subprocess.run([sys.executable, "-c", _CHILD.format(root=ROOT, fn=fn)], env=env, cwd=ROOT, capture_output=True, text=True,
                        timeout=900)
     assert r.returncode == 0 and "CHILD OK" in r.stdout, r.stdout[-3000:] + r.stderr[-3000:]
@@ -428,7 +428,7 @@ def child_cross_selective_scan():
 
 def child_compose_blocks():
     from vmambair_b200 import archs, ops
-    assert archs._TRAIN_PATH == "compose"
+    archs.set_train_path("compose")
     for variant in ("sisr", "realsr"):
         torch.manual_seed(0)
         blk = archs.MamberBlock(dim=32, num_heads=1, ffn_expansion_factor=2.66, bias=False, LayerNorm_type="WithBias",
@@ -453,8 +453,8 @@ def test_cross_selective_scan_under_flag_in_child():
     _in_child("child_cross_selective_scan")
 
 
-def test_compose_block_under_flag_in_child():
-    _in_child("child_compose_blocks", {"VMB_TRAIN_PATH": "compose"})
+def test_compose_block_under_flag_in_child_via_set_train_path():
+    _in_child("child_compose_blocks")
 
 
 # ----------------------------------------------------------------------------- graph capture, warning
@@ -478,7 +478,7 @@ def test_deterministic_backward_in_cuda_graph():
         assert_all_equal(eager, captured, "graph replay")
 
 
-def test_fused_block_warns_once_under_flag():
+def test_fused_block_warns_once_under_flag_naming_set_train_path():
     from vmambair_b200 import archs
     blk = archs.MamberBlock(dim=32, num_heads=1, ffn_expansion_factor=2.66, bias=False, LayerNorm_type="WithBias").cuda()
     x = torch.randn(1, 32, 16, 24, device="cuda")
@@ -499,7 +499,7 @@ def test_fused_block_warns_once_under_flag():
         hits = [w for w in rec if "use_deterministic_algorithms" in str(w.message)]
         assert len(hits) == 1 and issubclass(hits[0].category, UserWarning)
         msg = str(hits[0].message)
-        assert "VMB_TRAIN_PATH=compose" in msg and "train_ops.cu" in msg and "channel_bwd.cu" in msg and "merge" in msg
+        assert "set_train_path('compose')" in msg and "train_ops.cu" in msg and "channel_bwd.cu" in msg and "merge" in msg
     finally:
         torch.use_deterministic_algorithms(prev)
         archs._FUSED_DET_WARNED = False

@@ -8,8 +8,7 @@ stride divisibility.  pixlin_path() / conv_path() mirror csrc/pixlin.cu (pixlin_
 csrc/conv3x3.cu (conv3x3_launch, launch_16, launch_tma) with vec_ok / w_vec / pair_ok of csrc/api.cu and the kernels; every case
 asserts the path it intends, so that a case cannot drift onto another path when the card or a heuristic changes, and
 test_every_path_is_covered asserts that the case list reaches every path.  Where two paths can take the same values they run on
-the same values (check_pair: within the sum of their two bounds).  The persistent tile walk of the TMA conv (VMB_CONV_PERSIST=1, read
-once per process) runs in a child process.
+the same values (check_pair: within the sum of their two bounds).
 
 The worst err / bound per path is printed at the end of the module.  It sits just below 1 wherever a term of the bound is an exact
 allowance rather than slack: the final round-to-nearest of a 16-bit output uses up to u_out * |ref|, and an x' whose fp32 and
@@ -17,8 +16,6 @@ float64 values round to neighbouring 16-bit values differs by exactly the T of t
 slack: the fp32 paths, which have neither, use 0.07 - 0.14 of it on the H100.
 """
 import os
-import subprocess
-import sys
 import zlib
 from collections import namedtuple
 
@@ -30,7 +27,6 @@ from vmambair_b200 import ops
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 BF16, F16, F32 = torch.bfloat16, torch.float16, torch.float32
 DT16 = [BF16, F16]
 RATIOS = {}  # path -> largest err / bound seen (printed at the end of the module)
@@ -363,43 +359,34 @@ def test_pixlin_w_all_vs_ring(dtype, K):
 
 
 # ============================================================================= conv3x3: path mirror
-kTH, kTW, kHalo = 8, 16, 10 * 18
+kTH, kTW = 8, 16
 
 
-def tma_smem(MT, stages, nhwc):
-    """TmaConvCfg<MT, NHWC>::smem(stages)"""
-    a, b = 9 * MT * 32, (kHalo * 32 if nhwc else 16 * 10 * 32 * 2)
-    stage = (a + b + 255) // 256 * 256
-    return stages * stage + (0 if nhwc else kHalo * 48) + 8 * stages + 1024
-
-
-def conv_path(x, Cout, nhwc, out, persist=False):
-    """(kernel, pair_ok, persistent) that conv3x3_launch takes for input x (the view passed to ops.conv3x3) and destination out"""
+def conv_path(x, Cout, nhwc, out):
+    """(kernel, pair_ok) that conv3x3_launch takes for input x (the view passed to ops.conv3x3) and destination out"""
     B, Cin, H, W = x.shape
     if x.dtype == F32:
-        return ("simt-nhwc" if nhwc else "simt-nchw"), None, False
+        return ("simt-nhwc" if nhwc else "simt-nchw"), None
     tiles = cdiv(W, kTW) * cdiv(H, kTH) * B
     n = sms()
     if nhwc:
-        MT, st, k = (16, 4, "tma-nhwc-16") if Cout <= 16 else (64, 3, "tma-nhwc-64")
+        k = "tma-nhwc-16" if Cout <= 16 else "tma-nhwc-64"
     else:
         aligned = W % 8 == 0 and x.stride(0) % 8 == 0 and x.stride(1) % 8 == 0 and aligned16(x) and x.stride(1) >= H * W and x.stride(0) > 0
         if not aligned:
-            return ("generic-16" if Cout <= 16 else "generic-64"), None, False
+            return ("generic-16" if Cout <= 16 else "generic-64"), None
         if Cout > 32 and tiles * cdiv(Cout, 64) >= n:
-            MT, st, k = 64, 3, "tma-nchw-64"
+            k = "tma-nchw-64"
         elif Cout > 16 and tiles * cdiv(Cout, 32) >= n:
-            MT, st, k = 32, 3, "tma-nchw-32"
+            k = "tma-nchw-32"
         else:
-            MT, st, k = 16, 4, "tma-nchw-16"
+            k = "tma-nchw-16"
     pair_ok = W % 4 == 0 and out.stride(0) % 2 == 0 and out.stride(1) % 2 == 0 and out.data_ptr() % 4 == 0
-    per_sm = max((227 * 1024) // tma_smem(MT, st, nhwc), 1)
-    cap = max(n * min(per_sm, 8) // cdiv(Cout, MT), 1)
-    return k, pair_ok, persist and tiles > 3 * cap
+    return k, pair_ok
 
 
 CONV_PATHS = {"tma-nchw-64", "tma-nchw-32", "tma-nchw-16", "tma-nhwc-16", "tma-nhwc-64", "generic-16", "generic-64", "simt-nchw",
-              "simt-nhwc", "pair_ok", "pair-elementwise", "persistent"}
+              "simt-nhwc", "pair_ok", "pair-elementwise"}
 MODES = [G.CONV_PLAIN, G.CONV_UNSHUFFLE2, G.CONV_SHUFFLE2, G.CONV_ADD_NEAREST]
 OUT_SHAPE = {G.CONV_PLAIN: lambda B, C, H, W: (B, C, H, W), G.CONV_UNSHUFFLE2: lambda B, C, H, W: (B, 4 * C, H // 2, W // 2),
              G.CONV_SHUFFLE2: lambda B, C, H, W: (B, C // 4, 2 * H, 2 * W), G.CONV_ADD_NEAREST: lambda B, C, H, W: (B, C, H, W)}
@@ -425,7 +412,7 @@ def conv_id(c):
     return f"{str(c.dtype)[6:]}-B{c.B}-{c.Cin}to{c.Cout}-{c.H}x{c.W}-mode{c.mode}-s{c.scale}-x_{c.x}-out_{c.out}"
 
 
-def make_conv(c, seed, persist=False, with_ref=True):
+def make_conv(c, seed, with_ref=True):
     torch.manual_seed(seed)
     dt, B, Cin, Cout, H, W = c.dtype, conv_batch(c), c.Cin, c.Cout, c.H, c.W
     dev = "cuda"
@@ -454,15 +441,15 @@ def make_conv(c, seed, persist=False, with_ref=True):
     ref = S = None
     if with_ref:
         ref, S = G.conv3x3_ref(x.double(), w.double(), bias.double(), c.mode, None if add is None else add.double(), c.scale)
-    k, pair_ok, pers = conv_path(xx, Cout, c.x == "nhwc", out, persist)
-    paths = {k} | ({"pair_ok" if pair_ok else "pair-elementwise"} if pair_ok is not None else set()) | ({"persistent"} if pers else set())
+    k, pair_ok = conv_path(xx, Cout, c.x == "nhwc", out)
+    paths = {k} | ({"pair_ok" if pair_ok else "pair-elementwise"} if pair_ok is not None else set())
     call = dict(x=xx, wp=ops.pack_conv3x3_weight(w, dt), bias=bias, c_out=Cout, mode=c.mode, out=out, add=add, add_scale=c.scale,
                 nhwc=c.x == "nhwc")
     return call, ref, S, paths
 
 
-def run_conv(c, seed=0, persist=False):
-    call, ref, S, paths = make_conv(c, seed, persist)
+def run_conv(c, seed=0):
+    call, ref, S, paths = make_conv(c, seed)
     if c.expect is not None:
         assert set(c.expect) <= paths, (sorted(c.expect), sorted(paths))
     got = ops.conv3x3(**call)
@@ -594,28 +581,6 @@ def test_bench_conv3x3_site(c):
     run_conv(c, seed=12)
 
 
-# ============================================================================= the persistent tile walk (child process)
-PERSIST_CASES = [Conv(BF16, 10, 20, 16, 128, 128, G.CONV_PLAIN, 1, expect={"tma-nchw-16", "persistent"}),
-                 Conv(F16, 13, 20, 80, 64, 64, G.CONV_SHUFFLE2, 1, out="slice", expect={"tma-nchw-64", "persistent"}),
-                 Conv(BF16, 10, 16, 48, 128, 128, G.CONV_UNSHUFFLE2, 1, x="nhwc", out="odd", expect={"tma-nhwc-64", "persistent"})]
-
-_CHILD = """
-import sys
-sys.path.insert(0, {root!r})
-from tests import test_pixlin_conv3x3_gpu as t
-for i, c in enumerate(t.PERSIST_CASES):
-    t.run_conv(c, seed=i, persist=True)
-print("CHILD OK", t.RATIOS)
-"""
-
-
-def test_conv3x3_persistent_walk_in_child():
-    env = dict(os.environ, VMB_CONV_PERSIST="1")
-    r = subprocess.run([sys.executable, "-c", _CHILD.format(root=ROOT)], env=env, cwd=ROOT, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0 and "CHILD OK" in r.stdout, r.stdout[-3000:] + r.stderr[-3000:]
-    print(r.stdout.strip().splitlines()[-1])
-
-
 # ============================================================================= coverage of the path table
 def test_every_path_is_covered():
     hit = set()
@@ -623,6 +588,4 @@ def test_every_path_is_covered():
         hit |= make_pixlin(c, 0, with_ref=False)[2]
     for c in CONV_CASES + BENCH_CONV:
         hit |= make_conv(c, 0, with_ref=False)[3]
-    for c in PERSIST_CASES:
-        hit |= make_conv(c, 0, persist=True, with_ref=False)[3]
     assert hit == PIXLIN_PATHS | CONV_PATHS, (sorted(PIXLIN_PATHS | CONV_PATHS - hit), sorted(hit - PIXLIN_PATHS - CONV_PATHS))

@@ -9,9 +9,15 @@ fwd_path() / bwd_path() restate the pickers of csrc/scan_fwd_tma.cu (scan_fwd_tm
 csrc/scan_bwd.cu (pick_rb_bwd), csrc/scan_bwd_tma.cu (bwd_tma_ss, grouped_ss) and the vec_ok rules of csrc/api.cu.  A path label
 is the kernel family (gen / tma / grp-tma) with RB and WPC or SS, the MODE (0 plain, 1 checkpoints, 2 grouped, 3 grouped +
 checkpoints), det / atomic, and the in / out dtypes.  Each case names the path it intends and asserts that the mirror agrees;
-test_every_path_is_covered asserts that the cases reach every label.  The knobs VMB_SCAN_TMA, VMB_SCAN_SS, VMB_SCAN_RB,
-VMB_SCAN_WPC, VMB_SCAN_BWD_TMA, VMB_SCAN_SS_BWD and VMB_SCAN_RB_BWD are read on every launch, so monkeypatch.setenv forces a path
-in this process.  The grouped oracle flips the reversed groups into sequence order, runs the flat oracle with one group per
+test_every_path_is_covered asserts that the cases reach every label.  A case reaches its launch configuration through its shape
+(on the H100's 132 SMs):
+  * TMA state split, from rows = batch * dim: forward SS 1 at >= 2112 rows, 2 at 1056 - 2111, 4 below; backward SS 1 at >= 1064,
+    2 at 532 - 1063, 4 below (the grouped backward then grows SS until the CTA's rows divide the group);
+  * generic forward RB, from L at fewer than 1536 rows: 8 at L <= 64, 4 at 65 - 128, 2 at 129 - 256, 1 above; WPC the largest of
+    4 / 2 / 1 whose RB * WPC rows divide the group;
+  * generic backward RB, from rows: 2 below 1536, 4 below 6144, 8 above, halved until it divides the rows per group.
+VMB_SCAN_TMA=0 / VMB_SCAN_BWD_TMA=0 (read on every launch, set with monkeypatch.setenv) put TMA-eligible shapes on the generic
+kernels.  The grouped oracle flips the reversed groups into sequence order, runs the flat oracle with one group per
 direction and flips the results back.  The worst err / bound per path is printed at the end of the module.
 """
 import os
@@ -31,8 +37,7 @@ BF16, F16, F32 = torch.bfloat16, torch.float16, torch.float32
 DTYPES = [F32, BF16, F16]
 T, CKPT = 16, 64  # kScanT, kScanCkpt (csrc/scan_params.h)
 RATIOS = {}  # path -> largest err / bound seen
-KNOBS = ("VMB_SCAN_TMA", "VMB_SCAN_SS", "VMB_SCAN_RB", "VMB_SCAN_WPC", "VMB_SCAN_BWD_TMA", "VMB_SCAN_SS_BWD", "VMB_SCAN_RB_BWD",
-         "VMB_SCAN_BWD_TMA_F32")
+KNOBS = ("VMB_SCAN_TMA", "VMB_SCAN_BWD_TMA", "VMB_SCAN_BWD_TMA_F32")
 
 
 def sms():
@@ -74,8 +79,6 @@ def fwd_path(batch, dim, L, N, G, dtype, vec_ok, grouped, ckpt, out_f32=False):
         ss = 1
         while ss < 4 and rows // 2 * ss < 8 * sms():
             ss <<= 1
-        if _env("VMB_SCAN_SS") in (1, 2, 4):
-            ss = _env("VMB_SCAN_SS")
         if rpg % (2 * 4 // ss) == 0:
             return f"fwd-tma-ss{ss}-m{mode}-{io}"
     if grouped:
@@ -86,17 +89,11 @@ def fwd_path(batch, dim, L, N, G, dtype, vec_ok, grouped, ckpt, out_f32=False):
         rb >>= 1
     while rb < 8 and rpg % (rb * 2) == 0 and (32 // rb) * T >= 2 * L:
         rb *= 2
-    e = _env("VMB_SCAN_RB", 0)
-    if 0 < e <= 8 and e & (e - 1) == 0 and rpg % e == 0:
-        rb = e
     if grouped and ckpt and rb > 2:
         rb = 2
     wpc = 4
     while wpc > 1 and rpg % (rb * wpc):
         wpc >>= 1
-    e = _env("VMB_SCAN_WPC", 0)
-    if e > 0 and e & (e - 1) == 0 and rpg % (rb * e) == 0 and e <= 4:
-        wpc = e
     return f"fwd-gen-rb{rb}-wpc{wpc}-m{mode}-{io}"
 
 
@@ -104,8 +101,6 @@ def bwd_tma_ss(batch, dim):
     rows, ss = batch * dim, 1
     while ss < 4 and rows // (2 * 4 // ss) * 2 <= 2 * sms():
         ss <<= 1
-    if _env("VMB_SCAN_SS_BWD") in (1, 2, 4):
-        ss = _env("VMB_SCAN_SS_BWD")
     return ss
 
 
@@ -125,15 +120,10 @@ def bwd_path(batch, dim, L, N, G, dtype, vec_ok, grouped, ckpt, det, dout_f32=Fa
         ss = bwd_tma_ss(batch, dim)
         if rpg % (2 * 4 // ss) == 0:
             return f"bwd-tma-ss{ss}-{d}-{io}", 8 // ss
-    rb = 0
-    e = _env("VMB_SCAN_RB_BWD", 0)
-    if 0 < e <= 8 and e & (e - 1) == 0 and rpg % e == 0:
-        rb = e
-    if not rb:
-        rows = batch * dim
-        rb = 2 if rows < 1536 else 4 if rows < 6144 else 8
-        while rb > 1 and rpg % rb:
-            rb >>= 1
+    rows = batch * dim
+    rb = 2 if rows < 1536 else 4 if rows < 6144 else 8
+    while rb > 1 and rpg % rb:
+        rb >>= 1
     return f"bwd-gen-rb{rb}-{d}-{io}", rb
 
 
@@ -169,77 +159,93 @@ def all_paths():
 
 
 # ============================================================================= cases
-# kind: "flat" / "grouped"; bwd: also run the backward on the forward's checkpoints (None: forward only, else det 0 / 1)
+# kind: "flat" / "grouped"; bwd: None runs the forward only, 0 / 1 also the backward (atomic / det) on the forward's checkpoints,
+#       CKPT_ONLY the forward with checkpoints but no backward (the grouped backward needs an even number of rows per group)
 # layout: "dense" / "strided" (u, delta, dout channel slices of wider buffers, B and C halves of one (B, G, 2N, L) buffer) /
 #         "misaligned" (flat: u one element into its storage -> no 16 B rows)
 # env: knobs; expect: (forward label, backward label or None) the case is written for, None where the natural path is recorded
 Case = namedtuple("Case", "kind dtype b D L N G env bwd layout out_f32 model expect")
 Case.__new__.__defaults__ = ("dense", False, False, None)
+CKPT_ONLY = -1
 
 
 def case_id(c):
     env = "-".join(f"{k[9:].lower()}{v}" for k, v in sorted(c.env.items()))
+    bwd = "" if c.bwd is None else "-ckpt" if c.bwd == CKPT_ONLY else "-det" if c.bwd else "-atomic"
     return (f"{c.kind}-{dname(c.dtype)}{'-f32out' if c.out_f32 else ''}-b{c.b}-D{c.D}-L{c.L}-N{c.N}-G{c.G}-{c.layout}"
-            f"{'-model' if c.model else ''}{'' if c.bwd is None else ('-det' if c.bwd else '-atomic')}{'-' + env if env else ''}")
+            f"{'-model' if c.model else ''}{bwd}{'-' + env if env else ''}")
+
+
+def gen_rpg(rb, wpc):
+    """rows per group on which the generic forward's picker, once RB is reached, keeps it and takes WPC: RB * WPC divides them,
+    and (WPC < 4) 2 * RB * WPC does not"""
+    return rb * wpc * (1 if wpc == 4 else 3)
+
+
+# (L, N) per generic forward RB at few rows: L in that RB's range; L >= 512 only with dstate > 16 or an odd L (no 16 B rows),
+# which keep the TMA kernel off
+GEN_LN = {1: [(300, 16), (4104, 17), (1001, 15), (511, 1)], 2: [(200, 16), (129, 15), (256, 17), (136, 1)],
+          4: [(100, 16), (65, 15), (128, 17), (72, 1)], 8: [(64, 16), (33, 15), (16, 17), (40, 1)]}
 
 
 def matrix():
     cs = []
-    Ls = [520, 1000, 4104, 512]
-    Ns = [16, 15, 17, 1]
     for dt in DTYPES:
         ofs = [False] + ([True] if dt != F32 else [])
         for of in ofs:
             io = dname(dt) + ("-f32out" if of else "")
             gio = dname(dt) + ("-f32dout" if of else "")
-            # generic forward: every (RB, WPC), MODE 0 and 1; MODE 1 runs the generic backward at the same RB
+            # generic forward: every (RB, WPC), MODE 0 and 1; MODE 1 runs the generic backward (RB 2, or 1 at odd rows per group)
             i = 0
             for rb in (1, 2, 4, 8):
                 for wpc in (1, 2, 4):
                     for ck in (0, 1):
                         i += 1
                         det = (rb + wpc + ck) % 2
-                        L, N = (Ls[i % 4], Ns[i % 4]) if not of else (1000, 16)
-                        env = dict(VMB_SCAN_TMA=0, VMB_SCAN_RB=rb, VMB_SCAN_WPC=wpc, VMB_SCAN_BWD_TMA=0, VMB_SCAN_RB_BWD=rb)
-                        exp_b = f"bwd-gen-rb{rb}-{'det' if det else 'atomic'}-{gio}" if ck else None
-                        cs.append(Case("flat", dt, 1, 64, L, N, 2, env, det if ck else None, "strided" if i % 3 == 0 else "dense",
+                        rpg = gen_rpg(rb, wpc)
+                        L, N = GEN_LN[rb][(i + rb) % 4] if not of else (GEN_LN[rb][0][0], 16)
+                        exp_b = f"bwd-gen-rb{1 if rpg % 2 else 2}-{'det' if det else 'atomic'}-{gio}" if ck else None
+                        cs.append(Case("flat", dt, 1, 2 * rpg, L, N, 2, {}, det if ck else None, "strided" if i % 3 == 0 else "dense",
                                        of, i % 5 == 0, (f"fwd-gen-rb{rb}-wpc{wpc}-m{ck}-{io}", exp_b)))
-            # generic backward with the atomic / det mode the loop above did not give each RB
-            for rb in (1, 2, 4, 8):
+            # generic backward at each RB, atomic and det: RB 1 from an odd rows per group, 2 / 4 / 8 from the row count
+            for rb, b, D, L, fwd in ((1, 2, 20, 65, "rb1-wpc1"), (2, 2, 32, 511, "rb1-wpc4"), (4, 16, 128, 65, "rb4-wpc4"),
+                                     (8, 48, 128, 65, "rb4-wpc4")):
                 for det in (0, 1):
-                    env = dict(VMB_SCAN_TMA=0, VMB_SCAN_RB=2, VMB_SCAN_WPC=1, VMB_SCAN_BWD_TMA=0, VMB_SCAN_RB_BWD=rb)
-                    cs.append(Case("flat", dt, 2, 32, 65 if rb % 2 else 511, 16, 4, env, det, "dense", of, False,
-                                   (f"fwd-gen-rb2-wpc1-m1-{io}", f"bwd-gen-rb{rb}-{'det' if det else 'atomic'}-{gio}")))
-            # TMA forward: SS 1 / 2 / 4, MODE 0 and 1; MODE 1 runs the TMA backward at the same SS, atomic and det
-            for ss in (1, 2, 4):
-                env = dict(VMB_SCAN_SS=ss, VMB_SCAN_SS_BWD=ss)
-                L = (512, 4104, 1000)[ss // 2]
-                cs.append(Case("flat", dt, 2, 48, L, 16, 2, env, None, "dense", of, ss == 2, (f"fwd-tma-ss{ss}-m0-{io}", None)))
-                for det in (0, 1):
-                    cs.append(Case("flat", dt, 2, 48, (520, 4104)[det], 16, 2, env, det, "strided" if det else "dense", of,
-                                   ss == 4, (f"fwd-tma-ss{ss}-m1-{io}", f"bwd-tma-ss{ss}-{'det' if det else 'atomic'}-{gio}")))
-        # grouped, generic forward: every (RB, WPC) at MODE 2, RB <= 2 at MODE 3 (clamped there: RB 4 / 8 are not instantiated)
-        for rb in (1, 2, 4, 8):
-            for wpc in (1, 2, 4):
-                env = dict(VMB_SCAN_TMA=0, VMB_SCAN_RB=rb, VMB_SCAN_WPC=wpc)
-                L = (64, 520, 1000)[(rb + wpc) % 3]
-                cs.append(Case("grouped", dt, 1, 4 * 32, L, 16 if wpc != 2 else 15, 4, env, None, "strided", False, rb == 4,
+                    cs.append(Case("flat", dt, b, D, L, 16, 4, {}, det, "dense", of, False,
+                                   (f"fwd-gen-{fwd}-m1-{io}", f"bwd-gen-rb{rb}-{'det' if det else 'atomic'}-{gio}")))
+            # TMA forward: SS 4 / 2 / 1 at 384 / 1536 / 3072 rows, MODE 0 and 1; MODE 1 runs the TMA backward, whose SS steps at
+            # other row counts: 384 rows -> SS 4, 768 -> 2 (forward 4), 1536 and 3072 -> 1
+            for D, L, ss in ((192, 1000, 4), (768, 512, 2), (1536, 520, 1)):
+                cs.append(Case("flat", dt, 2, D, L, 16, 2, {}, None, "dense", of, ss == 2, (f"fwd-tma-ss{ss}-m0-{io}", None)))
+            for D, L, fss, bss, dets in ((192, 4104, 4, 4, (0, 1)), (384, 1000, 4, 2, (0, 1)), (768, 520, 2, 1, (0, 1)),
+                                         (1536, 512, 1, 1, (1,))):
+                for det in dets:
+                    cs.append(Case("flat", dt, 2, D, L, 16, 2, {}, det, "strided" if det else "dense", of, fss == 4 and det == 1,
+                                   (f"fwd-tma-ss{fss}-m1-{io}", f"bwd-tma-ss{bss}-{'det' if det else 'atomic'}-{gio}")))
+        # grouped, generic forward: every (RB, WPC) at MODE 2; L < 512 or dstate 15 keeps it off the TMA kernel
+        for rb, Ls in ((1, (264, 520, 1000)), (2, (136, 200, 256)), (4, (72, 96, 128)), (8, (8, 32, 64))):
+            for wpc, L in zip((1, 2, 4), Ls):
+                N = 15 if wpc == 2 or L >= 512 else 16
+                cs.append(Case("grouped", dt, 1, 4 * gen_rpg(rb, wpc), L, N, 4, {}, None, "strided", False, rb == 4,
                                (f"fwd-gen-rb{rb}-wpc{wpc}-m2-{dname(dt)}", None)))
-                if rb <= 4:
-                    rbe = min(rb, 2)
-                    det = (rb + wpc) % 2
-                    ss = 4 if wpc == 4 else 2
-                    env = dict(env, VMB_SCAN_SS_BWD=ss)
-                    cs.append(Case("grouped", dt, 1, 4 * 32, (520, 1000, 64)[wpc // 2], 16, 4, env, det, "strided", False, False,
-                                   (f"fwd-gen-rb{rbe}-wpc{wpc}-m3-{dname(dt)}", f"bwd-grp-tma-ss{ss}-{'det' if det else 'atomic'}-{dname(dt)}")))
-        # grouped, TMA forward: SS 1 / 2 / 4, MODE 2 and 3, with the grouped backward at the same SS (atomic and det)
-        for ss in (1, 2, 4):
-            env = dict(VMB_SCAN_SS=ss, VMB_SCAN_SS_BWD=ss)
-            cs.append(Case("grouped", dt, 1, 4 * 16, (512, 1000, 4104)[ss // 2], 16, 4, env, None, "strided", False, ss == 1,
+        # grouped, generic forward with checkpoints (MODE 3, RB <= 2: the last two shapes pick RB 4 / 8, clamped to 2 there), with
+        # the grouped backward at SS 4 (few rows); RB 1 at WPC 1 needs an odd rows per group, which the backward does not take
+        for k, (rb, wpc, R, L) in enumerate(((1, 1, 3, 400), (1, 2, 6, 520), (1, 4, 4, 1000), (2, 1, 6, 200), (2, 2, 12, 136),
+                                             (2, 4, 8, 256), (2, 2, 12, 128), (2, 4, 16, 64))):
+            det = k % 2 if R % 2 == 0 else CKPT_ONLY
+            exp_b = None if det == CKPT_ONLY else f"bwd-grp-tma-ss4-{'det' if det else 'atomic'}-{dname(dt)}"
+            cs.append(Case("grouped", dt, 1, 4 * R, L, 15 if L >= 512 else 16, 4, {}, det, "strided", False, False,
+                           (f"fwd-gen-rb{rb}-wpc{wpc}-m3-{dname(dt)}", exp_b)))
+        # grouped, TMA forward: SS 4 / 2 / 1 by rows, MODE 2 and 3; MODE 3 runs the grouped backward (atomic and det) at the SS of
+        # its own row steps, as the flat one
+        for b, R, L, ss in ((1, 16, 512, 4), (2, 192, 1000, 2), (4, 192, 520, 1)):
+            cs.append(Case("grouped", dt, b, 4 * R, L, 16, 4, {}, None, "strided", False, ss == 1,
                            (f"fwd-tma-ss{ss}-m2-{dname(dt)}", None)))
-            for det in (0, 1):
-                cs.append(Case("grouped", dt, 2, 4 * 8, (4104, 520)[det], 16, 4, env, det, "strided", False, det == 1,
-                               (f"fwd-tma-ss{ss}-m3-{dname(dt)}", f"bwd-grp-tma-ss{ss}-{'det' if det else 'atomic'}-{dname(dt)}")))
+        for b, R, L, fss, bss, dets in ((2, 48, 4104, 4, 4, (0, 1)), (2, 96, 1000, 4, 2, (0, 1)), (2, 192, 520, 2, 1, (0, 1)),
+                                        (4, 192, 512, 1, 1, (0,))):
+            for det in dets:
+                cs.append(Case("grouped", dt, b, 4 * R, L, 16, 4, {}, det, "strided", False, det == 1,
+                               (f"fwd-tma-ss{fss}-m3-{dname(dt)}", f"bwd-grp-tma-ss{bss}-{'det' if det else 'atomic'}-{dname(dt)}")))
         # the grouped backward at short L (always the TMA kernel, zero-filled boxes past the end) and its natural SS
         for det in (0, 1):
             cs.append(Case("grouped", dt, 1, 4 * 6, 64, 16, 4, {}, det, "strided", False, False, None))
@@ -258,14 +264,19 @@ def edges():
     for i, N in enumerate(Ns):
         dt = DTYPES[(i + 1) % 3]
         cs.append(Case("flat", dt, 1, 16, 1000 if N < 64 else 300, N, 2, {}, i % 2, "dense", dt != F32 and i % 2 == 0, i % 3 == 0))
-    for rb in (1, 2, 4, 8):  # dstate 256 on every generic RB, forward and backward
-        cs.append(Case("flat", BF16, 1, 16, 200, 256, 2, dict(VMB_SCAN_RB=rb, VMB_SCAN_RB_BWD=rb), 1, "dense", False, True, None))
+    # dstate 256 on every generic RB, forward (RB from L) and backward (RB from rows): 9 rows per group -> RB 1 both ways
+    for rb, wpc, b, D, L in ((1, 1, 1, 18, 300), (2, 4, 1, 16, 200), (4, 4, 6, 256, 72), (8, 4, 24, 256, 16)):
+        cs.append(Case("flat", BF16, b, D, L, 256, 2, {}, 1, "dense", False, True,
+                       (f"fwd-gen-rb{rb}-wpc{wpc}-m1-bf16", f"bwd-gen-rb{rb}-det-bf16")))
     cs += [Case("flat", BF16, 2, 18, 1000, 16, 3, {}, 0, "dense", False, False, None),         # 6 rows per group: TMA at SS 4
            Case("flat", F16, 1, 9, 1000, 16, 3, {}, 1, "strided", False, False, None),         # 3 rows per group (odd): generic
            Case("flat", F32, 1, 15, 4104, 16, 5, {}, 0, "dense", False, True, None),           # 3 rows per group, long
            Case("flat", BF16, 2, 16, 1000, 16, 2, {}, 1, "misaligned", False, False, None),    # no 16 B rows: generic
            Case("flat", F16, 2, 16, 1001, 16, 2, {}, 0, "dense", False, False, None),          # odd L: no 16 B rows
            Case("flat", BF16, 8, 384, 1000, 16, 4, {}, 1, "dense", False, True, None),         # SS = 1 by the SM count
+           # a TMA shape on the generic kernels (the switches): RB 2 forward at L = 520, RB 4 backward at 2048 rows
+           Case("flat", BF16, 2, 1024, 520, 16, 2, dict(VMB_SCAN_TMA=0, VMB_SCAN_BWD_TMA=0), 1, "strided", False, True,
+                ("fwd-gen-rb2-wpc4-m1-bf16", "bwd-gen-rb4-det-bf16")),
            Case("grouped", BF16, 8, 4 * 96, 1000, 16, 4, {}, 0, "strided", False, True, None)]
     return cs
 
@@ -349,7 +360,7 @@ def run_flat(c, monkeypatch, seed):
         assert fp == c.expect[0], (fp, c.expect[0])
     ref, S = cscan.scan_fwd_mag(u, delta, A, Bm, Cm, Dv, bias, sp)
     check(out, ref, S, F32 if c.out_f32 else c.dtype, "out", [fp])
-    if c.bwd is None:
+    if c.bwd is None or c.bwd == CKPT_ONLY:
         return
     grads = ops.selective_scan_bwd(ud, dd, Ad, Bd, Cd, Dd, bd, gd, ck, sp, dout_float=c.out_f32, deterministic=bool(c.bwd))
     bvec = vec and flat_vec_ok([gd], F32 if c.out_f32 else c.dtype)
@@ -406,7 +417,7 @@ def run_grouped(c, monkeypatch, seed):
     ref, S = ref.view(b, G, R, L), S.view(b, G, R, L)
     for g in range(G):
         check(ys[:, g], _seq(ref[:, g], revs[g]), _seq(S[:, g], revs[g]), c.dtype, f"out[{g}]", [fp])
-    if c.bwd is None:
+    if c.bwd is None or c.bwd == CKPT_ONLY:
         return
     gbuf = torch.randn(b, G, R + 8, L).to(c.dtype)
     for g in range(G):

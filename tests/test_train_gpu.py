@@ -101,7 +101,7 @@ def test_side_stream_weight_gradients_equal_single_stream_on_a_net(amp):
     """the weight-gradient kernels on the second stream (fused_train._Side) vs everything on one stream: a 4-level net with FlatAdam's
     flat gradient buffer, eager and replayed from a CUDA graph.  fp32 activations: only the order of the fp32 atomic adds differs
     (1e-4); bf16 autocast: the forward itself is reproducible only up to bf16 rounding flips behind the out_norm statistics'
-    atomics (tools/side_debug.py: 0 ... 2e-3 on the output, 2e-3 ... 1e-2 on the gradients between identical single-stream runs),
+    atomics (0 ... 2e-3 on the output, 2e-3 ... 1e-2 on the gradients between identical single-stream runs),
     so that case only guards against gross errors (a missing or doubled weight gradient is O(1))."""
     import torch.nn.functional as F
     from vmambair_b200 import fused_train

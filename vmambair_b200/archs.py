@@ -19,13 +19,12 @@ Three execution paths share the parameters, for MamberBlock and for a standalone
   * `fused_train` (CUDA, grad enabled; default): the fused stages with their hand-written backward kernels
     (vmambair_b200.fused_train);
   * `compose`: the same math composed from torch ops + this repo's selective-scan operator with autograd
-    (VMB_TRAIN_PATH=compose / set_train_path; the module-level cross-check and the fallback for unsupported shapes).
+    (set_train_path("compose"); the module-level cross-check and the fallback for unsupported shapes).
 """
 from __future__ import annotations
 
 import math
 import numbers
-import os
 import warnings
 
 import torch
@@ -35,7 +34,7 @@ import torch.nn.functional as F
 from .selective_scan import selective_scan_fn
 
 # training path: "fused" = fused_train (native forward + backward kernels); "compose" = torch ops + the scan operator (round 1)
-_TRAIN_PATH = os.environ.get("VMB_TRAIN_PATH", "fused")
+_TRAIN_PATH = "fused"
 
 
 def set_train_path(path: str) -> None:
@@ -309,7 +308,7 @@ _FUSED_DET_MSG = (
     "torch.use_deterministic_algorithms(True) is on, but MamberBlock runs its fused path, which is not bitwise reproducible: "
     "the fused training step's backward accumulates in fp32 atomics (the train_ops.cu and channel_bwd.cu kernels, the scan and "
     "the wgrad parameter phases), and inference computes the merge statistics in two kernels with atomics.  For reproducible "
-    "training set VMB_TRAIN_PATH=compose (or archs.set_train_path('compose')): torch ops plus this library's deterministic "
+    "training call archs.set_train_path('compose'): torch ops plus this library's deterministic "
     "selective-scan backward.")
 
 

@@ -284,22 +284,11 @@ __global__ void __launch_bounds__(128) conv3x3_tma_kernel(const Conv3Params p, c
     uint64_t* full = reinterpret_cast<uint64_t*>(Bt + Cfg::BT_BYTES);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int tiles_x = (p.W + kTW - 1) / kTW, tiles_xy = tiles_x * ((p.H + kTH - 1) / kTH);
-    const int ntile = tiles_xy * p.B;              // pixel tiles of the whole batch
+    // one pixel tile per CTA: grid.x walks the tiles of the whole batch
+    const int b = blockIdx.x / tiles_xy, tile = blockIdx.x % tiles_xy;
+    const int x0 = (tile % tiles_x) * kTW, y0 = (tile / tiles_x) * kTH;
     const int m0 = blockIdx.y * MT;
     const int nchunk = (p.Cin + 15) / 16;
-    // persistent over pixel tiles: this CTA owns tiles blockIdx.x, + gridDim.x, ...; the (tile, chunk) pairs form ONE stream of
-    // iterations through the stage ring, so the boxes of the next tile are in flight while this tile is multiplied and stored
-    // (launched with one tile per CTA by default, see launch_tma)
-    const int my_tiles = (ntile - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
-    const int total_it = my_tiles * nchunk;
-    auto tile_of = [&](int it, int& x0, int& y0, int& b, int& kc) {
-        const int T = blockIdx.x + (it / nchunk) * gridDim.x;
-        kc = it % nchunk;
-        b = T / tiles_xy;
-        const int r = T % tiles_xy;
-        x0 = (r % tiles_x) * kTW;
-        y0 = (r / tiles_x) * kTH;
-    };
 
     if (tid == 0) {
 #pragma unroll
@@ -309,13 +298,11 @@ __global__ void __launch_bounds__(128) conv3x3_tma_kernel(const Conv3Params p, c
     __syncthreads();
     // one stage = the weights box + the input box on one mbarrier; the weights are static parameters, so the boxes of the first
     // STAGES chunks are requested while the preceding kernel of the stream is still draining (PDL), the activations after it
-    auto issue_w = [&](int it, int s) {
+    auto issue_w = [&](int kc, int s) {
         mbarrier_expect_tx(&full[s], Cfg::A_BYTES + Cfg::B_BYTES);
-        tma_load_4d(smem + s * Cfg::STAGE, &mapW, &full[s], (it % nchunk) * 16, m0, 0, 0);
+        tma_load_4d(smem + s * Cfg::STAGE, &mapW, &full[s], kc * 16, m0, 0, 0);
     };
-    auto issue_x = [&](int it, int s) {
-        int x0, y0, b, kc;
-        tile_of(it, x0, y0, b, kc);
+    auto issue_x = [&](int kc, int s) {
         unsigned char* dst = smem + s * Cfg::STAGE + Cfg::A_BYTES;
         if constexpr (NHWC) tma_load_4d(dst, &mapX, &full[s], kc * 16, x0 - 1, y0 - 1, b);
         else tma_load_4d(dst, &mapX, &full[s], x0 - kRawX, y0 - 1, kc * 16, b);
@@ -323,13 +310,13 @@ __global__ void __launch_bounds__(128) conv3x3_tma_kernel(const Conv3Params p, c
     if (tid == 0) {
 #pragma unroll
         for (int s = 0; s < STAGES; ++s)
-            if (s < total_it) issue_w(s, s);
+            if (s < nchunk) issue_w(s, s);
     }
     pdl_wait();
     if (tid == 0) {
 #pragma unroll
         for (int s = 0; s < STAGES; ++s)
-            if (s < total_it) issue_x(s, s);
+            if (s < nchunk) issue_x(s, s);
     }
 
     float acc[MI][4][4];
@@ -357,26 +344,18 @@ __global__ void __launch_bounds__(128) conv3x3_tma_kernel(const Conv3Params p, c
     // 32-bit stores need even element offsets: W % 4 == 0 (true on this path), even strides, 4 B-aligned base
     const bool pair_ok = p.W % 4 == 0 && p.o_bs % 2 == 0 && p.o_cs % 2 == 0 && (reinterpret_cast<uintptr_t>(p.out) & 3) == 0;
 
-    int x0 = 0, y0 = 0, b = 0, kc = -1;
-    bool jok[4] = {false, false, false, false};  // n-tiles inside the image (warp-uniform): the others are skipped
-    for (int it = 0; it < total_it; ++it) {
-        if (++kc == nchunk) kc = 0;
-        {
-            if (kc == 0) {  // a new pixel tile
-                int k0;
-                tile_of(it, x0, y0, b, k0);
+    bool jok[4];  // n-tiles inside the image (warp-uniform): the others are skipped
 #pragma unroll
-                for (int j = 0; j < 4; ++j) jok[j] = (y0 + trow0 + (j >> 1) < p.H) && (x0 + (j & 1) * 8 < p.W);
+    for (int j = 0; j < 4; ++j) jok[j] = (y0 + trow0 + (j >> 1) < p.H) && (x0 + (j & 1) * 8 < p.W);
 #pragma unroll
-                for (int i = 0; i < MI; ++i)
+    for (int i = 0; i < MI; ++i)
 #pragma unroll
-                    for (int j = 0; j < 4; ++j)
+        for (int j = 0; j < 4; ++j)
 #pragma unroll
-                        for (int e = 0; e < 4; ++e) acc[i][j][e] = 0.f;
-            }
-        }
-        const int slot = it % STAGES;
-        mbarrier_wait(&full[slot], (it / STAGES) & 1);
+            for (int e = 0; e < 4; ++e) acc[i][j][e] = 0.f;
+    for (int kc = 0; kc < nchunk; ++kc) {
+        const int slot = kc % STAGES;
+        mbarrier_wait(&full[slot], (kc / STAGES) & 1);
         const unsigned char* A = smem + slot * Cfg::STAGE;
         const unsigned char* Braw = A + Cfg::A_BYTES;
         if constexpr (!NHWC) {
@@ -417,22 +396,20 @@ __global__ void __launch_bounds__(128) conv3x3_tma_kernel(const Conv3Params p, c
             }
         }
         __syncthreads();  // every warp is done with this stage (and with Bt)
-        if (tid == 0 && it + STAGES < total_it) {
+        if (tid == 0 && kc + STAGES < nchunk) {
             fence_proxy_async();  // the stage was read through the generic proxy; the refill writes through the async proxy
-            issue_w(it + STAGES, slot);
-            issue_x(it + STAGES, slot);
-        }
-        if (kc == nchunk - 1) {  // tile finished: store it (the next tile's boxes are already on their way)
-#pragma unroll
-            for (int mi = 0; mi < MI; ++mi)
-#pragma unroll
-                for (int j = 0; j < 4; ++j)
-#pragma unroll
-                    for (int h = 0; h < 2; ++h)
-                        conv_store_frag<T>(p, b, m0 + mi * 16 + g + h * 8, y0 + trow0 + (j >> 1), x0 + (j & 1) * 8 + 2 * t,
-                                           acc[mi][j][2 * h], acc[mi][j][2 * h + 1], pair_ok, lane);
+            issue_w(kc + STAGES, slot);
+            issue_x(kc + STAGES, slot);
         }
     }
+#pragma unroll
+    for (int mi = 0; mi < MI; ++mi)
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+                conv_store_frag<T>(p, b, m0 + mi * 16 + g + h * 8, y0 + trow0 + (j >> 1), x0 + (j & 1) * 8 + 2 * t,
+                                   acc[mi][j][2 * h], acc[mi][j][2 * h + 1], pair_ok, lane);
 }
 
 // ---- fp32 I/O (parity mode): direct FFMA convolution, one output pixel x 16 output channels per thread ---------------------
@@ -524,19 +501,9 @@ int launch_tma(const Conv3Params& p, int dtype, cudaStream_t stream) {
     }
     auto kern = conv3x3_tma_kernel<T, MT, STAGES, NHWC>;
     VMB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));  // per device: set at every launch
-    // pixel tiles of the whole batch on grid.x, one CTA per tile.  The kernel can also walk several tiles per CTA (grid.x < ntile:
-    // one stream of (tile, chunk) iterations through the stage ring) -- it stays off by default (VMB_CONV_PERSIST=1 turns it on for
-    // problems beyond 3 resident waves)
-    const int ntile = cdiv(p.W, kTW) * cdiv(p.H, kTH) * p.B, mt = cdiv(p.Cout, MT);
-    int gx = ntile;
-    static const bool persist = [] { const char* e = getenv("VMB_CONV_PERSIST"); return e && atoi(e) == 1; }();
-    if (persist) {
-        const int per_sm = (227 * 1024) / SMEM > 0 ? (227 * 1024) / SMEM : 1;
-        int cap = num_sms() * (per_sm > 8 ? 8 : per_sm) / mt;
-        if (cap < 1) cap = 1;
-        if (ntile > 3 * cap) gx = cap;
-    }
-    VMB_CUDA(launch_pdl(kern, dim3(gx, mt, 1), dim3(128), SMEM, stream, p, mapW, mapX));
+    // pixel tiles of the whole batch on grid.x, one CTA per tile
+    const int ntile = cdiv(p.W, kTW) * cdiv(p.H, kTH) * p.B;
+    VMB_CUDA(launch_pdl(kern, dim3(ntile, cdiv(p.Cout, MT), 1), dim3(128), SMEM, stream, p, mapW, mapX));
     return VMB_OK;
 }
 

@@ -470,10 +470,6 @@ static int launch_cfg(const ScanBwdParams& p, cudaStream_t stream) {
 // warp-chunks must be a multiple of the checkpoint interval (64): RB in {8,4,2,1}
 static int pick_rb_bwd(const ScanBwdParams& p) {
     const int rpg = p.rows_per_group;
-    if (const char* e = getenv("VMB_SCAN_RB_BWD")) {
-        const int rb = atoi(e);
-        if (rb > 0 && rb <= 8 && (rb & (rb - 1)) == 0 && rpg % rb == 0) return rb;
-    }
     // few rows -> fewer rows per warp (more warps; their smem footprint still allows >= 3 warps per SM at RB=2)
     const long rows = (long)p.batch * p.dim;
     int rb = rows < 1536 ? 2 : rows < 6144 ? 4 : 8;

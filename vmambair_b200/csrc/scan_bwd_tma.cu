@@ -531,15 +531,11 @@ static int bwd_tma_ss(const ScanBwdParams& p, int rb) {
     const long rows = (long)p.batch * p.dim;
     int ss = 1;
     while (ss < 4 && rows / (rb * 4 / ss) * 2 <= 2L * num_sms()) ss <<= 1;
-    if (const char* v = getenv("VMB_SCAN_SS_BWD")) {
-        const int x = atoi(v);
-        if (x == 1 || x == 2 || x == 4) ss = x;
-    }
     return ss;
 }
 
 // (rows per warp, state split): RB = 2 at every batch; the state split while the CTAs still fit one resident wave
-// (tools/scan_bwd_sweep.py sweeps it)
+// (DESIGN §1.2)
 bool scan_bwd_tma_pick(const ScanBwdParams& p, int dtype, int& rb, int& ss) {
     const char* e = getenv("VMB_SCAN_BWD_TMA");
     if (e && atoi(e) == 0) return false;

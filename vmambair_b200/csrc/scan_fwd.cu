@@ -379,19 +379,14 @@ static int launch_cfg(const ScanFwdParams& p, int ext, cudaStream_t stream) {
 static void pick_cfg(const ScanFwdParams& p, int& rb, int& wpc) {
     const int rpg = p.rows_per_group;
     const long rows = (long)p.batch * p.dim;
-    int env_rb = 0, env_wpc = 0;
-    if (const char* e = getenv("VMB_SCAN_RB")) env_rb = atoi(e);
-    if (const char* e = getenv("VMB_SCAN_WPC")) env_wpc = atoi(e);
     // aim for >= ~1500 warps, then grow RB for cheaper scans (tools/scan_sustained.py sweeps RB per shape)
     rb = rows < 1536 ? 1 : rows < 8192 ? 2 : rows < 32768 ? 4 : 8;
     while (rb > 1 && rpg % rb) rb >>= 1;
     // short sequences: a warp-chunk should not be much longer than L
     while (rb < 8 && rpg % (rb * 2) == 0 && (32 / rb) * T >= 2 * p.L) rb *= 2;
-    if (env_rb > 0 && env_rb <= 8 && (env_rb & (env_rb - 1)) == 0 && rpg % env_rb == 0) rb = env_rb;
     if (p.ndesc && p.ckpt && rb > 2) rb = 2;  // grouped + checkpoints (MODE 3) is instantiated at RB <= 2 only: RB 4 / 8 spill
     wpc = 4;
     while (wpc > 1 && (rpg % (rb * wpc) != 0)) wpc >>= 1;
-    if (env_wpc > 0 && (env_wpc & (env_wpc - 1)) == 0 && rpg % (rb * env_wpc) == 0 && env_wpc <= 4) wpc = env_wpc;
 }
 
 template <typename in_t, int RB, typename out_t>

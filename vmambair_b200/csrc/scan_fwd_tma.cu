@@ -419,7 +419,7 @@ static int launch_tma2(const ScanFwdParams& p, const ScanTmaMaps& maps, int ss, 
 
 template <typename in_t, typename out_t = in_t>
 static int launch_tma1(const ScanFwdParams& p, const ScanTmaMaps& maps, int ss, int ext, cudaStream_t stream) {
-    // rows per warp: 2 (scan_fwd_tma_pick; tools/scan_sweep.py: RB = 4 / 8 lose at every batch size, not instantiated)
+    // rows per warp: 2 (scan_fwd_tma_pick; DESIGN §1.1: RB = 4 / 8 lose at every batch size, not instantiated)
     return launch_tma2<in_t, 2, out_t>(p, maps, ss, ext, stream);
 }
 
@@ -432,15 +432,11 @@ bool scan_fwd_tma_pick(const ScanFwdParams& p, int& rb, int& ss) {
     const int rpg = p.rows_per_group;
     const long rows = (long)p.batch * p.dim;
     const long want = 8L * num_sms();  // >= 2 warps per scheduler
-    // rb = 2 at every batch size (tools/scan_sweep.py sweeps it): with more rows per warp the B/C tile reads shrink but the warp
-    // count drops, and the MUFU + LDS + SHFL instructions of a warp all queue on one path
+    // rb = 2 at every batch size (DESIGN §1.1): with more rows per warp the B/C tile reads shrink but the warp count drops, and
+    // the MUFU + LDS + SHFL instructions of a warp all queue on one path
     rb = 2;
     ss = 1;
     while (ss < 4 && rows / rb * ss < want) ss <<= 1;
-    if (const char* v = getenv("VMB_SCAN_SS")) {
-        const int x = atoi(v);
-        if (x == 1 || x == 2 || x == 4) ss = x;
-    }
     return rpg % (rb * kTmaWarps / ss) == 0;
 }
 

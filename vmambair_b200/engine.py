@@ -6,7 +6,6 @@ makes to upscale a batch of LQ tiles (host tensor in, host tensor out).
 from __future__ import annotations
 
 import copy
-import os
 
 import torch
 
@@ -65,8 +64,6 @@ class InferenceEngine:
         every launch there a fraction of a wave) run as that many parallel sub-batch branches; the full-resolution
         stages, which fill the GPU on their own, keep the whole batch."""
         self.device = torch.device(device)
-        if os.environ.get("VMB_CUDNN_BENCHMARK", "0") == "1":
-            torch.backends.cudnn.benchmark = True  # let cuDNN pick the fastest algorithm for the few non-OSS 3x3 convs (static shapes)
         # the caller's module is left untouched (it may be the training replica): the engine owns a cast copy
         self.net = cast_for_inference(copy.deepcopy(net).to(self.device).eval(), dtype)
         self.dtype = dtype

@@ -27,7 +27,6 @@ gradients.  fp32 activations (parity mode) send the weight gradients to the libr
 from __future__ import annotations
 
 import contextlib
-import os
 
 import torch
 
@@ -63,8 +62,7 @@ class _Side:
     stream = {}      # device index -> torch.cuda.Stream
     keep = []        # tensors the side-stream kernels read: kept alive until the join
     armed = False
-    on = os.environ.get("VMB_TRAIN_SIDE", "1") == "1"
-    mask = int(os.environ.get("VMB_SIDE_MASK", "255"))  # debugging: which groups of launches may go to the side stream
+    on = True        # False: everything on the current stream (the single-stream comparison of the tests)
 
 
 def join_side_stream():
@@ -80,9 +78,9 @@ def _side_join():
 
 
 @contextlib.contextmanager
-def _side(ok, dev, *keep, bit=255):
+def _side(ok, dev, *keep):
     """run the enclosed launches on the side stream when `ok` (their results go nowhere but into .grad buffers)"""
-    if not (ok and _Side.on and (_Side.mask & bit) and _DIRECT_GRADS and not torch.is_grad_enabled()):
+    if not (ok and _Side.on and _DIRECT_GRADS and not torch.is_grad_enabled()):
         yield False
         return
     st = _Side.stream.get(dev.index)
@@ -218,7 +216,7 @@ class _Front(torch.autograd.Function):
             dxz = torch.empty_like(xz)  # [d x_pre | d z_pre]
             (g_onw, k_onw), (g_onb, k_onb) = _acc(on_w, Z["onw"]), _acc(on_b, Z["onb"])
             dm = ops.merge_norm_gate_bwd(ws, xz[:, C:], dy2, dpooled, _f32(on_w), _f32(on_b), C, L, dz_out=dxz[:, C:], phase="data")
-            with _side(k_onw and k_onb, dev, ws, xz, dy2, dpooled, bit=32):
+            with _side(k_onw and k_onb, dev, ws, xz, dy2, dpooled):
                 d_onw, d_onb = ops.merge_norm_gate_bwd(ws, xz[:, C:], dy2, dpooled, _f32(on_w), _f32(on_b), C, L, dz_out=None,
                                                        zeroed=(g_onw, g_onb), phase="params")
             dys = ops.cross_scan([dm] * 4, C, H, W)  # gradient of the merged output, gathered into the four scan orders
@@ -237,7 +235,7 @@ class _Front(torch.autograd.Function):
             xw, dtw = x_proj_w.detach(), dt_w.detach()
             gx, gd = getattr(x_proj_w, "grad", None), getattr(dt_w, "grad", None)
             k_big = _DIRECT_GRADS and gx is not None and gd is not None and gx.dtype == gd.dtype == torch.float32 and not torch.is_grad_enabled()
-            with _side(k_big, dev, ddbl, xc, Z["dbig"], bit=1):
+            with _side(k_big, dev, ddbl, xc, Z["dbig"]):
                 dbig = ops.pixlin_wgrad(ddbl, xc, out=Z["dbig"], deterministic=False).view(4, C + 2 * N, C)
                 d_xproj = torch.cat([torch.bmm(dtw.transpose(1, 2), dbig[:, :C]), dbig[:, C:]], 1)  # [W_dt^T dW ; dW[C:]]
                 d_dtw = torch.bmm(dbig[:, :C], xw[:, :R].transpose(1, 2))                            # dW W_x[:R]^T
@@ -248,20 +246,20 @@ class _Front(torch.autograd.Function):
             # depthwise conv + SiLU
             (g_cw, k_cw), (g_cb, k_cb) = _acc(cw, Z["dcw"]), _acc(cb, Z["dcb"])
             dv = ops.dwconv3x3_bwd(xz[:, :C], _f32(cw.view(C, 9)), _f32(cb), dxc, C, H, W, 0, phase="data")
-            with _side(k_cw and (cb is None or k_cb), dev, xz, dv, bit=64):
+            with _side(k_cw and (cb is None or k_cb), dev, xz, dv):
                 d_cw, d_cb = ops.dwconv3x3_bwd(xz[:, :C], _f32(cw.view(C, 9)), _f32(cb), None, C, H, W, 0, zeroed=(g_cw, g_cb),
                                                phase="params", dv=dv)
             ops.dwconv3x3(dv, cwf, None, C, H, W, 2, out=dxz[:, :C])
             # in_conv + norm1
             dxn = ops.pixlin(dxz, WinT)
             (g_win, k_win), (g_bin, k_bin) = _acc(w_in, Z["dwin"]), _acc(b_in, Z["dbin"])
-            with _side(k_win and (b_in is None or k_bin), dev, x3, dxz, bit=2):
+            with _side(k_win and (b_in is None or k_bin), dev, x3, dxz):
                 xn = ops.layernorm_fwd(x3, ln_mode, _f32(n1w), _f32(n1b)) if ln_mode else x3
                 d_win = ops.pixlin_wgrad(dxz, xn, out=g_win, dbias=g_bin, deterministic=False).view_as(w_in)
             (g_n1w, k_n1w), (g_n1b, k_n1b) = _acc(n1w, Z["n1w"]), _acc(n1b, Z["n1b"])
             if ln_mode:
                 dx, st1 = ops.layernorm_bwd(x3, dxn, ln_mode, _f32(n1w), phase="data")
-                with _side(k_n1w and (n1b is None or k_n1b), dev, x3, dxn, st1, bit=128):
+                with _side(k_n1w and (n1b is None or k_n1b), dev, x3, dxn, st1):
                     d_n1w, d_n1b = ops.layernorm_bwd(x3, dxn, ln_mode, _f32(n1w), zeroed=(g_n1w, g_n1b), phase="params", stats=st1)
             else:
                 dx, d_n1w, d_n1b = dxn, None, None
@@ -308,24 +306,24 @@ class _Tail(torch.autograd.Function):
             # project_out
             dgg = ops.pixlin(dout3, WpoutT)
             (g_wpout, k_wpout), (g_bpout, k_bpout) = _acc(w_pout, Z["wpout"]), _acc(b_pout, Z["bpout"])
-            with _side(k_wpout and (b_pout is None or k_bpout), dev, dout3, gg, bit=4):
+            with _side(k_wpout and (b_pout is None or k_bpout), dev, dout3, gg):
                 d_wpout = ops.pixlin_wgrad(dout3, gg, out=g_wpout, dbias=g_bpout if b_pout is not None else None, deterministic=False).view_as(w_pout)
             # depthwise conv + GELU gate
             (g_fdw, k_fdw), (g_fdwb, k_fdwb) = _acc(fdw, Z["fdw"]), _acc(fdwb, Z["fdwb"])
             dv = ops.dwconv3x3_bwd(t, _f32(fdw.view(2 * h, 9)), _f32(fdwb), dgg, h, H, W, 1, phase="data")
-            with _side(k_fdw and (fdwb is None or k_fdwb), dev, t, dv, bit=64):
+            with _side(k_fdw and (fdwb is None or k_fdwb), dev, t, dv):
                 d_fdw, d_fdwb = ops.dwconv3x3_bwd(t, _f32(fdw.view(2 * h, 9)), _f32(fdwb), None, h, H, W, 1, zeroed=(g_fdw, g_fdwb),
                                                   phase="params", dv=dv)
             dt = ops.dwconv3x3(dv, fdwf, None, 2 * h, H, W, 2)
             # project_in + norm2 (+ the residual branch of the EFFN)
             dx1n = ops.pixlin(dt, WpinT)
             (g_wpin, k_wpin), (g_bpin, k_bpin) = _acc(w_pin, Z["wpin"]), _acc(b_pin, Z["bpin"])
-            with _side(k_wpin and (b_pin is None or k_bpin), dev, x1, dt, bit=8):
+            with _side(k_wpin and (b_pin is None or k_bpin), dev, x1, dt):
                 x1n = ops.layernorm_fwd(x1, ln_mode, _f32(n2w), _f32(n2b))
                 d_wpin = ops.pixlin_wgrad(dt, x1n, out=g_wpin, dbias=g_bpin if b_pin is not None else None, deterministic=False).view_as(w_pin)
             (g_n2w, k_n2w), (g_n2b, k_n2b) = _acc(n2w, Z["n2w"]), _acc(n2b, Z["n2b"])
             dx1, st2 = ops.layernorm_bwd(x1, dx1n, ln_mode, _f32(n2w), add=dout3, phase="data")
-            with _side(k_n2w and (n2b is None or k_n2b), dev, x1, dx1n, st2, bit=128):
+            with _side(k_n2w and (n2b is None or k_n2b), dev, x1, dx1n, st2):
                 d_n2w, d_n2b = ops.layernorm_bwd(x1, dx1n, ln_mode, _f32(n2w), zeroed=(g_n2w, g_n2b), phase="params", stats=st2)
             # out_conv with the channel gate in front, residual behind
             dy2, dc, d_wout, d_bout = _out_conv_bwd(dx1, y23, cg, w_out, b_out, WoutT, gate_mode, Z["wb"], Z["bout"])
@@ -346,7 +344,7 @@ def _out_conv_bwd(dx1, y23, cg, w_out, b_out, WoutT, gate_mode, wb_acc, bout_acc
     g_bout, k_bout = _acc(b_out, bout_acc)
     g_wout = getattr(w_out, "grad", None)
     k_wout = _DIRECT_GRADS and g_wout is not None and g_wout.dtype == torch.float32 and not torch.is_grad_enabled()
-    with _side(k_wout and (b_out is None or k_bout), dev, dx1, y23, cg, wb_acc, bit=16):
+    with _side(k_wout and (b_out is None or k_bout), dev, dx1, y23, cg, wb_acc):
         wb = ops.pixlin_wgrad(dx1, y23, per_batch=True, out=wb_acc, dbias=g_bout, deterministic=False)  # (B, C_out, C_in): scaled per image by the gate
         if gate_mode == 1:
             d_wout = (wb * (1.0 + cg)[:, None, :]).sum(0)

@@ -7,7 +7,6 @@ autocast, fp32 parameters), captured in ONE CUDA graph; then the single collecti
 gradients over NCCL -- and one fused Adam + EMA kernel over the flat parameter buffers (vmambair_b200.optim.FlatAdam)."""
 from __future__ import annotations
 
-import os
 import time
 
 import torch
@@ -50,39 +49,38 @@ def run_train(args, build_net, ClockSampler, env_rank, dist_max, barrier, peaks,
     # forward + loss + backward of the static-shape step captured in ONE CUDA graph; the all-reduce and the optimizer kernel follow it
     graph, static_loss = None, None
     lq_s, gt_s = lq.clone(), gt.clone()
-    if os.environ.get("VMB_TRAIN_GRAPH", "1") == "1":
-        try:
-            side = torch.cuda.Stream(dev)
-            side.wait_stream(torch.cuda.current_stream(dev))
-            with torch.cuda.stream(side):
-                for _ in range(3):
-                    opt.flat_grad.zero_()
-                    fwd_bwd(lq_s, gt_s)
-            torch.cuda.current_stream(dev).wait_stream(side)
-            torch.cuda.synchronize(dev)
-            opt.check_views()
-            opt.flat_grad.zero_()
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                static_loss = fwd_bwd(lq_s, gt_s)
-            # the replayed step must reproduce the eager one (loss and gradients) before it is trusted
-            opt.flat_grad.zero_()
-            graph.replay()
-            torch.cuda.synchronize(dev)
-            l_g, g_g = float(static_loss), opt.flat_grad.clone()
-            opt.flat_grad.zero_()
-            l_e = float(fwd_bwd(lq_s, gt_s))
-            torch.cuda.synchronize(dev)
-            rel = float((opt.flat_grad - g_g).norm() / opt.flat_grad.norm().clamp_min(1e-12))
-            opt.flat_grad.zero_()
-            if abs(l_g - l_e) > 1e-3 * abs(l_e) + 1e-6 or rel > 2e-2:
-                raise RuntimeError(f"graph replay differs from eager: loss {l_g} vs {l_e}, grad rel diff {rel}")
-        except Exception as e:  # report and fall back to the eager step (never silently)
-            print(f"[train_bench] CUDA-graph capture of fwd+bwd failed, running eagerly: {type(e).__name__}: {e}", flush=True)
-            graph = None
-            torch.cuda.synchronize(dev)
-            opt.check_views()
-            opt.flat_grad.zero_()
+    try:
+        side = torch.cuda.Stream(dev)
+        side.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(side):
+            for _ in range(3):
+                opt.flat_grad.zero_()
+                fwd_bwd(lq_s, gt_s)
+        torch.cuda.current_stream(dev).wait_stream(side)
+        torch.cuda.synchronize(dev)
+        opt.check_views()
+        opt.flat_grad.zero_()
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            static_loss = fwd_bwd(lq_s, gt_s)
+        # the replayed step must reproduce the eager one (loss and gradients) before it is trusted
+        opt.flat_grad.zero_()
+        graph.replay()
+        torch.cuda.synchronize(dev)
+        l_g, g_g = float(static_loss), opt.flat_grad.clone()
+        opt.flat_grad.zero_()
+        l_e = float(fwd_bwd(lq_s, gt_s))
+        torch.cuda.synchronize(dev)
+        rel = float((opt.flat_grad - g_g).norm() / opt.flat_grad.norm().clamp_min(1e-12))
+        opt.flat_grad.zero_()
+        if abs(l_g - l_e) > 1e-3 * abs(l_e) + 1e-6 or rel > 2e-2:
+            raise RuntimeError(f"graph replay differs from eager: loss {l_g} vs {l_e}, grad rel diff {rel}")
+    except Exception as e:  # report and fall back to the eager step (never silently)
+        print(f"[train_bench] CUDA-graph capture of fwd+bwd failed, running eagerly: {type(e).__name__}: {e}", flush=True)
+        graph = None
+        torch.cuda.synchronize(dev)
+        opt.check_views()
+        opt.flat_grad.zero_()
 
     def step(lq_t, gt_t):
         if graph is not None:

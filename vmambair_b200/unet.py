@@ -15,19 +15,18 @@ separate pass over HBM (and, on cuDNN, an NCHW<->NHWC transform either side of e
 The two middle convs of the SR tail (96 -> 384 at 64x64 and 128x128: 22 + 87 GFLOP per 8-image batch, compute-bound) stay on the
 library convolution (cuDNN's sm_90 kernels, NHWC) with this library's NHWC PixelShuffle between them.
 
-Inference only: with gradients enabled the modules' nn.Conv2d / torch.cat path (autograd) is used.  VMB_UNET=torch restores that
+Inference only: with gradients enabled the modules' nn.Conv2d / torch.cat path (autograd) is used.  set_mode("torch") restores that
 path for inference as well (cross-checks, tests).
 """
 from __future__ import annotations
 
-import os
 
 import torch
 import torch.nn as nn
 
 from . import fused, ops
 
-_MODE = os.environ.get("VMB_UNET", "native")
+_MODE = "native"
 
 
 def set_mode(mode: str) -> None:
