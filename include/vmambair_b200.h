@@ -618,6 +618,57 @@ typedef struct {
 int vmb_ssim(const vmb_ssim_args* a, void* stream);
 int64_t vmb_ssim_workspace_bytes(const vmb_ssim_args* a);
 
+/* ---- NIQE: calculate_niqe of Deraining/basicsr/metrics/niqe.py (niqe, compute_feature, estimate_aggd_param) --------------------
+ * Three launches per call: vmb_niqe_prep, vmb_niqe_features, vmb_niqe_score; vmb_niqe_table once per device.  Blocks are 96 x 96 at
+ * scale 1 and 48 x 48 on the half plane; an image's H and W are cut to whole blocks before anything is filtered.  No atomics: every
+ * sum has a fixed order, so results are bitwise reproducible and do not depend on the batch. */
+#define VMB_NIQE_BLOCK 96
+#define VMB_NIQE_TABLE 9801   /* gam = np.arange(0.2, 10.001, 0.001) */
+#define VMB_NIQE_FEATURES 36  /* 18 per scale */
+#define VMB_NIQE_Y 0          /* to_y_channel (1 or 3 channels), bit for bit as vmb_to_y_channel */
+#define VMB_NIQE_GRAY 1       /* cv2.cvtColor(img / 255., COLOR_BGR2GRAY) * 255. in float32: (B .114f + G .587f) + R .299f, unfused */
+#define VMB_NIQE_PLANE 2      /* the value as float32 (input_order='HW'); 1 channel */
+
+/* table[i] = gamma(2 / g)^2 / (gamma(1 / g) gamma(3 / g)), g = 0.2 + i ((0.2 + 0.001) - 0.2), in fp64 (device tgamma). */
+int vmb_niqe_table(double* table, void* stream);
+
+/* The float32 plane of `src` (batch images, H x W, already cropped to whole blocks: H, W multiples of 96) after the float32 cast and
+ * `convert` -> plane (batch, H, W), and half (batch, H / 2, W / 2) = fl32(((q00 + q01) + (q10 + q11)) * .25f) * 255.f with
+ * q = fl32(v / 255.f) over each 2 x 2 quad, standing in for cv2.resize(img / 255., (w // 2, h // 2), INTER_LINEAR) * 255. */
+typedef struct {
+    vmb_metric_src src;
+    int batch, H, W, channels, convert;
+    float *plane, *half;
+} vmb_niqe_prep_args;
+int vmb_niqe_prep(const vmb_niqe_prep_args* a, void* stream);
+
+/* One CTA per block and scale.  MSCN: mu = window * img, sigma = sqrt(|window * fl32(img^2) - mu^2|), n = (img - mu) / (sigma + 1),
+ * each convolution (edges 'nearest' on the cut plane) summed in fp64 and rounded once to float32, the rest float32.  Per block, five
+ * distributions (n, and n times n rolled circularly within the block by [0,1], [1,0], [1,1], [1,-1], float32 products) fitted as
+ * estimate_aggd_param does, from fp64 sums; alpha by search of `table` (vmb_niqe_table, on the device).  features (batch, blocks, 36)
+ * fp64: row w nbh + h for block (h, w), scale 1's 18 features then scale 2's.  mscn, mscn_half (NULL: not written): the normalised
+ * planes, (batch, H, W) and (batch, H / 2, W / 2).  window: the 7 x 7 Gaussian of the pristine parameters, row-major. */
+typedef struct {
+    const float *plane, *half;
+    const double* table;
+    double* features;
+    float *mscn, *mscn_half;
+    double window[49];
+    int batch, H, W;
+} vmb_niqe_features_args;
+int vmb_niqe_features(const vmb_niqe_features_args* a, void* stream);
+
+/* One CTA per image: score[b] = sqrt(d ((cov_pris + cov_d) / 2)^-1 d^T), d = mu_pris - nanmean(features[b], axis 0), cov_d the
+ * ddof-1 covariance of the rows without a NaN, all fp64, sums in row order; NaN with fewer than two such rows (blocks 0 included).
+ * mu_pris (36) and cov_pris (36 x 36, row-major): fp64 on the device. */
+typedef struct {
+    const double* features;
+    const double *mu_pris, *cov_pris;
+    double* score;
+    int batch, blocks;
+} vmb_niqe_score_args;
+int vmb_niqe_score(const vmb_niqe_score_args* a, void* stream);
+
 /* ---- degradations: the Real-ESRGAN synthesis operators of basicsr that RealSR/VmambaIR/models/MambaRealSR_model.py:145-260 uses --
  * Every image is float32 NCHW, contiguous: `batch` images of `channels` planes of H x W.  Nothing reads the host. */
 

@@ -288,6 +288,27 @@ class SsimArgs(C.Structure):
                 ("ssim", vp), ("workspace", vp)]
 
 
+NIQE_BLOCK, NIQE_TABLE, NIQE_FEATURES = 96, 9801, 36  # VMB_NIQE_BLOCK / _TABLE / _FEATURES
+NIQE_Y, NIQE_GRAY, NIQE_PLANE = 0, 1, 2  # VMB_NIQE_Y / _GRAY / _PLANE
+
+
+class NiqePrepArgs(C.Structure):
+    _c_name_ = "vmb_niqe_prep_args"
+    _fields_ = [("src", MetricSrc), ("batch", C.c_int), ("H", C.c_int), ("W", C.c_int), ("channels", C.c_int), ("convert", C.c_int),
+                ("plane", vp), ("half", vp)]
+
+
+class NiqeFeaturesArgs(C.Structure):
+    _c_name_ = "vmb_niqe_features_args"
+    _fields_ = [("plane", vp), ("half", vp), ("table", vp), ("features", vp), ("mscn", vp), ("mscn_half", vp),
+                ("window", C.c_double * 49), ("batch", C.c_int), ("H", C.c_int), ("W", C.c_int)]
+
+
+class NiqeScoreArgs(C.Structure):
+    _c_name_ = "vmb_niqe_score_args"
+    _fields_ = [("features", vp), ("mu_pris", vp), ("cov_pris", vp), ("score", vp), ("batch", C.c_int), ("blocks", C.c_int)]
+
+
 class Filter2dArgs(C.Structure):
     _c_name_ = "vmb_filter2d_args"
     _fields_ = [("img", vp), ("out", vp), ("kernel", vp), ("batch", C.c_int), ("channels", C.c_int), ("H", C.c_int), ("W", C.c_int),
@@ -498,6 +519,10 @@ SYMBOLS = {
     "vmb_psnr_workspace_bytes": (C.c_int64, [C.POINTER(PsnrArgs)]),
     "vmb_ssim": (C.c_int, [C.POINTER(SsimArgs), vp]),
     "vmb_ssim_workspace_bytes": (C.c_int64, [C.POINTER(SsimArgs)]),
+    "vmb_niqe_table": (C.c_int, [vp, vp]),
+    "vmb_niqe_prep": (C.c_int, [C.POINTER(NiqePrepArgs), vp]),
+    "vmb_niqe_features": (C.c_int, [C.POINTER(NiqeFeaturesArgs), vp]),
+    "vmb_niqe_score": (C.c_int, [C.POINTER(NiqeScoreArgs), vp]),
     "vmb_filter2d": (C.c_int, [C.POINTER(Filter2dArgs), vp]),
     "vmb_usm_sharp": (C.c_int, [C.POINTER(UsmSharpArgs), vp]),
     "vmb_jpeg": (C.c_int, [C.POINTER(JpegArgs), vp]),

@@ -1,11 +1,10 @@
 // PSNR and SSIM of the reference's metric code (Deraining/basicsr/metrics/psnr_ssim.py, Deraining/Deraining/utils.py) on the device.
-// Sources are decoded in the loads (dtype, tensor2img quantisation, channel order, the Y channel); nothing intermediate is written.
-// The Y chain spells out every rounding (__fdiv_rn, __dmul_rn, __dadd_rn, ...) so nvcc cannot contract it: it equals the reference's
-// numpy arithmetic bit for bit.  Every sum is deterministic: per-CTA partials in a fixed order, then one CTA per image adds them in
+// Sources are decoded in the loads (dtype, tensor2img quantisation, channel order, the Y channel: metric_src.cuh); nothing
+// intermediate is written.  Every sum is deterministic: per-CTA partials in a fixed order, then one CTA per image adds them in
 // index order (no floating-point atomics), so a result depends on the image size only, never on scheduling.
 #include <math.h>
 
-#include "common.cuh"
+#include "metric_src.cuh"
 
 namespace vmb {
 
@@ -16,32 +15,6 @@ constexpr int kPsnrItems = 8;               // pixels per thread a PSNR CTA aims
 constexpr int kPsnrMaxBlocks = 1024;        // per image
 constexpr int kTW = 32, kTH = 16, kR = 5;   // SSIM output tile (x, y) and the window's radius
 constexpr int kInW = kTW + 2 * kR, kInH = kTH + 2 * kR;
-
-// the reference's float64 value of element (b, y, x, c)
-__device__ __forceinline__ double load_val(const vmb_metric_src& s, int b, int y, int x, int c) {
-    const int64_t i = b * s.batch_stride + y * s.row_stride + x * s.pixel_stride + c * s.channel_stride;
-    if (s.dtype == VMB_MSRC_U8) return (double)reinterpret_cast<const uint8_t*>(s.img)[i];
-    if (s.dtype == VMB_MSRC_U16) return (double)reinterpret_cast<const uint16_t*>(s.img)[i];
-    if (s.dtype == VMB_MSRC_F32) return (double)reinterpret_cast<const float*>(s.img)[i];
-    if (s.dtype == VMB_MSRC_F64) return reinterpret_cast<const double*>(s.img)[i];
-    const float q = s.dtype == VMB_MSRC_Q_F32    ? reinterpret_cast<const float*>(s.img)[i]
-                    : s.dtype == VMB_MSRC_Q_BF16 ? to_f32(reinterpret_cast<const __nv_bfloat16*>(s.img)[i])
-                                                 : to_f32(reinterpret_cast<const __half*>(s.img)[i]);
-    // tensor2img: clamp_(0, 1), (x * 255.0).round() in float32 (half to even), uint8; fminf / fmaxf map a NaN to 0 as the cast does
-    return (double)rintf(__fmul_rn(fminf(fmaxf(q, 0.f), 1.f), 255.f));
-}
-
-// to_y_channel of one BGR pixel: img.astype(float32) / 255., np.dot(img, [24.966, 128.553, 65.481]) + 16.0 in float64 (left to
-// right), / 255. and .astype(float32) (_convert_output_type_range), then * 255. in float32
-__device__ __forceinline__ float y_bgr(double b, double g, double r) {
-    const double xb = __fdiv_rn(__double2float_rn(b), 255.f), xg = __fdiv_rn(__double2float_rn(g), 255.f),
-                 xr = __fdiv_rn(__double2float_rn(r), 255.f);
-    const double d = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(xb, 24.966), __dmul_rn(xg, 128.553)), __dmul_rn(xr, 65.481)), 16.0);
-    return __fmul_rn(__double2float_rn(__ddiv_rn(d, 255.0)), 255.f);
-}
-
-// to_y_channel of a one-channel image: the float32 round trip / 255. * 255.
-__device__ __forceinline__ float y_gray(double v) { return __fmul_rn(__fdiv_rn(__double2float_rn(v), 255.f), 255.f); }
 
 // the value a metric sees at plane c of pixel (b, y, x): the source value, or (plane 0) its Y
 __device__ __forceinline__ double metric_val(const vmb_metric_src& s, int channels, int y_channel, int b, int y, int x, int c) {
@@ -264,11 +237,9 @@ int64_t ssim_tiles(const vmb_ssim_args& a) {
 
 using namespace vmb;
 
-static bool src_ok(const vmb_metric_src& s) { return s.img != nullptr && s.dtype >= VMB_MSRC_U8 && s.dtype <= VMB_MSRC_Q_F16; }
-
 static int check_pair(const vmb_metric_src& s1, const vmb_metric_src& s2, int batch, int H, int W, int channels, int y_channel,
                       const char* who) {
-    VMB_CHECK(src_ok(s1) && src_ok(s2), "%s: null image or unknown source dtype (%d, %d)", who, s1.dtype, s2.dtype);
+    VMB_CHECK(metric_src_ok(s1) && metric_src_ok(s2), "%s: null image or unknown source dtype (%d, %d)", who, s1.dtype, s2.dtype);
     VMB_CHECK(batch > 0 && batch < 65536 && H > 0 && W > 0 && (channels == 1 || channels == 3) && (y_channel == 0 || y_channel == 1),
               "%s: bad batch %d, size %d x %d, channels %d (1 or 3) or y_channel %d", who, batch, H, W, channels, y_channel);
     return VMB_OK;

@@ -64,17 +64,17 @@ class _View:
         return ops.metric_src(self.t, self.offset, self.strides, self.quantize)
 
 
-def _view(t, quantize):
+def _view(t, quantize, who="psnr_ssim"):
     if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dim() == 4):
-        raise ValueError("psnr_ssim: images must be 4-D CUDA tensors")
+        raise ValueError(f"{who}: images must be 4-D CUDA tensors")
     if quantize and t.is_floating_point():
         if t.shape[1] != 3 or t.dtype not in ops.MSRC_Q:
-            raise ValueError(f"psnr_ssim: quantize=True takes (B, 3, H, W) float32 / bf16 / fp16 RGB, got {tuple(t.shape)} {t.dtype}")
+            raise ValueError(f"{who}: quantize=True takes (B, 3, H, W) float32 / bf16 / fp16 RGB, got {tuple(t.shape)} {t.dtype}")
         B, _, H, W = t.shape
         sb, sc, sh, sw = t.stride()
         return _View(t, 2 * sc, (B, H, W, 3), (sb, sh, sw, -sc), True)  # channel 0 (B) is plane 2
     if t.shape[3] not in (1, 3) or t.dtype not in ops.MSRC:
-        raise ValueError(f"psnr_ssim: images must be (B, H, W, 1 or 3) uint8 / uint16 / float32 / float64, got {tuple(t.shape)} {t.dtype}")
+        raise ValueError(f"{who}: images must be (B, H, W, 1 or 3) uint8 / uint16 / float32 / float64, got {tuple(t.shape)} {t.dtype}")
     return _View(t, 0, tuple(t.shape), t.stride(), False)
 
 

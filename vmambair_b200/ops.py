@@ -955,6 +955,52 @@ def ssim_mean(t, src1, src2, batch, H, W, channels, y_channel, mode, taps, mix=N
     return out
 
 
+# ---- NIQE (csrc/niqe.cu): calculate_niqe of the reference's niqe.py; nothing read on the host ----
+NIQE_CONVERT = {"y": _lib.NIQE_Y, "gray": _lib.NIQE_GRAY, None: _lib.NIQE_PLANE}
+
+
+def niqe_table(device):
+    """-> (9801,) float64 on `device`: r(gamma) of estimate_aggd_param over gam = np.arange(0.2, 10.001, 0.001)"""
+    out = torch.empty(_lib.NIQE_TABLE, dtype=torch.float64, device=device)
+    _run("vmb_niqe_table", out, "niqe_table", _ptr(out), nbytes=out.numel() * 8)
+    return out
+
+
+def niqe_prep(t, src, batch, H, W, channels, convert):
+    """-> (plane (batch, H, W), half (batch, H / 2, W / 2)), float32: `src` (a metric_src view of CUDA tensor t, already cut to whole
+    96 x 96 blocks) as the plane NIQE filters, under `convert` (a key of NIQE_CONVERT), and its 2 x 2 mean"""
+    plane = torch.empty((batch, H, W), dtype=torch.float32, device=t.device)
+    half = torch.empty((batch, H // 2, W // 2), dtype=torch.float32, device=t.device)
+    a = _lib.NiqePrepArgs(src=src, batch=batch, H=H, W=W, channels=channels, convert=NIQE_CONVERT[convert], plane=_ptr(plane),
+                          half=_ptr(half))
+    _run("vmb_niqe_prep", t, "niqe_prep", a, nbytes=batch * H * W * (channels * t.element_size() + 5))
+    return plane, half
+
+
+def niqe_features(plane, half, table, window, mscn=False):
+    """-> (batch, blocks, 36) float64 features (the reference's distparam) of the prep planes; window: 49 floats (the 7 x 7 Gaussian,
+    row-major).  mscn=True: also the normalised planes, (features, mscn (batch, H, W), mscn_half (batch, H / 2, W / 2))."""
+    batch, H, W = plane.shape
+    nb = (H // _lib.NIQE_BLOCK) * (W // _lib.NIQE_BLOCK)
+    feats = torch.empty((batch, nb, _lib.NIQE_FEATURES), dtype=torch.float64, device=plane.device)
+    m1 = torch.empty_like(plane) if mscn else None
+    m2 = torch.empty_like(half) if mscn else None
+    a = _lib.NiqeFeaturesArgs(plane=_ptr(plane), half=_ptr(half), table=_ptr(table), features=_ptr(feats), mscn=_ptr(m1),
+                              mscn_half=_ptr(m2), window=(C.c_double * 49)(*window), batch=batch, H=H, W=W)
+    _run("vmb_niqe_features", plane, "niqe_features", a, nbytes=(plane.numel() + half.numel()) * 4 + feats.numel() * 8)
+    return (feats, m1, m2) if mscn else feats
+
+
+def niqe_score(feats, mu_pris, cov_pris):
+    """-> (batch,) float64 NIQE scores of (batch, blocks, 36) features against the pristine model (36,) / (36, 36) float64"""
+    batch, nb, _ = feats.shape
+    out = torch.empty(batch, dtype=torch.float64, device=feats.device)
+    a = _lib.NiqeScoreArgs(features=_ptr(feats) if nb else None, mu_pris=_ptr(mu_pris), cov_pris=_ptr(cov_pris), score=_ptr(out),
+                           batch=batch, blocks=nb)
+    _run("vmb_niqe_score", feats, "niqe_score", a, nbytes=feats.numel() * 8)
+    return out
+
+
 # ---- degradations (csrc/degrade.cu): basicsr's Real-ESRGAN synthesis operators; float32 NCHW, contiguous, nothing read on the host ----
 NOISE_GAUSSIAN, NOISE_POISSON = 0, 1  # VMB_NOISE_*
 
