@@ -471,7 +471,9 @@ int vmb_sum4_add(const void* x4, const void* add, void* out, int batch, long per
  * Deraining/basicsr/models/base_model.py:54-62).  grad is first multiplied by grad_scale (1/world after the all-reduce) and, when
  * max_grad_norm > 0, by min(1, max_grad_norm / (||grad|| + 1e-6)).  state: 4 floats on the device, zero-initialised by the
  * caller; state[0] is the step count, advanced by this call (so CUDA-graph replays keep the bias correction right).
- * ema (NULL: none): ema = ema_decay * ema + (1 - ema_decay) * param.  zero_grad != 0 clears the gradient buffer. */
+ * ema (NULL: none): ema = ema_decay * ema + (1 - ema_decay) * param.  zero_grad != 0 clears the gradient buffer.
+ * lr_dev (NULL: use lr): the learning rate read from the device (one fp32), e.g. written by vmb_lr_schedule earlier in the stream,
+ * so that a captured CUDA graph follows the schedule. */
 typedef struct {
     float* param; float* grad; float* exp_avg; float* exp_avg_sq; float* ema; float* state;
     long n;
@@ -479,6 +481,7 @@ typedef struct {
     int decoupled_weight_decay;   /* 0: Adam (L2 added to the gradient), 1: AdamW */
     float grad_scale, max_grad_norm, ema_decay;
     int zero_grad;
+    const float* lr_dev;
 } vmb_adam_args;
 int vmb_fused_adam(const vmb_adam_args* a, void* stream);
 
@@ -851,6 +854,61 @@ typedef struct {
     int dtype;
 } vmb_bce_logits_bwd_args;
 int vmb_bce_logits_bwd(const vmb_bce_logits_bwd_args* a, void* stream);
+
+/* ---- GAN training step (vmambair_b200.gan_train): the pieces of MambaRealSRGAN.optimize_parameters
+ * (RealSR/VmambaIR/models/MambaRealSRGAN_model.py:289-364) that autograd and the host would otherwise do.  fp32 math, fp32 or bf16
+ * tensors, contiguous; no atomics and no host reads. */
+
+/* *out = weight mean(|x - y|) over n elements (the recipes' L1Loss, reduction 'mean'), or weight mean(x) when y is NULL (the loss
+ * dict's out_d_real / out_d_fake).  x and y share `dtype`.  Per-CTA partials, then one CTA adds them in order.
+ * workspace: vmb_mean_loss_workspace_bytes(n) bytes. */
+typedef struct {
+    const void *x, *y;
+    float* out;
+    void* workspace;
+    int64_t n;
+    float weight;
+    int dtype;
+} vmb_mean_loss_args;
+int vmb_mean_loss(const vmb_mean_loss_args* a, void* stream);
+int64_t vmb_mean_loss_workspace_bytes(int64_t n);
+
+/* The generator's output gradient, the junction of its three losses:
+ * dout = w_pix sign(out - gt) / n + g_percep + g_gan over n elements (sign(0) = 0, as torch's l1_loss backward).  out and gt are
+ * `in_dtype`, g_percep and g_gan fp32 (NULL: that term is absent), dout `out_dtype`. */
+typedef struct {
+    const void *out, *gt;
+    const float *g_percep, *g_gan;
+    void* dout;
+    int64_t n;
+    float w_pix;
+    int in_dtype, out_dtype;
+} vmb_gan_out_grad_args;
+int vmb_gan_out_grad(const vmb_gan_out_grad_args* a, void* stream);
+
+/* Learning-rate schedule of one optimizer at iteration `it`:
+ * lr = base step_gamma^(it / step_size) milestone_gamma^(number of milestones <= it - 1).
+ * The first factor is MambaRealSRGAN's generator decay (lr_sr, gamma_sr, lr_decay_sr; step_size <= 0: none), the second basicsr's
+ * MultiStepLR, which has stepped it - 1 times when iteration `it` runs.  All in double (Python's float), the result rounded to fp32. */
+#define VMB_LR_MAX_MILESTONES 8
+typedef struct {
+    double base, step_gamma, milestone_gamma;
+    int64_t step_size;
+    int64_t milestones[VMB_LR_MAX_MILESTONES];
+    int n_milestones;
+} vmb_lr_rule;
+/* One thread: *iter += 1, then lr[k] = rule[k] at the new *iter for k < n_rules (at most 2: generator, discriminator). */
+typedef struct {
+    int64_t* iter;
+    float* lr;
+    vmb_lr_rule rule[2];
+    int n_rules;
+} vmb_lr_schedule_args;
+int vmb_lr_schedule(const vmb_lr_schedule_args* a, void* stream);
+
+/* ema = decay ema + (1 - decay) param over n fp32 elements: vmb_fused_adam's EMA alone, for iterations that skip the optimizer
+ * step but not basicsr's model_ema(). */
+int vmb_ema_update(float* ema, const float* param, int64_t n, float decay, void* stream);
 
 /* ---- Perceptual loss: basicsr's PerceptualLoss (losses/basic_loss.py) on VGGFeatureExtractor (archs/vgg_arch.py), the generator
  * step's perceptual_opt of both GAN recipes, between its convolutions.  It replaces the extractor's ReLU and MaxPool2d modules, the

@@ -234,7 +234,8 @@ class AdamArgs(C.Structure):
     _fields_ = [("param", vp), ("grad", vp), ("exp_avg", vp), ("exp_avg_sq", vp), ("ema", vp), ("state", vp),
                 ("n", C.c_long), ("lr", C.c_float), ("beta1", C.c_float), ("beta2", C.c_float), ("eps", C.c_float),
                 ("weight_decay", C.c_float), ("decoupled_weight_decay", C.c_int),
-                ("grad_scale", C.c_float), ("max_grad_norm", C.c_float), ("ema_decay", C.c_float), ("zero_grad", C.c_int)]
+                ("grad_scale", C.c_float), ("max_grad_norm", C.c_float), ("ema_decay", C.c_float), ("zero_grad", C.c_int),
+                ("lr_dev", vp)]
 
 
 class ImageMaxArgs(C.Structure):
@@ -392,6 +393,31 @@ class BceLogitsBwdArgs(C.Structure):
                 ("dtype", C.c_int)]
 
 
+class MeanLossArgs(C.Structure):
+    _c_name_ = "vmb_mean_loss_args"
+    _fields_ = [("x", vp), ("y", vp), ("out", vp), ("workspace", vp), ("n", i64), ("weight", C.c_float), ("dtype", C.c_int)]
+
+
+class GanOutGradArgs(C.Structure):
+    _c_name_ = "vmb_gan_out_grad_args"
+    _fields_ = [("out", vp), ("gt", vp), ("g_percep", vp), ("g_gan", vp), ("dout", vp), ("n", i64), ("w_pix", C.c_float),
+                ("in_dtype", C.c_int), ("out_dtype", C.c_int)]
+
+
+LR_MAX_MILESTONES = 8  # VMB_LR_MAX_MILESTONES
+
+
+class LrRule(C.Structure):
+    _c_name_ = "vmb_lr_rule"
+    _fields_ = [("base", C.c_double), ("step_gamma", C.c_double), ("milestone_gamma", C.c_double), ("step_size", i64),
+                ("milestones", i64 * LR_MAX_MILESTONES), ("n_milestones", C.c_int)]
+
+
+class LrScheduleArgs(C.Structure):
+    _c_name_ = "vmb_lr_schedule_args"
+    _fields_ = [("iter", vp), ("lr", vp), ("rule", LrRule * 2), ("n_rules", C.c_int)]
+
+
 PERCEP_L1, PERCEP_L2, PERCEP_FRO = 0, 1, 2  # VMB_PERCEP_L1 / _L2 / _FRO
 PERCEP_MAX_FEATS = 37  # VMB_PERCEP_MAX_FEATS
 
@@ -539,6 +565,11 @@ SYMBOLS = {
     "vmb_bce_logits": (C.c_int, [C.POINTER(BceLogitsArgs), vp]),
     "vmb_bce_logits_workspace_bytes": (C.c_int64, [C.c_int64]),
     "vmb_bce_logits_bwd": (C.c_int, [C.POINTER(BceLogitsBwdArgs), vp]),
+    "vmb_mean_loss": (C.c_int, [C.POINTER(MeanLossArgs), vp]),
+    "vmb_mean_loss_workspace_bytes": (C.c_int64, [C.c_int64]),
+    "vmb_gan_out_grad": (C.c_int, [C.POINTER(GanOutGradArgs), vp]),
+    "vmb_lr_schedule": (C.c_int, [C.POINTER(LrScheduleArgs), vp]),
+    "vmb_ema_update": (C.c_int, [vp, vp, C.c_int64, C.c_float, vp]),
     "vmb_percep_norm": (C.c_int, [C.POINTER(PercepNormArgs), vp]),
     "vmb_percep_norm_bwd": (C.c_int, [C.POINTER(PercepNormBwdArgs), vp]),
     "vmb_percep_stage": (C.c_int, [C.POINTER(PercepStageArgs), vp]),

@@ -569,6 +569,7 @@ __global__ void __launch_bounds__(256) gate_bwd_kernel(const GateBwdParams p) {
 // clip_grad_norm_, SRGAN/VmambaIR/models/MambaSISR_model.py:141-147, Deraining/basicsr/models/image_restoration_model.py:165-173,
 // Deraining/basicsr/models/base_model.py:54-62) instead of ~1 500 per-tensor launches.  `state` (device, 4 floats):
 // [0] step count (incremented by the trailing 1-thread kernel: graph replays advance it), [1] sum of squared gradients.
+// lr_dev, when set, is read on the device (a schedule kernel earlier in the stream writes it), so graph replays follow the schedule.
 __global__ void __launch_bounds__(256) sqsum_kernel(const float* __restrict__ g, long n, float* __restrict__ state) {
     __shared__ float sred[8];
     float acc = 0.f;
@@ -585,12 +586,13 @@ __global__ void __launch_bounds__(256) fused_adam_kernel(const AdamParams p) {
         const float total = sqrtf(p.state[1]) * p.grad_scale;
         gs *= fminf(p.max_norm / (total + 1e-6f), 1.f);
     }
-    const float step_size = p.lr / bc1, inv_sqrt_bc2 = rsqrtf(bc2);
+    const float lr = p.lr_dev ? *p.lr_dev : p.lr;
+    const float step_size = lr / bc1, inv_sqrt_bc2 = rsqrtf(bc2);
     for (long i = (long)blockIdx.x * 256 + threadIdx.x; i < p.n; i += (long)gridDim.x * 256) {
         float w = p.param[i];
         float g = p.grad[i] * gs;
         if (p.weight_decay != 0.f) {
-            if (p.decoupled) w -= p.lr * p.weight_decay * w;  // AdamW
+            if (p.decoupled) w -= lr * p.weight_decay * w;  // AdamW
             else g = fmaf(p.weight_decay, w, g);                // Adam (L2)
         }
         const float m = fmaf(p.beta1, p.m[i], (1.f - p.beta1) * g);
@@ -838,7 +840,8 @@ extern "C" int vmb_fused_adam(const vmb_adam_args* a, void* stream) {
     VMB_CHECK(a->n > 0 && a->lr >= 0.f && a->beta1 >= 0.f && a->beta1 < 1.f && a->beta2 >= 0.f && a->beta2 < 1.f && a->eps > 0.f,
               "fused_adam: bad hyper-parameters");
     AdamParams p{a->param, a->grad, a->exp_avg, a->exp_avg_sq, a->ema, a->state, a->n, a->lr, a->beta1, a->beta2, a->eps,
-                 a->weight_decay, a->decoupled_weight_decay, a->grad_scale, a->max_grad_norm, a->ema_decay, a->zero_grad};
+                 a->weight_decay, a->decoupled_weight_decay, a->grad_scale, a->max_grad_norm, a->ema_decay, a->zero_grad,
+                 a->lr_dev};
     return fused_adam_launch(p, static_cast<cudaStream_t>(stream));
 }
 

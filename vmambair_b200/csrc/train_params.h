@@ -40,6 +40,7 @@ struct AdamParams {
     int decoupled;
     float grad_scale, max_norm, ema_decay;
     int zero_grad;
+    const float* lr_dev;  // nullptr: lr
 };
 struct PrepJob {
     const float* src; const float* src2; void* dst; void* dst2;

@@ -66,8 +66,11 @@ class _Side:
 
 
 def join_side_stream():
-    """make the current stream wait for the weight-gradient stream (idempotent; optim.FlatAdam.step calls it before it reads .grad)"""
-    _side_join()
+    """make the current stream wait for the weight-gradient stream (idempotent; optim.FlatAdam.step calls it before it reads .grad).
+    Nothing to do once the end-of-backward callback has joined it: waiting then would also tie a CUDA-graph capture to a stream the
+    capture never forked (a graph whose backward did not use the side stream, after an earlier eager backward that did)."""
+    if _Side.armed:
+        _side_join()
 
 
 def _side_join():

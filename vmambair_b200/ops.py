@@ -1170,6 +1170,64 @@ def bce_logits_bwd(x, grad_loss, target, weight):
     return gx
 
 
+# ---- GAN training step (csrc/gan_step.cu): pixel loss, logit means, the generator's output-gradient junction, the learning-rate
+# schedule and the EMA alone; fixed-order sums, nothing read on the host ----
+def mean_loss(x, y=None, weight=1.0, out=None):
+    """weight * mean(|x - y|) (the recipes' L1Loss), or weight * mean(x) when y is None -> 0-dim float32 tensor (`out` if given).
+    x, y: contiguous tensors of one dtype (float32 or bfloat16) and element count (the kernel indexes them linearly)"""
+    if y is not None and (y.dtype != x.dtype or y.numel() != x.numel()):
+        raise ValueError(f"mean_loss: x {x.dtype} {tuple(x.shape)} and y {y.dtype} {tuple(y.shape)} differ")
+    if not x.is_contiguous() or (y is not None and (not y.is_contiguous() or y.device != x.device)):
+        raise ValueError("mean_loss: x and y must be contiguous tensors on one device")
+    n = x.numel()
+    out = torch.empty((), dtype=torch.float32, device=x.device) if out is None else out
+    work = torch.empty(_lib.lib().vmb_mean_loss_workspace_bytes(n) // 4, dtype=torch.float32, device=x.device)
+    a = _lib.MeanLossArgs(x=_ptr(x), y=_ptr(y), out=_ptr(out), workspace=_ptr(work), n=n, weight=float(weight), dtype=_gan_dt(x))
+    _run("vmb_mean_loss", x, "mean_loss", a, nbytes=n * x.element_size() * (1 if y is None else 2), kernels=2)
+    return out
+
+
+def gan_out_grad(out, gt, g_percep, g_gan, w_pix, dtype):
+    """the generator's output gradient w_pix * sign(out - gt) / n + g_percep + g_gan, in `dtype`.  out, gt: contiguous, one dtype
+    (float32 or bfloat16); g_percep, g_gan: contiguous float32 or None (term absent).  The kernel indexes all of them linearly."""
+    if gt.dtype != out.dtype or gt.numel() != out.numel():
+        raise ValueError(f"gan_out_grad: out {out.dtype} {tuple(out.shape)} and gt {gt.dtype} {tuple(gt.shape)} differ")
+    for g in (g_percep, g_gan):
+        if g is not None and (g.dtype != torch.float32 or g.numel() != out.numel()):
+            raise ValueError(f"gan_out_grad: a loss gradient is {g.dtype} {tuple(g.shape)}, not float32 {tuple(out.shape)}")
+    if not all(t.is_contiguous() and t.device == out.device for t in (out, gt, g_percep, g_gan) if t is not None):
+        raise ValueError("gan_out_grad: out, gt and the loss gradients must be contiguous tensors on one device")
+    dout = torch.empty(out.shape, dtype=dtype, device=out.device)
+    a = _lib.GanOutGradArgs(out=_ptr(out), gt=_ptr(gt), g_percep=_ptr(g_percep), g_gan=_ptr(g_gan), dout=_ptr(dout), n=out.numel(),
+                            w_pix=float(w_pix), in_dtype=_gan_dt(out), out_dtype=_gan_dt(dout))
+    nb = out.numel() * (2 * out.element_size() + 4 * sum(g is not None for g in (g_percep, g_gan)) + dout.element_size())
+    _run("vmb_gan_out_grad", out, "gan_out_grad", a, nbytes=nb)
+    return dout
+
+
+def lr_rule(base, step_gamma=1.0, step_size=0, milestones=(), milestone_gamma=1.0):
+    """one optimizer's schedule for lr_schedule: base * step_gamma ** (it // step_size) * milestone_gamma ** #{m <= it - 1}"""
+    if len(milestones) > _lib.LR_MAX_MILESTONES:
+        raise ValueError(f"lr_rule: {len(milestones)} milestones, at most {_lib.LR_MAX_MILESTONES}")
+    return _lib.LrRule(base=float(base), step_gamma=float(step_gamma), milestone_gamma=float(milestone_gamma), step_size=int(step_size),
+                       milestones=(_lib.i64 * _lib.LR_MAX_MILESTONES)(*map(int, milestones)), n_milestones=len(milestones))
+
+
+def lr_schedule(it, lr, rules):
+    """one thread on the device: it += 1 (int64, 1 element), then lr[k] = rules[k] at the new it (lr: float32, len(rules) elements)"""
+    if it.dtype != torch.int64 or lr.dtype != torch.float32 or lr.numel() < len(rules) or not 1 <= len(rules) <= 2:
+        raise ValueError("lr_schedule: it must be int64, lr float32 with one element per rule, 1 or 2 rules")
+    a = _lib.LrScheduleArgs(iter=_ptr(it), lr=_ptr(lr), rule=(_lib.LrRule * 2)(*rules), n_rules=len(rules))
+    _run("vmb_lr_schedule", it, "lr_schedule", a)
+
+
+def ema_update(ema, param, decay):
+    """ema = decay * ema + (1 - decay) * param over two float32 buffers of one size, in place"""
+    if ema.dtype != torch.float32 or param.dtype != torch.float32 or ema.numel() != param.numel():
+        raise ValueError("ema_update: ema and param must be float32 buffers of one size")
+    _run("vmb_ema_update", ema, "ema_update", _ptr(ema), _ptr(param), ema.numel(), float(decay), nbytes=12 * ema.numel())
+
+
 # ---- perceptual loss (csrc/perceptual.cu): basicsr's PerceptualLoss between the VGG convolutions; output and ground truth as one
 # 2B batch, fp32 or bf16 activations, contiguous; every reduction in a fixed order, nothing read on the host ----
 PERCEP_CRIT = {"l1": _lib.PERCEP_L1, "l2": _lib.PERCEP_L2, "fro": _lib.PERCEP_FRO}

@@ -53,14 +53,19 @@ class FlatAdam:
             o += p.numel()
 
     @torch.no_grad()
-    def step(self, grad_scale: float = 1.0, zero_grad: bool = True):
+    def step(self, grad_scale: float = 1.0, zero_grad: bool = True, lr_device: torch.Tensor | None = None):
+        """lr_device: a float32 CUDA tensor whose first element is the learning rate, read by the kernel on the device (so that a
+        captured CUDA graph follows a schedule that a kernel earlier in the stream writes); None: self.lr"""
         from . import fused_train
+        if lr_device is not None and not (lr_device.dtype == torch.float32 and lr_device.device == self.flat_param.device):
+            raise ValueError(f"FlatAdam.step: lr_device must be a float32 tensor on {self.flat_param.device}")
         fused_train.join_side_stream()  # normally already joined by the end-of-backward callback
         a = _lib.AdamArgs(param=self.flat_param.data_ptr(), grad=self.flat_grad.data_ptr(), exp_avg=self.exp_avg.data_ptr(),
                           exp_avg_sq=self.exp_avg_sq.data_ptr(), ema=self.ema.data_ptr() if self.ema is not None else None,
                           state=self.state.data_ptr(), n=self.n, lr=self.lr, beta1=self.betas[0], beta2=self.betas[1], eps=self.eps,
                           weight_decay=self.weight_decay, decoupled_weight_decay=int(self.decoupled), grad_scale=grad_scale,
-                          max_grad_norm=self.max_grad_norm, ema_decay=self.ema_decay, zero_grad=int(zero_grad))
+                          max_grad_norm=self.max_grad_norm, ema_decay=self.ema_decay, zero_grad=int(zero_grad),
+                          lr_dev=lr_device.data_ptr() if lr_device is not None else None)
         with torch.cuda.device(self.flat_param.device):
             st = C.c_void_p(torch.cuda.current_stream(self.flat_param.device).cuda_stream)
             _lib.check(_lib.lib().vmb_fused_adam(C.byref(a), st), "fused_adam")
