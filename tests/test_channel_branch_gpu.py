@@ -1,6 +1,6 @@
 """The channel-direction OSS kernels against the float64 reference of oracle/channel_ref.py, on every path the launchers pick:
-- forward: channel_branch_v2_kernel (default) and channel_branch_kernel (v1: taken when v2's shared memory does not fit, or
-  VMB_CH_V=1), each through ops.channel_branch;
+- forward: channel_branch_v2_kernel (default) and channel_branch_kernel (v1: taken when v2's shared memory does not fit), each
+  through ops.channel_branch;
 - backward: channel_branch_bwd_kernel through ops.channel_branch_bwd, where ops.channel_branch_bwd_supported says it fits;
 - end to end: fused_train.channel_gate, which runs the two kernels (the _Channel Function) where the backward fits and torch autograd
   over SS2D_1.cforward_pooled (the flat scan) above that.
@@ -18,8 +18,7 @@ all-zero result and a parameter gradient missing its largest single image's cont
 
 Which path a case takes is derived from mirrors of the launchers' shared-memory formulas (fwd_v2 / bwd_kernel below), and asserted:
 the backward mirror against ops.channel_branch_bwd_supported and the library's vmb_channel_branch_bwd_smem_bytes; the forward mirror
-by the default output being bitwise equal to the VMB_CH_V=1 output exactly where the mirror says v1 runs (and differing somewhere
-where it says v2 runs, at C >= 32).  With 227 KB of shared memory per block the mirrors give:
+against the kernel a torch.profiler trace names.  With 227 KB of shared memory per block the mirrors give:
   forward v2:        sisr / mamber32 C <= 255, mamber33 C <= 383, realsr C <= 384   (v1 above, up to C = 593 / 665 / 451)
   backward kernel:   sisr / mamber32 C <= 245, mamber33 C <= 370, realsr C <= 377   (the torch fallback above)
 (realsr at ssm_ratio 1 and N = 16, Rc = ceil(C / 16); a smaller rank or N moves its limits up.)
@@ -34,6 +33,7 @@ import pytest
 import torch
 
 from oracle import channel_ref as cr
+from tests.test_enhance_gpu import kernel_census, kernel_names
 from vmambair_b200 import _lib, fused_train, ops
 
 pytestmark = pytest.mark.gpu
@@ -200,27 +200,15 @@ def test_bound_resolves(case):
 
 # ----------------------------------------------------------------------------- forward
 @pytest.mark.parametrize("case", CASES, ids=IDS)
-def test_channel_branch_forward(case, monkeypatch):
-    """ops.channel_branch on the default path and with VMB_CH_V=1, each against float64; the path the mirror predicts"""
+def test_channel_branch_forward_on_mirrored_kernel(case):
+    """ops.channel_branch against float64; the kernel a profiler trace names is the one the shared-memory mirror fwd_v2 predicts
+    (v1 runs only where v2 does not fit)"""
     C, L = case[1], case[6]
     a, prm, pooled, _, c_ref, _, _ = setup(case)
-    monkeypatch.delenv("VMB_CH_V", raising=False)
-    c_def = ops.channel_branch(pooled, 1.0 / L, prm, C)
-    monkeypatch.setenv("VMB_CH_V", "1")
-    c_v1 = ops.channel_branch(pooled, 1.0 / L, prm, C)
+    census, c = kernel_census(lambda: ops.channel_branch(pooled, 1.0 / L, prm, C))
     v2 = fwd_v2(C, *dims(prm))
-    check(c_def, c_ref, "c (default path)", "forward v2" if v2 else "forward v1", "c")
-    check(c_v1, c_ref, "c (VMB_CH_V=1)", "forward v1", "c")
-    # the two kernels differ only in the order of the 16-state sum of h C.  With dt ~ 1e-3 that sum is ~1e-3 of D u and its rounding
-    # can vanish in y, so the path is also probed with Dsc = 0, where y is that sum alone
-    probe = dict(prm, Dsc=torch.zeros_like(prm["Dsc"]))
-    p_v1 = ops.channel_branch(pooled, 1.0 / L, probe, C)
-    monkeypatch.delenv("VMB_CH_V")
-    p_def = ops.channel_branch(pooled, 1.0 / L, probe, C)
-    if not v2:
-        assert torch.equal(c_def, c_v1) and torch.equal(p_def, p_v1), "the mirror says v1 runs by default, but the default output is not v1's"
-    elif C >= 32:
-        assert not torch.equal(p_def, p_v1), "the mirror says v2 runs by default, but the default output is v1's bit for bit"
+    assert kernel_names(census) == {"channel_branch_v2_kernel" if v2 else "channel_branch_kernel": 1}, census
+    check(c, c_ref, "c", "forward v2" if v2 else "forward v1", "c")
 
 
 # ----------------------------------------------------------------------------- backward kernel

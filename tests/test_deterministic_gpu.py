@@ -200,7 +200,7 @@ def test_flat_values_vs_oracle_and_reference_kernels(det_flag, monkeypatch):
         for name in ["a", "b", "c", "d", "e"]:
             tsg.test_bwd_golden_vectors(os.path.join(ROOT, "tests", "golden"), name)
         for dt in tso.DT16:
-            tso.test_bwd_fp32_dout("tma", dt, (True, True, True), monkeypatch)
+            tso.test_bwd_fp32_dout("tma", dt, (True, True, True))
             tso.test_bwd_fp32_dout_generic_shapes(dt)
         for b in (8, 4, 1):
             for it in (torch.float32, torch.bfloat16):

@@ -284,9 +284,36 @@ def test_sizes_not_multiple_of_8_equal_the_composed_path(weights, shape, pre_pad
     assert ok, stats
 
 
+def kernel_census(fn):
+    """(the kernels fn launches, as a Counter of their names in a torch.profiler trace, without copies and memsets; fn's result).
+    The kernel records of a session's first milliseconds can be lost (a census once missed the first kernel of each session:
+    image_to_planes of enhance(), conv_first of the net; sessions of a few short kernels lost all of them), so the session opens with
+    a spin of about 0.1 s, fn runs twice, and only the kernels after a marker kernel between the two runs are counted; the result is
+    the second run's."""
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        torch.cuda._sleep(200_000_000)  # the lead-in: spin_kernel, 2e8 cycles
+        torch.cuda.synchronize()
+        for run in range(2):
+            out = fn()
+            torch.cuda.synchronize()
+            if run == 0:
+                torch.cuda._sleep(1000)  # the marker: spin_kernel
+                torch.cuda.synchronize()
+    ev = sorted((e for e in prof.events() if e.device_type.name == "CUDA"), key=lambda e: e.time_range.start)
+    marks = [i for i, e in enumerate(ev) if "spin_kernel" in e.name]  # the lead-in (if it was recorded), then the marker
+    assert marks, [e.name for e in ev]
+    return collections.Counter(e.name for e in ev[marks[-1] + 1:] if "emcpy" not in e.name and "emset" not in e.name), out
+
+
+def kernel_names(census):
+    """the bare function names in a census: "void vmb::scan_fwd_kernel<float, 2>(vmb::ScanFwdParams)" -> "scan_fwd_kernel" """
+    bare = lambda n: n.replace("(anonymous namespace)::", "").split("<")[0].split("(")[0].split(" ")[-1].split("::")[-1]
+    return collections.Counter(bare(n) for n in census.elements())
+
+
 def test_launch_census(ref, weights):
     """between the input and the output only the library's image kernels and the network run: no torch pad / permute / cast / copy"""
-    from torch.profiler import ProfilerActivity, profile
     name = "rgb8"
     up, _, _ = _upsampler(ref, weights, name)
     x = torch.from_numpy(ref[f"{name}/img"]).to(DEV)
@@ -295,24 +322,8 @@ def test_launch_census(ref, weights):
     up.enhance(x)
     up.runner(planes)
     torch.cuda.synchronize()
-
-    def kernels(fn):
-        # the kernel records of the first launches after the profiler starts can be lost (a census once missed the first kernel of
-        # each session: image_to_planes of enhance(), conv_first of the net), so fn runs twice in one session and only the kernels
-        # after a marker kernel between the two runs are counted
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            for run in range(2):
-                fn()
-                torch.cuda.synchronize()
-                if run == 0:
-                    torch.cuda._sleep(1000)  # the marker: spin_kernel
-                    torch.cuda.synchronize()
-        ev = sorted((e for e in prof.events() if e.device_type.name == "CUDA"), key=lambda e: e.time_range.start)
-        marks = [i for i, e in enumerate(ev) if "spin_kernel" in e.name]
-        assert len(marks) == 1, [e.name for e in ev]
-        return collections.Counter(e.name for e in ev[marks[0] + 1:] if "emcpy" not in e.name and "emset" not in e.name)
-    full = kernels(lambda: up.enhance(x))
-    net = kernels(lambda: up.runner(planes))
+    full, _ = kernel_census(lambda: up.enhance(x))
+    net, _ = kernel_census(lambda: up.runner(planes))
     extra = full - net
     assert sorted(extra) == sorted(k for k in extra if "image_to_planes_kernel" in k or "planes_to_image_kernel" in k), extra
     assert sum(extra.values()) == 2 and not (net - full), (extra, net - full)

@@ -3,6 +3,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from tests.test_pixlin_conv3x3_gpu import pixlin_path
+
 pytestmark = pytest.mark.gpu
 torch.backends.cudnn.allow_tf32 = False
 torch.backends.cuda.matmul.allow_tf32 = False
@@ -40,10 +42,12 @@ def test_pixlin_plain(dtype, K, M, P):
 
 
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
-@pytest.mark.parametrize("K,M,P,B", [(510, 96, 4096, 4), (512, 96, 1024, 2), (1021, 200, 64, 3), (400, 48, 520, 1), (510, 96, 72, 2)])
-def test_pixlin_kstream_path(dtype, K, M, P, B, monkeypatch):
-    """reduction-heavy plain GEMMs (K > 384: the EFFN / x_proj data gradients of the training path) run the K-streamed kernel:
-    against the fp32 contraction and against the resident-K kernel (VMB_PL_KSTREAM=0), bias / SiLU range / residual, strided views"""
+@pytest.mark.parametrize("K,M,P,B", [(510, 96, 4096, 4), (512, 96, 1024, 2), (1021, 200, 64, 3), (400, 48, 520, 1), (510, 96, 72, 2),
+                                     (510, 320, 1024, 2), (1021, 264, 72, 3)])
+def test_pixlin_kstream_path(dtype, K, M, P, B):
+    """reduction-heavy plain GEMMs (K > 384: the EFFN / x_proj data gradients of the training path) run the K-streamed kernel up to
+    M = 256 output rows in the input dtype; more rows or an fp32 output keep the resident-K kernel, which walks K in 384-row chunks.
+    Each against the fp32 contraction, bias / SiLU range / residual, strided views; the launcher's mirror names the kernel of each."""
     from vmambair_b200 import ops
     torch.manual_seed(K + M)
     big = torch.randn(B, K + 8, P, device="cuda").to(dtype)
@@ -52,18 +56,17 @@ def test_pixlin_kstream_path(dtype, K, M, P, B, monkeypatch):
     bias = torch.randn(M, device="cuda")
     res = torch.randn(B, M, P, device="cuda").to(dtype)
     ref = torch.einsum("mk,bkp->bmp", w[:, :K].float(), x.float())
-    outs = {}
-    for ks in ("1", "0"):
-        monkeypatch.setenv("VMB_PL_KSTREAM", ks)
-        o_plain = ops.pixlin(x, w)
-        o_full = ops.pixlin(x, w, bias, residual=res, act=(0, M // 2))
-        outs[ks] = (o_plain, o_full)
-    close(outs["1"][0], ref, dtype)
+    o_plain = ops.pixlin(x, w)
+    o_full = ops.pixlin(x, w, bias, residual=res, act=(0, M // 2))
+    o_f32 = ops.pixlin(x, w, bias, residual=res, act=(0, M // 2), out_dtype=torch.float32)
+    assert (pixlin_path(B, K, M, P, dtype, dtype, False, True, True) == {"kstream"}) == (M <= 256)
+    assert "mma-chunked-vecW" in pixlin_path(B, K, M, P, dtype, torch.float32, False, True, True)  # fp32 out: always resident-K
+    close(o_plain, ref, dtype)
     r2 = ref + bias.view(1, -1, 1)
     r2 = torch.cat([F.silu(r2[:, :M // 2]), r2[:, M // 2:]], 1) + res.float()
-    close(outs["1"][1], r2, dtype, scale=2.0)
-    # same accumulation precision as the resident-K kernel: equal up to the summation order
-    assert (outs["1"][0].float() - outs["0"][0].float()).abs().max() <= 2e-2 * ref.abs().max()
+    close(o_full, r2, dtype, scale=2.0)
+    assert o_f32.dtype == torch.float32
+    close(o_f32, r2, dtype, scale=2.0)
 
 
 @pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16])
@@ -179,12 +182,15 @@ def test_merge_norm_gate(dtype, C, H, W):
 
 
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
-@pytest.mark.parametrize("C,H,W,B", [(96, 64, 64, 3), (48, 32, 16, 2), (96, 16, 48, 1), (50, 16, 16, 2), (130, 32, 32, 1)])
+@pytest.mark.parametrize("C,H,W,B", [(96, 64, 64, 3), (48, 32, 16, 2), (96, 16, 48, 1), (50, 16, 16, 2), (130, 32, 32, 1),
+                                     (96, 128, 128, 2), (50, 128, 160, 1), (48, 256, 128, 1), (130, 128, 128, 1)])
 @pytest.mark.parametrize("inplace", [False, True])
-def test_merge_single_kernel_path(dtype, C, H, W, B, inplace, monkeypatch):
-    """H, W multiples of 16 and C <= 146: ONE kernel (16 x 16 pixel tiles, all channels per CTA, cp.async ring over the channels).
-    Against the fp32 composition, against the two-kernel path (VMB_MERGE_FUSED=0), both direction layouts, SiLU inside or outside,
-    and the workspace handed to the backward (merged fp32 values + per-pixel sum / sum of squares)."""
+def test_merge_single_kernel_path(dtype, C, H, W, B, inplace):
+    """H, W multiples of 16, C <= 96 and at least 128 x 128 pixels per image: ONE kernel (16 x 16 pixel tiles, all channels per CTA,
+    cp.async ring over the channels); other shapes: the two-kernel path.  Against the fp32
+    composition, both direction layouts, SiLU inside or outside, and the workspace handed to the backward: the merged fp32 values
+    bit for bit on either path (both sum in the composition's order), the per-pixel sum / sum of squares within the fp32 error of
+    a sum over the channels."""
     from vmambair_b200 import ops
     torch.manual_seed(C + H)
     L = H * W
@@ -199,24 +205,19 @@ def test_merge_single_kernel_path(dtype, C, H, W, B, inplace, monkeypatch):
     else:
         y = ((f[:, 0] + f[:, 2].flip(-1)) + T(f[:, 1])) + T(f[:, 3].flip(-1))
     yn = ln_ref(y, lw, lb).to(dtype).float()
-    out = {}
-    for fused in ("1", "0"):
-        monkeypatch.setenv("VMB_MERGE_FUSED", fused)
-        y2a, pa = ops.merge_norm_gate(ys, z, lw, lb, C, H, W, in_place_order=inplace)
-        y2b, pb, ws = ops.merge_norm_gate(ys, z, lw, lb, C, H, W, in_place_order=inplace, z_preact=True, return_ws=True)
-        out[fused] = (y2a, pa, y2b, pb, ws.view(torch.float32)[:B * C * L + 2 * B * L].clone())
-    y2a, pa, y2b, pb, ws = out["1"]
+    y2a, pa = ops.merge_norm_gate(ys, z, lw, lb, C, H, W, in_place_order=inplace)
+    y2b, pb, ws = ops.merge_norm_gate(ys, z, lw, lb, C, H, W, in_place_order=inplace, z_preact=True, return_ws=True)
     close(y2a, yn * z.float(), dtype, scale=2.0)
     close(y2b, yn * F.silu(z.float()), dtype, scale=2.0)
     torch.testing.assert_close(pa, y2a.float().sum(-1), rtol=2e-3, atol=2e-2)
     torch.testing.assert_close(pb, y2b.float().sum(-1), rtol=2e-3, atol=2e-2)
-    # the merged fp32 values are bit-identical to the two-kernel path (same summation order); the statistics differ by their own
-    # summation order over the channels only
-    assert torch.equal(ws[:B * C * L], out["0"][4][:B * C * L])
-    torch.testing.assert_close(ws[:B * C * L].view(B, C, L), y, rtol=0, atol=0)
-    torch.testing.assert_close(ws[B * C * L:], out["0"][4][B * C * L:], rtol=1e-5, atol=1e-4)
-    # outputs of the two paths: equal except where the last bit of the statistics moved a rounding boundary
-    assert (y2a.float() - out["0"][0].float()).abs().max() <= 2e-2 * y2a.float().abs().max()
+    ws = ws.view(torch.float32)
+    assert torch.equal(ws[:B * C * L].view(B, C, L), y)
+    # statistics (B, L, 2): any order of C fp32 additions (and one rounding per square) is within (C + 1) u of the sum of |terms|
+    y64 = y.double()
+    stats_ref = torch.stack([y64.sum(1), y64.square().sum(1)], -1)
+    bound = (C + 1) * 2.0 ** -24 * torch.stack([y64.abs().sum(1), y64.square().sum(1)], -1)
+    assert bool(((ws[B * C * L:B * C * L + 2 * B * L].view(B, L, 2).double() - stats_ref).abs() <= bound).all())
 
 
 @pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16])
@@ -307,24 +308,6 @@ def test_sr_tail_channels_last_matches_plain_tail():
         b = net.tail(feat)
     assert a.shape == b.shape and a.is_contiguous()
     torch.testing.assert_close(a, b, rtol=1e-4, atol=1e-5)
-
-
-@pytest.mark.parametrize("variant,dim", [("sisr", 96), ("mamber33", 48), ("realsr", 64), ("mamber32", 40)])
-def test_channel_branch_versions_agree(variant, dim, monkeypatch):
-    """the channel-direction OSS: restructured kernel (v2, default) against the first version, all model variants"""
-    from vmambair_b200 import archs, fused, ops
-    torch.manual_seed(dim)
-    blk = archs.MamberBlock(dim=dim, num_heads=1, ffn_expansion_factor=2.66, bias=False, LayerNorm_type="WithBias", variant=variant).cuda()
-    with torch.no_grad():
-        for p_ in blk.parameters():
-            p_.add_(0.05 * torch.randn_like(p_))
-    c = fused._prepare(blk, torch.float32, torch.device("cuda"))
-    pooled = torch.randn(5, dim, device="cuda") * 40.0
-    monkeypatch.setenv("VMB_CH_V", "1")
-    v1 = ops.channel_branch(pooled, 1.0 / 64, c["ch"], dim)
-    monkeypatch.setenv("VMB_CH_V", "2")
-    v2 = ops.channel_branch(pooled, 1.0 / 64, c["ch"], dim)
-    torch.testing.assert_close(v2, v1, rtol=1e-4, atol=1e-5)
 
 
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float32])

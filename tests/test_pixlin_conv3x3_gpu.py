@@ -15,7 +15,6 @@ allowance rather than slack: the final round-to-nearest of a 16-bit output uses 
 float64 values round to neighbouring 16-bit values differs by exactly the T of that element.  The fp32 accumulation term is the
 slack: the fp32 paths, which have neither, use 0.07 - 0.14 of it on the H100.
 """
-import os
 import zlib
 from collections import namedtuple
 
@@ -120,8 +119,7 @@ def pixlin_path(B, K, M, P, dtype, out_dtype, pro, vec_ok, w_vec):
     kpad = ceil16(K)
     if dtype == F32:
         return {"f32-resident" if kpad <= PL_KC_F32 else "f32-chunked"}
-    env = os.environ.get("VMB_PL_KSTREAM")
-    if (env is None or int(env) != 0) and out_dtype == dtype and not pro and vec_ok and w_vec and K > PL2_KC and M <= 2 * KS_MT:
+    if out_dtype == dtype and not pro and vec_ok and w_vec and K > PL2_KC and M <= 2 * KS_MT:
         return {"kstream"}
     n = sms()
     big = cdiv(P, 128) * B >= n and pixlin_smem(K, 2, 128, 2) <= 100 * 1024

@@ -1,8 +1,8 @@
 """fp32 output from 16-bit inputs (`selective_scan_cuda_oflex`) and the state-dimension-1 layout (`selective_scan_cuda_ndstate`).
 
 Every case is checked against the float64 oracle (oracle.cscan) on the same dtype-rounded inputs, on both forward paths (TMA
-kernel, generic kernel) and both backward paths (TMA kernel; generic kernel with VMB_SCAN_BWD_TMA=0).  Each case asserts the
-launcher's path condition, so a layout cannot drift onto the other path unnoticed.
+kernel, generic kernel) and both backward paths (TMA kernel; generic kernel).  Each case asserts the launcher's path condition,
+so a layout cannot drift onto the other path unnoticed.
 
 fp32 accuracy is shown, not assumed: the forward bound is test_scan_gpu.py's fp32 bound (its relative term capped at a quarter of
 the 16-bit unit roundoff, which only tightens it for fp16), and the test asserts that one 16-bit rounding of `out` breaks it.  The backward's fp32-level bound is set by the fp32 operator on the same values (16-bit inputs
@@ -183,6 +183,11 @@ def run_bwd(g, dout, softplus):
     return grads
 
 
+def _misaligned(t):
+    """a copy of t one element into its storage"""
+    return torch.empty(t.numel() + 1, dtype=t.dtype, device=t.device)[1:].view(t.shape).copy_(t)
+
+
 def max_err(got, ref):
     return (got.double().cpu() - ref).abs().max().item()
 
@@ -190,22 +195,25 @@ def max_err(got, ref):
 @pytest.mark.parametrize("path", ["tma", "generic"])
 @pytest.mark.parametrize("flags", [(True, True, True), (False, False, False), (True, True, False)])
 @pytest.mark.parametrize("dtype", DT16)
-def test_bwd_fp32_dout(path, dtype, flags, monkeypatch):
+def test_bwd_fp32_dout(path, dtype, flags):
     has_D, has_bias, softplus = flags
     b, D, L, N, G = 2, 64, 1024, 16, 2
     ins = make_inputs(b, D, L, N, G, dtype, seed=101, has_D=has_D, has_bias=has_bias)
     dout = torch.randn(b, D, L, generator=torch.Generator().manual_seed(102))  # fp32
-    if path == "generic":
-        monkeypatch.setenv("VMB_SCAN_BWD_TMA", "0")
+    # generic: every dout one element into its storage, so its rows are not 16 B aligned (vec_ok false), on a layout that otherwise
+    # takes the TMA kernel
+    place = _misaligned if path == "generic" else (lambda t: t)
     g = cuda(ins)
-    assert bwd_takes_tma(g[0], N, G)  # the layout takes the TMA kernel unless the switch turns it off
-    ours = run_bwd(g, dout.cuda(), softplus)
+    assert bwd_takes_tma(g[0], N, G)
+    d = place(dout.cuda())
+    assert (d.data_ptr() % 16 != 0) == (path == "generic")
+    ours = run_bwd(g, d, softplus)
     ref = cscan.scan_bwd(*ins, dout, softplus)
     # the fp32 operator on the same values (16-bit inputs are exact in fp32): the fp32-level error of these gradients
     g32 = cuda([None if t is None else t.float() for t in ins])
-    f32 = run_bwd(g32, dout.cuda(), softplus)
+    f32 = run_bwd(g32, place(dout.cuda()), softplus)
     # the same 16-bit operator with dout rounded to 16 bits first
-    pre = run_bwd(g, dout.to(dtype).cuda(), softplus)
+    pre = run_bwd(g, place(dout.to(dtype).cuda()), softplus)
     for i, n in enumerate(GRAD_NAMES):
         if ref[i] is None:
             assert ours[i] is None and pre[i] is None, n

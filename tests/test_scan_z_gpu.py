@@ -1,6 +1,6 @@
 """The `selective_scan_cuda` stand-in (z-gated forward, pair-layout checkpoints with the last state, gate backward) and the
 autograd entry `mamba_selective_scan_fn`, against the float64 oracle composed with the gate (test_scan_z_cpu.py), on both forward
-paths (TMA kernel; generic kernel with VMB_SCAN_TMA=0)."""
+paths (TMA kernel; generic kernel for an L < 512 or a u that is not 16 B aligned)."""
 import ctypes as C
 
 import pytest
@@ -68,10 +68,15 @@ def close(x, ref, rtol, atol, what, floor=0.0):
     assert bool(ok.all()), f"{what}: {int((~ok).sum())} / {ok.numel()} beyond rtol {rtol} atol {atol}; max err {(x - ref).abs().max():.3e}"
 
 
-def run_fn(g, softplus, dout):
-    """mamba_selective_scan_fn forward (return_last_state=True) + backward -> (out, state, grads in GRADS order)"""
+def run_fn(g, softplus, dout, misalign=False):
+    """mamba_selective_scan_fn forward (return_last_state=True) + backward -> (out, state, grads in GRADS order).
+    misalign: u one element into its storage, so that its rows are not 16 B aligned"""
     from vmambair_b200.selective_scan import mamba_selective_scan_fn
-    u, delta, A, Bm, Cm, Dv, z, bias = [None if t is None else t.detach().clone().requires_grad_() for t in g]
+    ts = [None if t is None else t.detach().clone() for t in g]
+    if misalign:  # vmb_selective_scan_fwd / _bwd: no 16 B rows (vec_ok false), so neither TMA kernel takes the call
+        ts[0] = torch.empty(ts[0].numel() + 1, dtype=ts[0].dtype, device=ts[0].device)[1:].view(ts[0].shape).copy_(ts[0])
+        assert ts[0].data_ptr() % 16 != 0
+    u, delta, A, Bm, Cm, Dv, z, bias = [None if t is None else t.requires_grad_() for t in ts]
     out, state = mamba_selective_scan_fn(u, delta, A, Bm, Cm, Dv, z=z, delta_bias=bias, delta_softplus=softplus, return_last_state=True)
     out.backward(dout.cuda())
     grads = [t.grad if t is not None else None for t in (u, delta, A, Bm, Cm, z, Dv, bias)]
@@ -87,15 +92,13 @@ def run_fn(g, softplus, dout):
 @pytest.mark.parametrize("has_D", [False, True])
 @pytest.mark.parametrize("dtype", DTYPES)
 @pytest.mark.parametrize("has_z", [False, True])
-def test_reference_parametrization(has_z, dtype, has_D, has_bias, softplus, groups, L, path, monkeypatch):
+def test_reference_parametrization(has_z, dtype, has_D, has_bias, softplus, groups, L, path):
     if path == "tma" and L < 512:
         pytest.skip("L < 512 runs the generic forward only")
-    if path == "generic":
-        monkeypatch.setenv("VMB_SCAN_TMA", "0")
     b, D, N = 2, 64, 16
     ins = make_inputs(b, D, L, N, groups, dtype, seed=L + 7 * groups, has_D=has_D, has_bias=has_bias, has_z=has_z)
     dout = torch.randn(b, D, L, generator=torch.Generator().manual_seed(5)).to(dtype)
-    out, state, grads = run_fn(cuda(ins), softplus, dout)
+    out, state, grads = run_fn(cuda(ins), softplus, dout, misalign=path == "generic")
     ref, rgrads, last = oracle(ins, dout, softplus)
     rtol, atol, rtolw, atolw = tolerances(dtype, has_z)
     assert out.dtype == dtype and state.dtype == torch.float32 and tuple(state.shape) == (b, D, N)

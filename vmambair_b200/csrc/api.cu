@@ -8,13 +8,6 @@
 #include "oss_params.h"
 
 namespace vmb {
-bool pdl_enabled() {
-    static const bool on = [] {
-        const char* e = getenv("VMB_PDL");
-        return e ? atoi(e) != 0 : true;
-    }();
-    return on;
-}
 int num_sms() {
     static const int n = [] {
         int dev = 0, v = 0;
@@ -163,7 +156,7 @@ extern "C" int vmb_selective_scan_bwd(const vmb_scan_bwd_args* a, void* stream) 
 extern "C" int64_t vmb_scan_bwd_det_workspace_bytes(const vmb_scan_bwd_args* a) {
     ScanBwdParams p;
     if (scan_bwd_params(a, p) != VMB_OK) return -1;
-    return scan_bwd_det_workspace(p, a->dtype);
+    return scan_bwd_det_workspace(p);
 }
 
 static inline bool dt_ok(int d) { return d == VMB_F32 || d == VMB_BF16 || d == VMB_F16; }

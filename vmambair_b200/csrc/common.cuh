@@ -37,8 +37,7 @@ void set_error(const char* fmt, ...);
 // (and no global store) may precede the wait.  Both are no-ops for a kernel launched without the attribute.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-bool pdl_enabled();  // VMB_PDL (default 1), read once
-int num_sms();       // SMs of the current device, read once (launch heuristics size their grids by it)
+int num_sms();  // SMs of the current device, read once (launch heuristics size their grids by it)
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
     cudaLaunchConfig_t cfg = {};
@@ -50,7 +49,7 @@ inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, siz
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 1 : 0;
+    cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
 

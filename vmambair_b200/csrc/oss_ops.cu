@@ -851,17 +851,13 @@ __global__ void __launch_bounds__(512) merge_fused_kernel(const MergeParams p, f
 
 // the workspace regions of the fused kernel sit behind the fp32 merged values and the statistics
 static bool merge_fused_applicable(const MergeParams& p, int dtype) {
-    int mode = 2;  // VMB_MERGE_FUSED: 0 never, 1 whenever legal (tests), default: from 128 x 128 pixels per image up
-    if (const char* e = getenv("VMB_MERGE_FUSED")) mode = atoi(e);
-    if (mode == 0) return false;
     auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
     const bool legal = (dtype == VMB_BF16 || dtype == VMB_F16) && p.H % 16 == 0 && p.W % 16 == 0 && p.C <= 16 * MF_MAXPW &&
                        merge_fused_smem(p.C) <= 200 * 1024 && al16(p.ys) && al16(p.z) && al16(p.y2) && p.z_bs % 8 == 0 && p.z_cs % 8 == 0;
-    if (!legal || mode == 1) return legal;
-    // the normalisation kernel of the two-kernel path walks all pixels of a channel in one CTA, which dominates at large images; a
-    // CTA of the single kernel walks all channel groups of its tile at any size, which dominates at small ones (tools/merge_bench.py
-    // times both)
-    return (long)p.H * p.W >= 16384;
+    // from 128 x 128 pixels per image up: the normalisation kernel of the two-kernel path walks all pixels of a channel in one CTA,
+    // which dominates at large images; a CTA of the single kernel walks all channel groups of its tile at any size, which dominates
+    // at small ones.  On the H100 the crossover lies between 32 x 32 and 64 x 64 (DESIGN §1.4: timings, and why it is kept here)
+    return legal && (long)p.H * p.W >= 16384;
 }
 
 int merge_launch(const MergeParams& p, int dtype, cudaStream_t stream) {
@@ -1212,10 +1208,8 @@ int channel_launch(const ChannelParams& p, cudaStream_t stream) {
     const int RN = p.Rc + 2 * p.N;
     const size_t base = sizeof(float) * ((size_t)p.dc * p.C + 2 * RN * (p.C | 1) + 4 * p.dc * p.C + p.C + 64 + 2 * RN * p.dc +
                                          2 * p.dc * p.Rc + 2 * p.dc + 3 * p.dc + 1);
-    const char* ve = getenv("VMB_CH_V");
-    const int version = ve ? atoi(ve) : 2;
     const size_t smem2 = base + sizeof(float) * (size_t)2 * p.dc * 16 * (p.C | 1);
-    if (version == 2 && 2 * p.dc * 16 <= CH2_THREADS && smem2 <= 227 * 1024) {
+    if (2 * p.dc * 16 <= CH2_THREADS && smem2 <= 227 * 1024) {
         if (smem2 > 48 * 1024)
             VMB_CUDA(cudaFuncSetAttribute(channel_branch_v2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
         VMB_CUDA(launch_pdl(channel_branch_v2_kernel, dim3(p.B), dim3(CH2_THREADS), smem2, stream, p));

@@ -676,9 +676,6 @@ static int launch_kstream(const PixlinParams& p, cudaStream_t stream) {
 }
 
 static bool kstream_applicable(const PixlinParams& p, int dtype, int out_dtype) {
-    if (const char* e = getenv("VMB_PL_KSTREAM")) {
-        if (atoi(e) == 0) return false;
-    }
     return (dtype == VMB_BF16 || dtype == VMB_F16) && out_dtype == dtype && p.ln_mode == 0 && p.gate_mode == 0 && p.vec_ok && p.w_vec &&
            p.K > PL2_KC && p.M <= 2 * KS_MT;
 }

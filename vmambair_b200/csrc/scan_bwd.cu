@@ -296,7 +296,7 @@ __global__ void __launch_bounds__(32, 8) scan_bwd_kernel(const ScanBwdParams p) 
                     if constexpr (DET) {
                         if (l < L && n0 < N) scratch[(int64_t)(n0 / 2) * L + l] = acc;
                     } else {
-                        if (l < L && n0 < N && !p.debug_nored) red_add_f32x4(scratch + (int64_t)(n0 / 2) * L + l, acc);
+                        if (l < L && n0 < N) red_add_f32x4(scratch + (int64_t)(n0 / 2) * L + l, acc);
                     }
                 }
                 __syncwarp();
@@ -483,15 +483,13 @@ template <> struct DtOf<__nv_bfloat16> { static constexpr int v = VMB_BF16; };
 template <> struct DtOf<__half> { static constexpr int v = VMB_F16; };
 
 template <typename in_t, typename g_t = in_t>
-static int launch_t(const ScanBwdParams& p_in, cudaStream_t stream) {
+static int launch_t(const ScanBwdParams& p, cudaStream_t stream) {
     constexpr bool dout_f32 = !std::is_same<g_t, in_t>::value;
-    ScanBwdParams p = p_in;
-    if (const char* e = getenv("VMB_BWD_NORED")) p.debug_nored = atoi(e);
     const size_t scratch_bytes = sizeof(float4) * (size_t)p.batch * p.G * (p.npad / 2) * p.L;
     VMB_CUDA(cudaMemsetAsync(p.dBC, 0, scratch_bytes, stream));
     int rc;
     int trb, tss;
-    if (scan_bwd_tma_pick(p, DtOf<in_t>::v, trb, tss)) {  // fast path: TMA-staged 4-warp CTAs (scan_bwd_tma.cu)
+    if (scan_bwd_tma_pick(p, trb, tss)) {  // fast path: TMA-staged 4-warp CTAs (scan_bwd_tma.cu)
         rc = scan_bwd_tma_launch(p, DtOf<in_t>::v, trb, tss, stream, dout_f32);
     } else
     switch (pick_rb_bwd(p)) {
@@ -510,16 +508,16 @@ static int launch_t(const ScanBwdParams& p_in, cudaStream_t stream) {
 }
 
 // deterministic mode: contributors of one (batch, group) -- the CTAs (TMA path) or warps (generic path) that share it
-static int det_contributors(const ScanBwdParams& p, int dtype, int& trb, int& tss, int& rb) {
-    if (scan_bwd_tma_pick(p, dtype, trb, tss)) return p.rows_per_group / (trb * 4 / tss);
+static int det_contributors(const ScanBwdParams& p, int& trb, int& tss, int& rb) {
+    if (scan_bwd_tma_pick(p, trb, tss)) return p.rows_per_group / (trb * 4 / tss);
     trb = 0;
     rb = pick_rb_bwd(p);
     return p.rows_per_group / rb;
 }
 
-int64_t scan_bwd_det_workspace(const ScanBwdParams& p, int dtype) {
+int64_t scan_bwd_det_workspace(const ScanBwdParams& p) {
     int trb, tss, rb;
-    return scan_bwd_det_bytes(p, det_contributors(p, dtype, trb, tss, rb));
+    return scan_bwd_det_bytes(p, det_contributors(p, trb, tss, rb));
 }
 
 template <typename in_t, typename g_t = in_t>
@@ -527,7 +525,7 @@ static int launch_det_t(const ScanBwdParams& p_in, cudaStream_t stream) {
     constexpr bool dout_f32 = !std::is_same<g_t, in_t>::value;
     ScanBwdParams p = p_in;
     int trb, tss, rb = 1;
-    const ScanBwdDetFin f = scan_bwd_det_carve(p, det_contributors(p, DtOf<in_t>::v, trb, tss, rb));
+    const ScanBwdDetFin f = scan_bwd_det_carve(p, det_contributors(p, trb, tss, rb));
     int rc;
     if (trb) {
         rc = scan_bwd_tma_launch(p, DtOf<in_t>::v, trb, tss, stream, dout_f32, true);

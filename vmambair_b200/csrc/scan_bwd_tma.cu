@@ -372,7 +372,7 @@ __global__ void __launch_bounds__(128, sizeof(in_t) == 4 ? 1 : 2)
             if (GW > 1) {
                 // dB/dC: the GW warps of the CTA that work on this pair set (different rows of the same group) meet, then each sums
                 // the RB * GW rows of its share of the cells: ONE vector reduction per (pair, position, CTA) instead of one per warp
-                // (the global reductions were 19-25 % of the kernel, tools/scan_bwd_nored.py)
+                // (the global reductions were 19-25 % of the kernel, DESIGN §1.2)
                 named_bar_sync<1 + (SS > 1 ? GW : 0)>(SS > 1 ? sp : 0, 32 * GW);
                 constexpr int CPW = K::CELLS / GW;
 #pragma unroll
@@ -393,7 +393,7 @@ __global__ void __launch_bounds__(128, sizeof(in_t) == 4 ? 1 : 2)
                     }
                     acc = make_float4(acc_b.x, acc_b.y, acc_c.x, acc_c.y);
                     const int l = c0 + cell;
-                    if (l < L && n0 < N && (DET || !p.debug_nored)) put_bc<DET>(scratch + (int64_t)np * L + l, acc);
+                    if (l < L && n0 < N) put_bc<DET>(scratch + (int64_t)np * L + l, acc);
                 }
             } else {
                 // dB/dC: sum the RB rows of each (segment, position) cell, one vector reduction per cell
@@ -407,7 +407,7 @@ __global__ void __launch_bounds__(128, sizeof(in_t) == 4 ? 1 : 2)
                         acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
                     }
                     const int l = c0 + cell;
-                    if (l < L && n0 < N && (DET || !p.debug_nored)) put_bc<DET>(scratch + (int64_t)np * L + l, acc);
+                    if (l < L && n0 < N) put_bc<DET>(scratch + (int64_t)np * L + l, acc);
                 }
                 __syncwarp();
             }
@@ -536,10 +536,7 @@ static int bwd_tma_ss(const ScanBwdParams& p, int rb) {
 
 // (rows per warp, state split): RB = 2 at every batch; the state split while the CTAs still fit one resident wave
 // (DESIGN §1.2)
-bool scan_bwd_tma_pick(const ScanBwdParams& p, int dtype, int& rb, int& ss) {
-    const char* e = getenv("VMB_SCAN_BWD_TMA");
-    if (e && atoi(e) == 0) return false;
-    if (dtype == VMB_F32 && getenv("VMB_SCAN_BWD_TMA_F32") && atoi(getenv("VMB_SCAN_BWD_TMA_F32")) == 0) return false;
+bool scan_bwd_tma_pick(const ScanBwdParams& p, int& rb, int& ss) {
     if (!p.vec_ok || p.npad != 16 || p.L < 512 || p.ckpt == nullptr) return false;
     rb = 2;
     ss = bwd_tma_ss(p, rb);

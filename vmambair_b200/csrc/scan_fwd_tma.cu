@@ -425,8 +425,6 @@ static int launch_tma1(const ScanFwdParams& p, const ScanTmaMaps& maps, int ss, 
 
 // (rows per warp, state split) for the TMA kernel; false when the shape is left to the generic kernel.
 bool scan_fwd_tma_pick(const ScanFwdParams& p, int& rb, int& ss) {
-    const char* e = getenv("VMB_SCAN_TMA");
-    if (e && atoi(e) == 0) return false;
     if (!p.vec_ok || p.npad != 16 || p.L < 512) return false;
     if (p.ndesc && p.N != 16) return false;  // grouped sources: the B/C boxes are 16 rows of a wider tensor
     const int rpg = p.rows_per_group;

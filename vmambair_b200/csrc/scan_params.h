@@ -76,7 +76,6 @@ struct ScanBwdParams {
     int64_t B_bs, B_gs, B_ns, C_bs, C_gs, C_ns;
     int softplus;
     bool vec_ok;
-    int debug_nored;  // profiling only (VMB_BWD_NORED=1): skip the dB/dC global reductions
 };
 
 // Grouped backward (vmb_selective_scan_bwd_grouped): G = ndesc <= 4 group descriptors; strides are the ScanBwdParams ones, shared by
@@ -121,7 +120,7 @@ inline ScanBwdDetFin scan_bwd_det_carve(ScanBwdParams& p, int nc) {
 }
 // gr: NULL for the flat operator, else the grouped destinations (each group's dB / dC in its memory order)
 int scan_bwd_det_finalize(const ScanBwdDetFin& f, const ScanBwdGroups* gr, int dtype, cudaStream_t stream);
-int64_t scan_bwd_det_workspace(const ScanBwdParams& p, int dtype);
+int64_t scan_bwd_det_workspace(const ScanBwdParams& p);
 int64_t scan_bwd_grouped_det_workspace(const ScanBwdParams& p);
 
 // out_f32 / dout_f32 (16-bit dtype only): `out` / `dout` are fp32 (selective_scan_cuda_oflex).  They are launcher arguments, not
@@ -133,7 +132,7 @@ int scan_fwd_tma_launch(const ScanFwdParams& p, int dtype, int rb, int ss, cudaS
 // elementwise backward of the z gate (vmb_scan_gate_bwd)
 int scan_gate_bwd_launch(const vmb_scan_gate_args& a, bool vec_ok, cudaStream_t stream);
 int scan_bwd_launch(const ScanBwdParams& p, int dtype, cudaStream_t stream, bool dout_f32 = false, bool det = false);
-bool scan_bwd_tma_pick(const ScanBwdParams& p, int dtype, int& rb, int& ss);
+bool scan_bwd_tma_pick(const ScanBwdParams& p, int& rb, int& ss);
 int scan_bwd_tma_launch(const ScanBwdParams& p, int dtype, int rb, int ss, cudaStream_t stream, bool dout_f32 = false, bool det = false);
 int scan_bwd_grouped_launch(const ScanBwdParams& p, const ScanBwdGroups& gr, int dtype, cudaStream_t stream, bool det = false);
 
