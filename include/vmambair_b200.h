@@ -889,13 +889,24 @@ int vmb_gan_out_grad(const vmb_gan_out_grad_args* a, void* stream);
 /* Learning-rate schedule of one optimizer at iteration `it`:
  * lr = base step_gamma^(it / step_size) milestone_gamma^(number of milestones <= it - 1).
  * The first factor is MambaRealSRGAN's generator decay (lr_sr, gamma_sr, lr_decay_sr; step_size <= 0: none), the second basicsr's
- * MultiStepLR, which has stepped it - 1 times when iteration `it` runs.  All in double (Python's float), the result rounded to fp32. */
+ * MultiStepLR, which has stepped it - 1 times when iteration `it` runs.  All in double (Python's float), the result rounded to fp32.
+ * n_periods > 0 replaces that formula by basicsr's cosine annealing with restarts (Deraining/basicsr/models/lr_scheduler.py:115-235,
+ * CosineAnnealingRestartCyclicLR; CosineAnnealingRestartLR is the case of equal eta_mins) at e = it - 1:
+ * with j the first period whose cumulative end c_j >= e, and c_{-1} = 0,
+ * lr = eta_mins[j] + restart_weights[j] 0.5 (base - eta_mins[j]) (1 + cos(pi (e - c_{j-1}) / periods[j])),
+ * evaluated in Python's order without contraction and rounded once to fp32.  Past the last period the reference has no lr (its
+ * get_position_from_periods returns None): the kernel writes NaN there, and the caller is expected to stop before. */
 #define VMB_LR_MAX_MILESTONES 8
+#define VMB_LR_MAX_PERIODS 8
 typedef struct {
     double base, step_gamma, milestone_gamma;
     int64_t step_size;
     int64_t milestones[VMB_LR_MAX_MILESTONES];
     int n_milestones;
+    int n_periods;
+    int64_t periods[VMB_LR_MAX_PERIODS];
+    double restart_weights[VMB_LR_MAX_PERIODS];
+    double eta_mins[VMB_LR_MAX_PERIODS];
 } vmb_lr_rule;
 /* One thread: *iter += 1, then lr[k] = rule[k] at the new *iter for k < n_rules (at most 2: generator, discriminator). */
 typedef struct {
@@ -905,6 +916,33 @@ typedef struct {
     int n_rules;
 } vmb_lr_schedule_args;
 int vmb_lr_schedule(const vmb_lr_schedule_args* a, void* stream);
+
+/* The restoration step's input preparation (vmambair_b200.restore_train): Restormer's progressive subset and crop
+ * (Deraining/basicsr/train.py:245-262) and ImageCleanModel's mixup (Deraining/basicsr/models/image_restoration_model.py:22-49),
+ * for lq and gt in one launch.  For each tensor t < n_tensors, image i < batch, channel, and (y, x) in its h x w window:
+ *   s(k)    = src[idx[k], channel, row0 + y, col0 + x]            (any strides, in elements)
+ *   dst[i]  = lam s(i) + one_minus_lam s(perm[i])                 when mix != 0: two fp32 products and one fp32 sum, as torch
+ *                                                                 evaluates lam * t + (1 - lam) * t[perm] with Python-float scalars
+ *   dst[i]  = s(i)                                                when mix == 0 (a pure gather)
+ * dst is contiguous (batch, c, h, w).  fp32 only.  The host makes every draw; indices and window origins travel here. */
+#define VMB_CROP_MIX_MAX_IMAGES 64
+typedef struct {
+    const float* src;
+    float* dst;
+    int64_t stride_n, stride_c, stride_h, stride_w;
+    int c, h, w;
+    int row0, col0;
+} vmb_crop_mix_tensor;
+typedef struct {
+    vmb_crop_mix_tensor t[2];
+    int n_tensors;
+    int batch;
+    int idx[VMB_CROP_MIX_MAX_IMAGES];
+    int perm[VMB_CROP_MIX_MAX_IMAGES];
+    float lam, one_minus_lam;
+    int mix;
+} vmb_batch_crop_mix_args;
+int vmb_batch_crop_mix(const vmb_batch_crop_mix_args* a, void* stream);
 
 /* ema = decay ema + (1 - decay) param over n fp32 elements: vmb_fused_adam's EMA alone, for iterations that skip the optimizer
  * step but not basicsr's model_ema(). */

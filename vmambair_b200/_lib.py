@@ -405,17 +405,35 @@ class GanOutGradArgs(C.Structure):
 
 
 LR_MAX_MILESTONES = 8  # VMB_LR_MAX_MILESTONES
+LR_MAX_PERIODS = 8  # VMB_LR_MAX_PERIODS
 
 
 class LrRule(C.Structure):
     _c_name_ = "vmb_lr_rule"
     _fields_ = [("base", C.c_double), ("step_gamma", C.c_double), ("milestone_gamma", C.c_double), ("step_size", i64),
-                ("milestones", i64 * LR_MAX_MILESTONES), ("n_milestones", C.c_int)]
+                ("milestones", i64 * LR_MAX_MILESTONES), ("n_milestones", C.c_int), ("n_periods", C.c_int),
+                ("periods", i64 * LR_MAX_PERIODS), ("restart_weights", C.c_double * LR_MAX_PERIODS),
+                ("eta_mins", C.c_double * LR_MAX_PERIODS)]
 
 
 class LrScheduleArgs(C.Structure):
     _c_name_ = "vmb_lr_schedule_args"
     _fields_ = [("iter", vp), ("lr", vp), ("rule", LrRule * 2), ("n_rules", C.c_int)]
+
+
+CROP_MIX_MAX_IMAGES = 64  # VMB_CROP_MIX_MAX_IMAGES
+
+
+class CropMixTensor(C.Structure):
+    _c_name_ = "vmb_crop_mix_tensor"
+    _fields_ = [("src", vp), ("dst", vp), ("stride_n", i64), ("stride_c", i64), ("stride_h", i64), ("stride_w", i64),
+                ("c", C.c_int), ("h", C.c_int), ("w", C.c_int), ("row0", C.c_int), ("col0", C.c_int)]
+
+
+class BatchCropMixArgs(C.Structure):
+    _c_name_ = "vmb_batch_crop_mix_args"
+    _fields_ = [("t", CropMixTensor * 2), ("n_tensors", C.c_int), ("batch", C.c_int), ("idx", C.c_int * CROP_MIX_MAX_IMAGES),
+                ("perm", C.c_int * CROP_MIX_MAX_IMAGES), ("lam", C.c_float), ("one_minus_lam", C.c_float), ("mix", C.c_int)]
 
 
 PERCEP_L1, PERCEP_L2, PERCEP_FRO = 0, 1, 2  # VMB_PERCEP_L1 / _L2 / _FRO
@@ -570,6 +588,7 @@ SYMBOLS = {
     "vmb_gan_out_grad": (C.c_int, [C.POINTER(GanOutGradArgs), vp]),
     "vmb_lr_schedule": (C.c_int, [C.POINTER(LrScheduleArgs), vp]),
     "vmb_ema_update": (C.c_int, [vp, vp, C.c_int64, C.c_float, vp]),
+    "vmb_batch_crop_mix": (C.c_int, [C.POINTER(BatchCropMixArgs), vp]),
     "vmb_percep_norm": (C.c_int, [C.POINTER(PercepNormArgs), vp]),
     "vmb_percep_norm_bwd": (C.c_int, [C.POINTER(PercepNormBwdArgs), vp]),
     "vmb_percep_stage": (C.c_int, [C.POINTER(PercepStageArgs), vp]),

@@ -1,8 +1,9 @@
 // The GAN training step's own kernels (vmambair_b200.gan_train): the pixel loss and the logit means as a two-level sum, the
 // generator's output-gradient junction of its three losses, the learning-rate schedule of both optimizers from the device's
-// iteration counter, and the EMA for iterations that skip the generator's optimizer step.  Every reduction has one fixed order
-// (the grid depends on n alone) and there are no atomics, so the results are bitwise repeatable; all math is fp32, tensors are fp32
-// or bf16 (VMB_F32 / VMB_BF16).  Nothing reads the host, so the step can be captured in a CUDA graph.
+// iteration counter (step decay and MultiStepLR, or cosine annealing with restarts for vmambair_b200.restore_train), and the EMA
+// for iterations that skip the generator's optimizer step.  Every reduction has one fixed order (the grid depends on n alone) and
+// there are no atomics, so the results are bitwise repeatable; all math is fp32, tensors are fp32 or bf16 (VMB_F32 / VMB_BF16).
+// Nothing reads the host, so the step can be captured in a CUDA graph.
 #include <math.h>
 
 #include "common.cuh"
@@ -90,7 +91,24 @@ int out_grad_launch(const vmb_gan_out_grad_args& a, dim3 grid, cudaStream_t s) {
 }
 
 // ---- learning-rate schedule ----
+// basicsr's cosine annealing with restarts at last_epoch e (lr_scheduler.py:115-235), in Python's order of evaluation: no
+// contraction into fma, so the double result is the host's up to cos()'s last bit
+__device__ float cosine_lr(const vmb_lr_rule& r, int64_t e) {
+    int64_t start = 0;
+    for (int j = 0; j < r.n_periods; ++j) {
+        if (e <= start + r.periods[j]) {
+            const double eta = r.eta_mins[j];
+            const double t = __ddiv_rn((double)(e - start), (double)r.periods[j]);
+            const double c = __dadd_rn(1.0, cos(__dmul_rn(M_PI, t)));
+            return (float)__dadd_rn(eta, __dmul_rn(__dmul_rn(__dmul_rn(r.restart_weights[j], 0.5), __dadd_rn(r.base, -eta)), c));
+        }
+        start += r.periods[j];
+    }
+    return __int_as_float(0x7fc00000);  // past the last period: the reference has no lr
+}
+
 __device__ float rule_lr(const vmb_lr_rule& r, int64_t it) {
+    if (r.n_periods > 0) return cosine_lr(r, it - 1);
     double lr = r.base;
     if (r.step_size > 0) lr *= pow(r.step_gamma, (double)(it / r.step_size));
     int passed = 0;
@@ -158,6 +176,12 @@ extern "C" int vmb_lr_schedule(const vmb_lr_schedule_args* a, void* stream) {
         VMB_CHECK(a->rule[k].base >= 0.f && a->rule[k].n_milestones >= 0 && a->rule[k].n_milestones <= VMB_LR_MAX_MILESTONES,
                   "lr_schedule: rule %d has base %g and %d milestones (at most %d)", k, a->rule[k].base,
                   a->rule[k].n_milestones, VMB_LR_MAX_MILESTONES);
+    for (int k = 0; k < a->n_rules; ++k) {
+        VMB_CHECK(a->rule[k].n_periods >= 0 && a->rule[k].n_periods <= VMB_LR_MAX_PERIODS, "lr_schedule: rule %d has %d periods (at most %d)",
+                  k, a->rule[k].n_periods, VMB_LR_MAX_PERIODS);
+        for (int j = 0; j < a->rule[k].n_periods; ++j)
+            VMB_CHECK(a->rule[k].periods[j] >= 1, "lr_schedule: rule %d period %d is %lld", k, j, (long long)a->rule[k].periods[j]);
+    }
     VMB_CUDA(launch_pdl(lr_schedule_kernel, dim3(1), dim3(1), 0, static_cast<cudaStream_t>(stream), *a));
     VMB_CUDA(cudaGetLastError());
     return VMB_OK;

@@ -40,14 +40,21 @@ _MODELS = ("MambaRealSRGAN", "MambaSISRGANModel")
 class LrRule:
     """lr at iteration it = base * step_gamma ** (it // step_size) * milestone_gamma ** #{m in milestones : m <= it - 1}; the first
     factor is MambaRealSRGAN's generator decay (step_size 0: none), the second basicsr's MultiStepLR, stepped it - 1 times when
-    iteration it runs (update_learning_rate steps from the second iteration on).  `at` is what the schedule kernel computes."""
+    iteration it runs (update_learning_rate steps from the second iteration on).  With `periods`, the rule is instead basicsr's
+    CosineAnnealingRestartCyclicLR (Deraining/basicsr/models/lr_scheduler.py:115-235) at last_epoch it - 1, one restart weight
+    and eta_min per period (equal eta_mins: CosineAnnealingRestartLR).  `at` is what the schedule kernel computes."""
     base: float
     step_gamma: float = 1.0
     step_size: int = 0
     milestones: tuple = ()
     milestone_gamma: float = 1.0
+    periods: tuple = ()
+    restart_weights: tuple = ()
+    eta_mins: tuple = ()
 
     def at(self, it: int) -> float:
+        if self.periods:
+            return self._cosine(it - 1)
         lr = float(self.base)
         if self.step_size > 0:
             lr *= math.pow(self.step_gamma, it // self.step_size)
@@ -56,8 +63,18 @@ class LrRule:
             lr *= math.pow(self.milestone_gamma, passed)
         return lr
 
+    def _cosine(self, e):
+        start = 0
+        for period, weight, eta_min in zip(self.periods, self.restart_weights, self.eta_mins):
+            if e <= start + period:  # get_position_from_periods: the first cumulative period >= e
+                return eta_min + weight * 0.5 * (self.base - eta_min) * (1 + math.cos(math.pi * ((e - start) / period)))
+            start += period
+        raise ValueError(f"iteration {e + 1}: the cosine schedule's periods {list(self.periods)} end at iteration {start + 1}, and "
+                         "the reference scheduler has no learning rate after them")
+
     def c_rule(self):
-        return ops.lr_rule(self.base, self.step_gamma, self.step_size, self.milestones, self.milestone_gamma)
+        return ops.lr_rule(self.base, self.step_gamma, self.step_size, self.milestones, self.milestone_gamma, self.periods,
+                           self.restart_weights, self.eta_mins)
 
 
 @dataclass

@@ -1205,12 +1205,22 @@ def gan_out_grad(out, gt, g_percep, g_gan, w_pix, dtype):
     return dout
 
 
-def lr_rule(base, step_gamma=1.0, step_size=0, milestones=(), milestone_gamma=1.0):
-    """one optimizer's schedule for lr_schedule: base * step_gamma ** (it // step_size) * milestone_gamma ** #{m <= it - 1}"""
+def lr_rule(base, step_gamma=1.0, step_size=0, milestones=(), milestone_gamma=1.0, periods=(), restart_weights=(), eta_mins=()):
+    """one optimizer's schedule for lr_schedule: base * step_gamma ** (it // step_size) * milestone_gamma ** #{m <= it - 1}; or, when
+    `periods` is given, basicsr's cosine annealing with restarts at last_epoch it - 1 (one restart weight and eta_min per period;
+    CosineAnnealingRestartLR is the case of equal eta_mins), which the step decay and milestones cannot be combined with"""
     if len(milestones) > _lib.LR_MAX_MILESTONES:
         raise ValueError(f"lr_rule: {len(milestones)} milestones, at most {_lib.LR_MAX_MILESTONES}")
+    if not len(periods) == len(restart_weights) == len(eta_mins) <= _lib.LR_MAX_PERIODS or any(int(p) < 1 for p in periods):
+        raise ValueError(f"lr_rule: periods {tuple(periods)}, restart_weights {tuple(restart_weights)} and eta_mins {tuple(eta_mins)} "
+                         f"must have one length, at most {_lib.LR_MAX_PERIODS}, and positive periods")
+    if periods and (milestones or step_size > 0):
+        raise ValueError("lr_rule: a cosine schedule takes no step decay or milestones")
+    n = _lib.LR_MAX_PERIODS
     return _lib.LrRule(base=float(base), step_gamma=float(step_gamma), milestone_gamma=float(milestone_gamma), step_size=int(step_size),
-                       milestones=(_lib.i64 * _lib.LR_MAX_MILESTONES)(*map(int, milestones)), n_milestones=len(milestones))
+                       milestones=(_lib.i64 * _lib.LR_MAX_MILESTONES)(*map(int, milestones)), n_milestones=len(milestones),
+                       n_periods=len(periods), periods=(_lib.i64 * n)(*map(int, periods)),
+                       restart_weights=(C.c_double * n)(*map(float, restart_weights)), eta_mins=(C.c_double * n)(*map(float, eta_mins)))
 
 
 def lr_schedule(it, lr, rules):
@@ -1226,6 +1236,49 @@ def ema_update(ema, param, decay):
     if ema.dtype != torch.float32 or param.dtype != torch.float32 or ema.numel() != param.numel():
         raise ValueError("ema_update: ema and param must be float32 buffers of one size")
     _run("vmb_ema_update", ema, "ema_update", _ptr(ema), _ptr(param), ema.numel(), float(decay), nbytes=12 * ema.numel())
+
+
+# ---- restoration step's input preparation (csrc/restore_step.cu): progressive subset / crop and mixup of lq and gt ----
+def batch_crop_mix(lq, gt, idx, row0, col0, size, scale, lam=None, perm=None, out=None):
+    """lq[idx][:, :, row0:row0 + size, col0:col0 + size] and gt's window at scale x those coordinates, mixed when lam is given:
+    out[i] = lam * s[i] + (1 - lam) * s[perm[i]], rounded as torch evaluates that expression with Python-float lam (fp32 products of
+    lam and of float32(1 - lam), one fp32 sum), else a pure gather.  lq, gt: float32 CUDA tensors (B, C, H, W) on one device, any
+    strides; size None: the whole of lq.  idx: up to 64 source images (repeats allowed); perm: a permutation of range(len(idx)).
+    out: (lq_out, gt_out), contiguous float32 tensors of the result's shapes to write into (e.g. a CUDA graph's inputs).
+    -> (lq_out, gt_out)"""
+    if any(t.dim() != 4 or t.dtype != torch.float32 or not t.is_cuda or t.device != lq.device for t in (lq, gt)):
+        raise ValueError("batch_crop_mix: lq and gt must be 4-d float32 CUDA tensors on one device")
+    B, scale = lq.shape[0], int(scale)
+    idx = [int(i) for i in idx]
+    k = len(idx)
+    size = (lq.shape[2], lq.shape[3]) if size is None else (int(size), int(size))
+    if gt.shape[0] != B or not 1 <= k <= _lib.CROP_MIX_MAX_IMAGES or not all(0 <= i < B for i in idx):
+        raise ValueError(f"batch_crop_mix: {k} indices {idx} into batches of {B} and {gt.shape[0]} images "
+                         f"(1 to {_lib.CROP_MIX_MAX_IMAGES})")
+    if scale < 1 or row0 < 0 or col0 < 0 or min(size) < 1 or row0 + size[0] > lq.shape[2] or col0 + size[1] > lq.shape[3] or \
+            scale * (row0 + size[0]) > gt.shape[2] or scale * (col0 + size[1]) > gt.shape[3]:
+        raise ValueError(f"batch_crop_mix: window {size} at ({row0}, {col0}), scale {scale}, leaves lq {tuple(lq.shape)} or "
+                         f"gt {tuple(gt.shape)}")
+    perm = list(range(k)) if perm is None else [int(p) for p in perm]
+    if sorted(perm) != list(range(k)):
+        raise ValueError(f"batch_crop_mix: perm {perm} is not a permutation of range({k})")
+    shapes = [(k, lq.shape[1], *size), (k, gt.shape[1], scale * size[0], scale * size[1])]
+    if out is None:
+        out = tuple(torch.empty(sh, dtype=torch.float32, device=lq.device) for sh in shapes)
+    if any(tuple(o.shape) != sh or o.dtype != torch.float32 or not o.is_contiguous() or o.device != lq.device
+           for o, sh in zip(out, shapes)):
+        raise ValueError(f"batch_crop_mix: out must be contiguous float32 tensors of shapes {shapes} on {lq.device}")
+
+    def tensor(src, dst, s):
+        return _lib.CropMixTensor(src=_ptr(src), dst=_ptr(dst), stride_n=src.stride(0), stride_c=src.stride(1), stride_h=src.stride(2),
+                                  stride_w=src.stride(3), c=dst.shape[1], h=dst.shape[2], w=dst.shape[3], row0=s * row0, col0=s * col0)
+
+    n = _lib.CROP_MIX_MAX_IMAGES
+    a = _lib.BatchCropMixArgs(t=(_lib.CropMixTensor * 2)(tensor(lq, out[0], 1), tensor(gt, out[1], scale)), n_tensors=2, batch=k,
+                              idx=(C.c_int * n)(*idx), perm=(C.c_int * n)(*perm), lam=1.0 if lam is None else float(lam),
+                              one_minus_lam=0.0 if lam is None else 1.0 - float(lam), mix=int(lam is not None))
+    _run("vmb_batch_crop_mix", lq, "batch_crop_mix", a, nbytes=4 * sum(o.numel() for o in out) * (3 if lam is not None else 2))
+    return out
 
 
 # ---- perceptual loss (csrc/perceptual.cu): basicsr's PerceptualLoss between the VGG convolutions; output and ground truth as one
