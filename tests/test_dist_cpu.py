@@ -22,14 +22,16 @@ def _worker(rank, world, port, q):
     dist.init_process_group("gloo", rank=rank, world_size=world)
     torch.manual_seed(rank)  # different init per rank on purpose
     m = torch.nn.Sequential(torch.nn.Linear(4, 3), torch.nn.Linear(3, 2))
+    v0 = [p._version for p in m.parameters()]
     broadcast_params(m)
+    bumped = [p._version > v for p, v in zip(m.parameters(), v0)]
     gar = FlatGradAllReduce(m.parameters()).attach()
     data = torch.arange(8 * 4, dtype=torch.float32).view(8, 4) / 10
     lo, hi = shard_batch(8, rank, world)
     gar.zero()
     m(data[lo:hi]).square().sum().backward()
     gar.reduce(world)
-    q.put((rank, [p.detach().clone() for p in m.parameters()], gar.flat.clone(), (lo, hi)))
+    q.put((rank, [p.detach().clone() for p in m.parameters()], gar.flat.clone(), (lo, hi), bumped))
     dist.barrier()
     dist.destroy_process_group()
 
@@ -64,6 +66,9 @@ def test_two_rank_flat_allreduce_matches_single_process():
     # replicas identical after broadcast, reduced gradients identical on both ranks
     for a, b in zip(res[0][1], res[1][1]):
         assert torch.equal(a, b)
+    # the broadcast writes through p.data, which has its own version counter: broadcast_params bumps each parameter's, on every
+    # rank, so weight caches keyed on _version (the inference path's) rebuild from the broadcast values
+    assert all(res[0][4]) and all(res[1][4]), (res[0][4], res[1][4])
     assert torch.equal(res[0][2], res[1][2])
     # equals the mean over ranks of the per-shard gradients computed in one process
     m = torch.nn.Sequential(torch.nn.Linear(4, 3), torch.nn.Linear(3, 2))

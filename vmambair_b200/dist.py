@@ -55,7 +55,9 @@ class FlatGradAllReduce:
 
 
 def broadcast_params(module: torch.nn.Module, src: int = 0):
-    """identical replicas at start (DDP does this at construction)."""
+    """identical replicas at start (DDP does this at construction).  The broadcast writes through p.data, whose version counter is
+    not p's, so each parameter's version is bumped after it: the inference weight caches key on it."""
     if dist.is_initialized() and dist.get_world_size() > 1:
         for p in module.parameters():
             dist.broadcast(p.data, src)
+            torch.autograd.graph.increment_version(p)

@@ -258,6 +258,8 @@ class GANTrainer:
             self._lq.copy_(lq, non_blocking=True)
             self._gt.copy_(gt, non_blocking=True)
             self.graph.replay()
+            for o in (self.opt_g, self.opt_d):  # the replayed Adam kernels run no Python: announce their writes to the inference caches
+                o.mark_written()
             return self._losses
         return self._iteration(lq, gt, g_on)
 
@@ -275,6 +277,8 @@ class GANTrainer:
         with torch.no_grad():
             for t, s in zip(self._state(), snap[0]):
                 t.copy_(s)
+        for o in (self.opt_g, self.opt_d):
+            o.mark_written()
         self.iter = snap[1]
 
     def capture(self, lq, gt):

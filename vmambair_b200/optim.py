@@ -69,6 +69,13 @@ class FlatAdam:
         with torch.cuda.device(self.flat_param.device):
             st = C.c_void_p(torch.cuda.current_stream(self.flat_param.device).cuda_stream)
             _lib.check(_lib.lib().vmb_fused_adam(C.byref(a), st), "fused_adam")
+        self.mark_written()
+
+    def mark_written(self):
+        """bump every parameter's version counter after a write behind autograd's back (the kernel above, a CUDA-graph replay of
+        it, a copy into flat_param): the inference weight caches (fused._prepare, unet._cached, the SR tail's channels-last copy)
+        key on _version and data_ptr, and neither changes when the flat buffer is written through its pointer or a view of it"""
+        torch.autograd.graph.increment_version(self.params)
 
     def ema_state_dict(self, module: torch.nn.Module):
         """EMA weights under the module's parameter names (the reference's net_g_ema / `params_ema` checkpoint entry)"""

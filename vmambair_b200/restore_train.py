@@ -234,6 +234,7 @@ class RestorationTrainer:
                                  out=(self._lq, self._gt) if replay else None)
         if replay:
             self.graph.replay()
+            self.opt_g.mark_written()  # the replayed Adam kernel runs no Python: announce its write to the inference caches
             return self._losses
         return self._iteration(*inp)
 
@@ -246,6 +247,7 @@ class RestorationTrainer:
         with torch.no_grad():
             for t, s in zip(self._state(), snap):
                 t.copy_(s)
+        self.opt_g.mark_written()
 
     def capture(self, lq, gt):
         """record the iteration of the next step's phase, on batches of that phase's shapes, as one CUDA graph (releasing the graph
